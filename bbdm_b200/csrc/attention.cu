@@ -5,7 +5,11 @@
 // qkv conv runs on the fp32 direct kernel (unaligned channel counts).  The template UNets
 // (head_dim 64) use the warp-specialised wgmma kernel in attention_tc.cu.
 //
-// CTA = 4 warps x 16 query rows = 64 queries of one (batch, head); KV tiles of 64 keys.
+// CTA = 4 warps x 16 query rows = 64 queries of one (batch, head); KV tiles of 64 keys.  The K and V^T
+// tiles live in static shared memory for head_dim <= 64; at 128 they take 71.7 KB, over the 48 KB static
+// limit, so that instance stages them in dynamic shared memory with the same layout.  At 128 the Q fragments
+// (64 registers) are also parked there, in fragment order (each thread reads back only its own 16-byte words),
+// and the S product runs k-step outer, n-tile inner: the same products in the same order per S entry.
 #include "common.cuh"
 
 namespace bbdm {
@@ -19,17 +23,18 @@ __device__ __forceinline__ void mma_bf16_16816(float* d, const uint32_t* a, uint
 
 __device__ __forceinline__ void split2(float x, float y, uint32_t& hi, uint32_t& lo) { split2x(x, y, hi, lo); }
 
+constexpr int ATT_KT = 64;          // keys per tile
+constexpr int ATT_LDV = ATT_KT + 8;   // padded V^T row (bf16 elements)
+
 template <int D>
-__global__ void __launch_bounds__(128)
-attention_kernel(const float* __restrict__ qkv, int T, int C, int heads, int order, float scale,
-                 float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_hi,
-                 __nv_bfloat16* __restrict__ out_lo) {
-  constexpr int KT = 64;            // keys per tile
+__device__ __forceinline__ void attention_body(const float* __restrict__ qkv, int T, int C, int heads, int order, float scale,
+                                               float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_hi,
+                                               __nv_bfloat16* __restrict__ out_lo,
+                                               __nv_bfloat16 (&Kh)[ATT_KT][D + 8], __nv_bfloat16 (&Kl)[ATT_KT][D + 8],
+                                               __nv_bfloat16 (&Vh)[D][ATT_LDV], __nv_bfloat16 (&Vl)[D][ATT_LDV],
+                                               uint4* __restrict__ qfrag) {     // D > 64: [KS][hi, lo][128 threads]
+  constexpr int KT = ATT_KT;        // keys per tile
   constexpr int KS = D / 16;        // k-steps over head_dim
-  constexpr int LDK = D + 8;        // padded row (bf16 elements)
-  constexpr int LDV = KT + 8;
-  __shared__ __align__(16) __nv_bfloat16 Kh[KT][LDK], Kl[KT][LDK];
-  __shared__ __align__(16) __nv_bfloat16 Vh[D][LDV], Vl[D][LDV];
 
   const int bh = blockIdx.y;
   const int b = bh / heads, head = bh % heads;
@@ -55,6 +60,13 @@ attention_kernel(const float* __restrict__ qkv, int T, int C, int heads, int ord
         if (qr < T) v = *reinterpret_cast<const float2*>(base + qr * row_stride + qoff + ks * 16 + h2 * 8 + 2 * t);
         split2(v.x * scale, v.y * scale, qh[ks][h2 * 2 + r2], ql[ks][h2 * 2 + r2]);
       }
+    }
+  }
+  if constexpr (D > 64) {
+#pragma unroll
+    for (int ks = 0; ks < KS; ++ks) {
+      qfrag[(2 * ks) * 128 + threadIdx.x] = make_uint4(qh[ks][0], qh[ks][1], qh[ks][2], qh[ks][3]);
+      qfrag[(2 * ks + 1) * 128 + threadIdx.x] = make_uint4(ql[ks][0], ql[ks][1], ql[ks][2], ql[ks][3]);
     }
   }
 
@@ -88,6 +100,25 @@ attention_kernel(const float* __restrict__ qkv, int T, int C, int heads, int ord
 
     // ---- S = Q K^T (16 x 64 per warp) -----------------------------------------------------
     float s[KT / 8][4];
+    if constexpr (D > 64) {
+#pragma unroll
+      for (int j = 0; j < KT / 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+#pragma unroll
+      for (int ks = 0; ks < KS; ++ks) {
+        const uint4 h4 = qfrag[(2 * ks) * 128 + threadIdx.x], l4 = qfrag[(2 * ks + 1) * 128 + threadIdx.x];
+        const uint32_t qh1[4] = {h4.x, h4.y, h4.z, h4.w}, ql1[4] = {l4.x, l4.y, l4.z, l4.w};
+#pragma unroll
+        for (int j = 0; j < KT / 8; ++j) {
+          const uint32_t bh0 = *reinterpret_cast<const uint32_t*>(&Kh[j * 8 + g][ks * 16 + 2 * t]);
+          const uint32_t bh1 = *reinterpret_cast<const uint32_t*>(&Kh[j * 8 + g][ks * 16 + 8 + 2 * t]);
+          const uint32_t bl0 = *reinterpret_cast<const uint32_t*>(&Kl[j * 8 + g][ks * 16 + 2 * t]);
+          const uint32_t bl1 = *reinterpret_cast<const uint32_t*>(&Kl[j * 8 + g][ks * 16 + 8 + 2 * t]);
+          mma_bf16_16816(s[j], ql1, bh0, bh1);
+          mma_bf16_16816(s[j], qh1, bl0, bl1);
+          mma_bf16_16816(s[j], qh1, bh0, bh1);
+        }
+      }
+    } else
 #pragma unroll
     for (int j = 0; j < KT / 8; ++j) {
       s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
@@ -183,6 +214,37 @@ attention_kernel(const float* __restrict__ qkv, int T, int C, int heads, int ord
   }
 }
 
+template <int D>
+__global__ void __launch_bounds__(128)
+attention_kernel(const float* __restrict__ qkv, int T, int C, int heads, int order, float scale,
+                 float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_hi,
+                 __nv_bfloat16* __restrict__ out_lo) {
+  constexpr int LDK = D + 8;        // padded row (bf16 elements)
+  __shared__ __align__(16) __nv_bfloat16 Kh[ATT_KT][LDK], Kl[ATT_KT][LDK];
+  __shared__ __align__(16) __nv_bfloat16 Vh[D][ATT_LDV], Vl[D][ATT_LDV];
+  attention_body<D>(qkv, T, C, heads, order, scale, out_f32, out_hi, out_lo, Kh, Kl, Vh, Vl, nullptr);
+}
+
+// Kh Kl Vh Vl, then the Q fragments: 2 planes x D/16 k-steps x 128 threads x 16 B
+template <int D>
+constexpr size_t attention_dyn_smem() { return (size_t)2 * (ATT_KT * (D + 8) + D * ATT_LDV) * 2 + (size_t)2 * (D / 16) * 128 * 16; }
+
+template <int D>
+__global__ void __launch_bounds__(128)
+attention_kernel_dyn(const float* __restrict__ qkv, int T, int C, int heads, int order, float scale,
+                     float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_hi,
+                     __nv_bfloat16* __restrict__ out_lo) {
+  typedef __nv_bfloat16 KTile[ATT_KT][D + 8];
+  typedef __nv_bfloat16 VTile[D][ATT_LDV];
+  extern __shared__ __align__(16) uint8_t att_smem[];     // Kh Kl Vh Vl Q-fragments, each 16-byte aligned
+  KTile& Kh = *reinterpret_cast<KTile*>(att_smem);
+  KTile& Kl = *reinterpret_cast<KTile*>(att_smem + sizeof(KTile));
+  VTile& Vh = *reinterpret_cast<VTile*>(att_smem + 2 * sizeof(KTile));
+  VTile& Vl = *reinterpret_cast<VTile*>(att_smem + 2 * sizeof(KTile) + sizeof(VTile));
+  uint4* qfrag = reinterpret_cast<uint4*>(att_smem + 2 * sizeof(KTile) + 2 * sizeof(VTile));
+  attention_body<D>(qkv, T, C, heads, order, scale, out_f32, out_hi, out_lo, Kh, Kl, Vh, Vl, qfrag);
+}
+
 }  // namespace bbdm
 
 using namespace bbdm;
@@ -204,8 +266,16 @@ extern "C" int bbdm_attention(const float* qkv, int B, int T, int C, int heads, 
   if (D == 64) attention_kernel<64><<<grid, 128, 0, s>>>(qkv, T, C, heads, order, scale, out_f32, oh, ol);
   else if (D == 32) attention_kernel<32><<<grid, 128, 0, s>>>(qkv, T, C, heads, order, scale, out_f32, oh, ol);
   else if (D == 16) attention_kernel<16><<<grid, 128, 0, s>>>(qkv, T, C, heads, order, scale, out_f32, oh, ol);
-  else {
-    set_error("attention: head_dim %d not supported (16, 32, 64)", D);
+  else if (D == 128) {
+    constexpr size_t smem = attention_dyn_smem<128>();
+    static DeviceOnce cfgd;
+    if (cfgd.need()) {
+      BBDM_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel_dyn<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      cfgd.mark();
+    }
+    attention_kernel_dyn<128><<<grid, 128, smem, s>>>(qkv, T, C, heads, order, scale, out_f32, oh, ol);
+  } else {
+    set_error("attention: head_dim %d not supported (16, 32, 64, 128)", D);
     return BBDM_E_UNSUPPORTED;
   }
   BBDM_LAUNCH_CHECK();

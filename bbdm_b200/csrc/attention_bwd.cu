@@ -341,8 +341,9 @@ extern "C" int bbdm_attention_bwd(const float* qkv, const float* out, const floa
     case 16: return launch_bwd<16>(p, B, s);
     case 32: return launch_bwd<32>(p, B, s);
     case 64: return launch_bwd<64>(p, B, s);
+    case 128: return launch_bwd<128>(p, B, s);     // kernel 2: 231,936 B of the 232,448 B opt-in shared memory
     default:
-      BBDM_REQUIRE(false, "attention_bwd: head_dim %d not supported (16, 32, 64)", D);
+      BBDM_REQUIRE(false, "attention_bwd: head_dim %d not supported (16, 32, 64, 128)", D);
   }
   return BBDM_OK;
 }

@@ -9,6 +9,9 @@
 // (K plain, V transposed); split-bf16 x3 products on mma.sync.m16n8k16 with fp32 accumulate;
 // every KV tile's P.V product starts from a zero accumulator and is added to O with a
 // round-to-nearest fp32 add (the tensor core's own accumulate truncates).
+// Q fragments stay in registers for D <= 64.  At D = 128 they would take 64 registers on top of the 64-float
+// output, so the CTA's 128 query rows are staged in shared memory once (both planes, same padded rows) and
+// each pair of k-steps is read back with ldmatrix while the S product walks the key n-tiles.
 #include "common.cuh"
 
 namespace bbdm {
@@ -60,7 +63,8 @@ attention_split_kernel(const AttnOperands ops, int T, int C, int heads, float sc
   constexpr int KS = D / 16;              // k-steps over head_dim
   constexpr int LD = D + 8;               // padded smem row (elements): 16 B skew, conflict-free ldmatrix
   constexpr int TILE = KT * LD;           // elements per plane tile
-  extern __shared__ __align__(16) __nv_bfloat16 sm[];   // [2 stages][Kh, Kl, Vh, Vl][KT][LD]
+  constexpr bool QS = D > 64;             // Q fragments from shared memory
+  extern __shared__ __align__(16) __nv_bfloat16 sm[];   // [2 stages][Kh, Kl, Vh, Vl][KT][LD] (QS: + [Qh, Ql][128][LD])
 
   const int bh = blockIdx.y;
   const int b = bh / heads, head = bh % heads;
@@ -93,7 +97,19 @@ attention_split_kernel(const AttnOperands ops, int T, int C, int heads, float sc
 
   // ---- Q fragments for this warp's 16 rows (registers, both planes) ----------------------------
   const int q0 = blockIdx.x * 128 + warp * 16;
-  uint32_t qh[KS][4], ql[KS][4];
+  uint32_t qh[QS ? 1 : KS][4], ql[QS ? 1 : KS][4];
+  if constexpr (QS) {                     // 128 rows x D/8 16-byte chunks per plane, zero-filled past Tq
+    constexpr int CPR = D / 8;
+    __nv_bfloat16* qs = sm + 2 * 4 * TILE;
+    for (int i = threadIdx.x; i < 2 * 128 * CPR; i += 256) {
+      const int plane = i / (128 * CPR), rem = i % (128 * CPR);
+      const int row = rem / CPR, ch = rem % CPR;
+      const int qr = blockIdx.x * 128 + row;
+      const bool ok = qr < Tq;
+      const __nv_bfloat16* src = (plane ? qbase_lo : qbase_hi) + (int64_t)(ok ? qr : 0) * rs_q + qoff + ch * 8;
+      cp_async16(smem_addr(qs + plane * 128 * LD + row * LD + ch * 8), src, ok ? 16 : 0);
+    }
+  } else
 #pragma unroll
   for (int ks = 0; ks < KS; ++ks)
 #pragma unroll
@@ -131,6 +147,35 @@ attention_split_kernel(const AttnOperands ops, int T, int C, int heads, float sc
 
     // ---- S = Q K^T : per 8-key n-tile j, ldmatrix.x4 covers two k-steps (b0,b1 | b0,b1) -----------
     float s[KT / 8][4];
+    if constexpr (QS) {
+      // same products in the same order per s[j]; the k-step pair is the outer loop so that only its
+      // Q fragments are live.  A fragment by ldmatrix.x4: matrix m = lane>>3 is (rows 8*(m&1).., k 8*(m>>1)..)
+      const uint32_t qh_a = smem_addr(sm + 2 * 4 * TILE), ql_a = qh_a + 128 * LD * 2;
+      const uint32_t qrow = (uint32_t)(((warp * 16 + (lane & 15)) * LD + (lane >> 4) * 8) * 2);
+#pragma unroll
+      for (int j = 0; j < KT / 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+#pragma unroll
+      for (int k2 = 0; k2 < KS / 2; ++k2) {
+        uint32_t ah0[4], al0[4], ah1[4], al1[4];
+        ldsm_x4(qh_a + qrow + k2 * 64, ah0[0], ah0[1], ah0[2], ah0[3]);
+        ldsm_x4(ql_a + qrow + k2 * 64, al0[0], al0[1], al0[2], al0[3]);
+        ldsm_x4(qh_a + qrow + k2 * 64 + 32, ah1[0], ah1[1], ah1[2], ah1[3]);
+        ldsm_x4(ql_a + qrow + k2 * 64 + 32, al1[0], al1[1], al1[2], al1[3]);
+#pragma unroll
+        for (int j = 0; j < KT / 8; ++j) {
+          const uint32_t roff = (uint32_t)(((j * 8 + (lane & 7)) * LD + (lane >> 3) * 8) * 2);
+          uint32_t h0, h1, h2, h3, l0, l1, l2, l3;
+          ldsm_x4(kh_a + roff + k2 * 64, h0, h1, h2, h3);
+          ldsm_x4(kl_a + roff + k2 * 64, l0, l1, l2, l3);
+          mma16816(s[j], al0, h0, h1);
+          mma16816(s[j], ah0, l0, l1);
+          mma16816(s[j], ah0, h0, h1);
+          mma16816(s[j], al1, h2, h3);
+          mma16816(s[j], ah1, l2, l3);
+          mma16816(s[j], ah1, h2, h3);
+        }
+      }
+    } else
 #pragma unroll
     for (int j = 0; j < KT / 8; ++j) {
       s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
@@ -258,7 +303,7 @@ static int launch_attention_split(const AttnOperands& ops, int B, int T, int C, 
   __nv_bfloat16* ol = (__nv_bfloat16*)out_lo;
 #define BBDM_AL(DD)                                                                                       \
   {                                                                                                       \
-    const size_t smem = (size_t)2 * 4 * 64 * (DD + 8) * 2;                                                \
+    const size_t smem = (size_t)2 * 4 * 64 * (DD + 8) * 2 + (DD > 64 ? (size_t)2 * 128 * (DD + 8) * 2 : 0); \
     static DeviceOnce cfgd;                                                                               \
     if (cfgd.need()) {                                                                                    \
       BBDM_CUDA_CHECK(cudaFuncSetAttribute(attention_split_kernel<DD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
@@ -267,10 +312,11 @@ static int launch_attention_split(const AttnOperands& ops, int B, int T, int C, 
     attention_split_kernel<DD><<<grid, 256, smem, s>>>(ops, T, C, heads, scale_log2, out_f32, oh, ol);   \
   }
   if (D == 64) BBDM_AL(64)
+  else if (D == 128) BBDM_AL(128)
   else if (D == 32) BBDM_AL(32)
   else if (D == 16) BBDM_AL(16)
   else {
-    set_error("attention_split: head_dim %d not supported (16, 32, 64)", D);
+    set_error("attention_split: head_dim %d not supported (16, 32, 64, 128)", D);
     return BBDM_E_UNSUPPORTED;
   }
 #undef BBDM_AL

@@ -139,6 +139,11 @@ __device__ __forceinline__ void wgmma_rs_n64_bf16(float* d, const uint32_t* a, u
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d), "n"(TB));
 }
 
+// warpgroup-wide register reallocation (all four warps of the warpgroup execute it); N: 24..256, multiple of 8
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;

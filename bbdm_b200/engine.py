@@ -25,6 +25,8 @@ from .unet import (AttentionBlock, Downsample, ResBlock, TimestepEmbedSequential
 
 GN_GROUPS = 32
 GN_EPS = 1e-5
+ATTN_HEAD_DIMS = (16, 32, 64, 128)       # head sizes the attention kernels are built for
+ATTN_TC_HEAD_DIMS = (64, 128)            # ... of which bbdm_attention_tc (wgmma) takes these
 
 
 def resample_to_res(resample):
@@ -221,7 +223,7 @@ class UNetEngine(KernelExecutor):
         self._w = {}
         self._table = None
         self.num_timesteps = 1000
-        self.attention_impl = "tcgen05"      # "mma.sync" selects bbdm_attention_split for head_dim 64 too
+        self.attention_impl = "tcgen05"      # "mma.sync" selects bbdm_attention_split for head_dim 64/128 too
         self.generation = 0          # bumps whenever cache/parameter ADDRESSES change (graphs key on it)
 
     # ------------------------------------------------------------------------------ weights
@@ -519,8 +521,8 @@ class UNetEngine(KernelExecutor):
         eq, ep = w[name + ".qkv"], w[name + ".proj_out"]
         heads = m.num_heads
         hd = Cc // heads
-        if hd not in (16, 32, 64):
-            raise NotImplementedError(f"attention head_dim {hd}: the sm_90a kernel supports 16/32/64")
+        if hd not in ATTN_HEAD_DIMS:
+            raise NotImplementedError(f"attention head_dim {hd}: the sm_90a kernels support 16/32/64/128")
         umma = self._umma_ok(Cc, Cc, W)
         mean, rstd = self._stats(pool, x, None)
         a_f32 = a_hi = a_lo = None
@@ -540,8 +542,8 @@ class UNetEngine(KernelExecutor):
         order = 1 if m.new_order else 0
         if umma:
             o_hi, o_lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
-            # head_dim 64 (all templates): warp-specialised wgmma kernel; else the mma.sync one
-            attn = be.attention_tc if (hd == 64 and self.attention_impl == "tcgen05") else be.attention_split
+            # head_dim 64 (all templates) or 128: warp-specialised wgmma kernel; else the mma.sync one
+            attn = be.attention_tc if (hd in ATTN_TC_HEAD_DIMS and self.attention_impl == "tcgen05") else be.attention_split
             attn(q_hi.view(B, T, 3 * Cc), q_lo.view(B, T, 3 * Cc), heads, order,
                  None, o_hi.view(B, T, Cc), o_lo.view(B, T, Cc))
         else:
@@ -577,8 +579,8 @@ class UNetEngine(KernelExecutor):
         B, H, W, Cc = x.shape
         T, heads, d = H * W, m.n_heads, m.d_head
         inner = heads * d
-        if d not in (16, 32, 64):
-            raise NotImplementedError(f"SpatialTransformer head_dim {d}: the sm_90a attention kernels take 16/32/64")
+        if d not in ATTN_HEAD_DIMS:
+            raise NotImplementedError(f"SpatialTransformer head_dim {d}: the sm_90a attention kernels take 16/32/64/128")
         if not (self._umma_ok(Cc, inner, W) and inner % 64 == 0):
             raise NotImplementedError("SpatialTransformer: channel counts must be multiples of 64 (tensor-core GEMMs)")
         bf = torch.bfloat16
@@ -609,7 +611,7 @@ class UNetEngine(KernelExecutor):
                                        want_f32=False)
             pool.put(n_hi, n_lo)
             o_hi, o_lo = pool.get(tok, bf), pool.get(tok, bf)
-            attn = be.attention_tc if (d == 64 and self.attention_impl == "tcgen05") else be.attention_split
+            attn = be.attention_tc if (d in ATTN_TC_HEAD_DIMS and self.attention_impl == "tcgen05") else be.attention_split
             attn(q_hi.view(B, T, 3 * inner), q_lo.view(B, T, 3 * inner), heads, 1, None, o_hi.view(B, T, inner),
                  o_lo.view(B, T, inner))
             pool.put(q_hi, q_lo)

@@ -394,7 +394,7 @@ def conv1x1(conv1d: torch.nn.Conv1d, x4: torch.Tensor, enabled: bool = True):
 class AttentionCoreFn(torch.autograd.Function):
     """softmax((q s)(k s)^T) v per head (QKVAttentionLegacy / QKVAttention, openaimodel.py:350-413) on a
     [B,3C,H,W] qkv tensor -> [B,C,H,W].  Forward: the sampling path's attention kernels (wgmma for
-    head_dim 64); backward: bbdm_attention_bwd (flash-style recompute, exact fp32) -- the T x T matrix is
+    head_dim 64 and 128); backward: bbdm_attention_bwd (flash-style recompute, exact fp32) -- the T x T matrix is
     never stored, which also replaces the reference's checkpoint() around the block (openaimodel.py:318)."""
 
     @staticmethod
@@ -405,7 +405,7 @@ class AttentionCoreFn(torch.autograd.Function):
         dev = qkv.device
         qn = _nhwc(qkv.detach()).contiguous()
         out = torch.empty((B, T, Cc), dtype=torch.float32, device=dev)
-        if Cc // heads == 64:
+        if Cc // heads in (64, 128):
             q_hi = torch.empty((B, H, W, C3), dtype=torch.bfloat16, device=dev)
             q_lo = torch.empty_like(q_hi)
             be.prep(qn, None, raw_hi=q_hi, raw_lo=q_lo)
@@ -436,7 +436,7 @@ def attention_core(qkv4: torch.Tensor, heads: int, new_order: bool, enabled: boo
     """[B,3C,H,W] -> [B,C,H,W] or None when the native kernels do not take the shape."""
     B, C3, H, W = qkv4.shape
     hd = C3 // 3 // heads
-    if not (enabled and _on_device(qkv4) and qkv4.dtype == torch.float32 and hd in (16, 32, 64) and (C3 // 3) % 4 == 0
+    if not (enabled and _on_device(qkv4) and qkv4.dtype == torch.float32 and hd in (16, 32, 64, 128) and (C3 // 3) % 4 == 0
             and B * heads <= 65535):
         return None
     return AttentionCoreFn.apply(qkv4, heads, 1 if new_order else 0)

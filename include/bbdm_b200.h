@@ -379,7 +379,7 @@ int bbdm_geglu_split(const float* u, int64_t rows, int N, float* out_f32, void* 
 
 /* Cross-attention core (CrossAttention.forward, attention.py:166-192): queries q [B,Tq,C] and keys|values
  * kv [B,Tkv,2C] (k = columns [0,C), v = [C,2C)), both as split-bf16 planes, head h = columns h*D..(h+1)*D of each;
- * out[b,i,:] = softmax_j(q_i.k_j * D^-1/2) v_j per head, flash-style (no Tq x Tkv buffer).  D in {16,32,64}. */
+ * out[b,i,:] = softmax_j(q_i.k_j * D^-1/2) v_j per head, flash-style (no Tq x Tkv buffer).  D in {16,32,64,128}. */
 int bbdm_attention_cross(const void* q_hi, const void* q_lo, const void* kv_hi, const void* kv_lo, int B, int Tq,
                          int Tkv, int C, int heads, float* out_f32, void* out_hi, void* out_lo, void* stream);
 
@@ -436,21 +436,21 @@ int bbdm_ema_multi(const void* const* params, const int64_t* numel, const int64_
  *   order 0 (QKVAttentionLegacy, openaimodel.py:350-375): [head][q|k|v][head_dim]
  *   order 1 (QKVAttention, :382-413):                      [q|k|v][head][head_dim]
  * out: fp32 [B,T,C] and/or split bf16 (A operand of the proj_out GEMM).
- * Split-bf16 tensor-core products with fp32 accumulation.  head_dim in {16,32,64}. */
+ * Split-bf16 tensor-core products with fp32 accumulation.  head_dim in {16,32,64,128}. */
 int bbdm_attention(const float* qkv, int B, int T, int C, int heads, int order,
                    float* out_f32, void* out_hi, void* out_lo, void* stream);
 
 /* Same attention core on PRE-SPLIT bf16 planes qkv_hi/qkv_lo [B,T,3C] (written by the qkv
  * conv's epilogue, BbdmConvArgs.out_hi/out_lo): no conversion or re-splitting of K/V per query
- * tile; cp.async double-buffered KV tiles, ldmatrix fragments, 128 queries per CTA. */
+ * tile; cp.async double-buffered KV tiles, ldmatrix fragments, 128 queries per CTA.  head_dim in {16,32,64,128}. */
 int bbdm_attention_split(const void* qkv_hi, const void* qkv_lo, int B, int T, int C, int heads,
                          int order, float* out_f32, void* out_hi, void* out_lo, void* stream);
 
-/* The same computation as a FlashAttention-style WARP-SPECIALISED wgmma kernel (head_dim 64):
+/* The same computation as a FlashAttention-style WARP-SPECIALISED wgmma kernel (head_dim 64 or 128):
  * TMA-staged Q / K / V tiles, S = Q K^T and O = P V on wgmma with register accumulators (V
  * consumed as an MN-major operand, P fed back from registers as the A operand), two 64-query
  * warpgroups per CTA, fp32 register accumulation of O with the
- * online-softmax rescale.  Returns BBDM_E_UNSUPPORTED for other head dims. */
+ * online-softmax rescale.  head_dim in {64,128}; returns BBDM_E_UNSUPPORTED for other head dims. */
 int bbdm_attention_tc(const void* qkv_hi, const void* qkv_lo, int B, int T, int C, int heads,
                       int order, float* out_f32, void* out_hi, void* out_lo, void* stream);
 
@@ -458,7 +458,7 @@ int bbdm_attention_tc(const void* qkv_hi, const void* qkv_lo, int B, int T, int 
  * QKVAttentionLegacy / QKVAttention, openaimodel.py:318,350-413, util.py:119-148): given qkv [B,T,3C],
  * out = attention(qkv) [B,T,C] and dout [B,T,C] (all fp32), writes dqkv [B,T,3C].  FlashAttention-style
  * recompute in exact fp32 -- no T x T tensor.  lse, delta: fp32 workspaces of B*heads*T elements each.
- * head_dim in {16,32,64}; deterministic. */
+ * head_dim in {16,32,64,128}; deterministic. */
 int bbdm_attention_bwd(const float* qkv, const float* out, const float* dout, int B, int T, int C, int heads,
                        int order, float* dqkv, float* lse, float* delta, void* stream);
 

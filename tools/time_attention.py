@@ -1,22 +1,110 @@
 #!/usr/bin/env python
-"""Time bbdm_attention_tc alone at the cfg2 shape (B=16, T=4096, C=1024, 16 heads) with CUDA events."""
-import os, sys, json, torch
+"""Time the attention kernels alone with CUDA events, per head_dim at equal FLOPs.
+
+    python tools/time_attention.py [--head-dims 64 128] [--B 16 --T 4096 --C 1024] [--out FILE]
+    python tools/time_attention.py B T C heads          # one head layout, head_dim = C / heads
+
+Default: the cfg2 middle-block shape (B=16, T=4096, C=1024) as 16 heads x 64 and as 8 heads x 128.  For each
+head_dim it times bbdm_attention_tc (split-bf16 planes in, split planes out) and bbdm_attention_bwd (exact fp32),
+alternating the variants over rounds and reporting the median.  Algorithmic FLOPs: forward 4 B T^2 C (QK^T, PV),
+backward 10 B T^2 C (the five T x T x D products of FlashAttention's backward), whatever the kernels recompute.
+One JSON line per (kernel, head_dim), each tagged with the card's name and power limit read in the same run."""
+import argparse
+import json
+import os
+import statistics
+import subprocess
+import sys
+
+import torch
+
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from bbdm_b200 import cabi
-be = cabi.CudaBackend()
-B, T, C, heads = (int(a) for a in (sys.argv[1:5] if len(sys.argv) > 4 else (16, 4096, 1024, 16)))
-q = torch.randn(B, T, 3 * C, device="cuda")
-hi = q.to(torch.bfloat16); lo = (q - hi.float()).to(torch.bfloat16)
-o_hi = torch.empty(B, T, C, dtype=torch.bfloat16, device="cuda"); o_lo = torch.empty_like(o_hi)
-for _ in range(3):
-    be.attention_tc(hi, lo, heads, 0, None, o_hi, o_lo)
-torch.cuda.synchronize()
-e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-e0.record()
-for _ in range(10):
-    be.attention_tc(hi, lo, heads, 0, None, o_hi, o_lo)
-e1.record(); torch.cuda.synchronize()
-be.check_fault()
-ms = e0.elapsed_time(e1) / 10
-fl = 4.0 * B * heads * T * T * (C // heads)
-print(json.dumps({"kernel": "attention_tc", "B": B, "T": T, "C": C, "heads": heads, "ms": ms, "algo_tflops": fl / ms / 1e9}))
+from bbdm_b200 import cabi  # noqa: E402
+
+
+def card():
+    info = {"gpu": torch.cuda.get_device_name(0)}
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, timeout=30)
+        info["power_limit_and_max_sm_clock"] = r.stdout.strip() or r.stderr.strip()
+    except (OSError, subprocess.SubprocessError) as e:
+        info["power_limit_and_max_sm_clock"] = f"unavailable: {e}"
+    return info
+
+
+def event_ms(fn, iters):
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(iters):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / iters
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("shape", type=int, nargs="*", metavar="B T C heads", help="time this one shape instead")
+    ap.add_argument("--head-dims", type=int, nargs="+", default=[64, 128])
+    ap.add_argument("--B", type=int, default=16)
+    ap.add_argument("--T", type=int, default=4096)
+    ap.add_argument("--C", type=int, default=1024)
+    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--fwd-iters", type=int, default=10)
+    ap.add_argument("--bwd-iters", type=int, default=2)
+    ap.add_argument("--out", default=None, help="also append the JSON lines to this file")
+    a = ap.parse_args()
+    if a.shape:
+        if len(a.shape) != 4 or a.shape[2] % a.shape[3]:
+            ap.error("positional form: B T C heads, with C divisible by heads")
+        a.B, a.T, a.C = a.shape[:3]
+        a.head_dims = [a.shape[2] // a.shape[3]]
+    assert torch.cuda.is_available(), "time_attention.py needs a GPU"
+    B, T, C = a.B, a.T, a.C
+    be = cabi.CudaBackend()
+    g = torch.Generator(device="cuda").manual_seed(0)
+    qkv = torch.randn(B, T, 3 * C, device="cuda", generator=g)
+    hi = qkv.to(torch.bfloat16)
+    lo = (qkv - hi.float()).to(torch.bfloat16)
+    o_hi = torch.empty(B, T, C, dtype=torch.bfloat16, device="cuda")
+    o_lo = torch.empty_like(o_hi)
+    out = torch.empty(B, T, C, device="cuda")
+    dout = torch.randn(B, T, C, device="cuda", generator=g)
+    dqkv = torch.empty_like(qkv)
+
+    runs = {}
+    for d in a.head_dims:
+        assert C % d == 0, (C, d)
+        heads = C // d
+        lse = torch.empty(B * heads * T, device="cuda")
+        delta = torch.empty_like(lse)
+        fwd = lambda h=heads: be.attention_tc(hi, lo, h, 0, None, o_hi, o_lo)
+        bwd = lambda h=heads, l=lse, dl=delta: be.attention_bwd(qkv, out, dout, h, 0, dqkv, l, dl)
+        be.attention_tc(hi, lo, heads, 0, out, None, None)      # the forward output the backward is given
+        fwd(); bwd()                                               # warm up every shape timed below
+        torch.cuda.synchronize()
+        runs[d] = (heads, fwd, bwd, {"fwd": [], "bwd": []})
+    info = card()
+    for _ in range(a.rounds):                                      # alternate the variants
+        for d, (heads, fwd, bwd, ms) in runs.items():
+            ms["fwd"].append(event_ms(fwd, a.fwd_iters))
+            ms["bwd"].append(event_ms(bwd, a.bwd_iters))
+    be.check_fault()
+
+    lines = []
+    for d, (heads, _, _, ms) in runs.items():
+        for kern, key, fl in (("attention_tc", "fwd", 4.0), ("attention_bwd", "bwd", 10.0)):
+            med = statistics.median(ms[key])
+            lines.append(json.dumps({"kernel": kern, "B": B, "T": T, "C": C, "heads": heads, "head_dim": d,
+                                     "ms": round(med, 4), "ms_rounds": [round(x, 4) for x in ms[key]],
+                                     "algo_tflops": round(fl * B * T * T * C / med / 1e9, 2), **info}))
+    for ln in lines:
+        print(ln)
+    if a.out:
+        with open(a.out, "a") as f:
+            f.write("\n".join(lines) + "\n")
+
+
+if __name__ == "__main__":
+    main()
