@@ -179,16 +179,26 @@ def test_conv_direct(be, B, H, W, Cin, Cout, k, stride):
 
 CONV_CASES = [
     # B, H,  W,  Cin, Cout, taps, Cin2, res_mode
-    (2, 16, 16, 64, 64, 9, 0, 0),        # smallest aligned case (BN=64)
-    (2, 16, 16, 128, 128, 9, 0, 1),      # BN=128 + same-res residual
-    (1, 32, 32, 128, 256, 9, 64, 0),     # BN=256 + fused 1x1 skip operand
+    # (tile plans: tests/_conv_plan.py; unless noted, a case runs BN=64 with one tile per CTA on 114 and 132 SMs)
+    (2, 16, 16, 64, 64, 9, 0, 0),        # smallest aligned case
+    (2, 16, 16, 128, 128, 9, 0, 1),      # same-res residual
+    (1, 32, 32, 128, 256, 9, 64, 0),     # fused 1x1 skip operand
     (2, 8, 8, 256, 512, 9, 0, 2),        # TW=8 tile geometry, nearest-up residual
     (2, 16, 16, 64, 128, 9, 0, 3),       # 2x2-avg residual
     (3, 4, 4, 256, 256, 9, 0, 1),        # tile spans several images (TB=8 > B: OOB batch rows)
     (2, 12, 20, 64, 64, 9, 0, 1),        # ragged: H, W not multiples of the box
-    (2, 16, 16, 128, 384, 1, 0, 1),      # 1x1 (qkv / proj_out shape), BN=128
+    (2, 16, 16, 128, 384, 1, 0, 1),      # 1x1 (qkv / proj_out shape)
     (1, 64, 64, 640, 128, 9, 640, 0),    # output-block shape: concat width + 1x1 skip
-    (5, 16, 16, 1024, 1024, 9, 0, 1),    # K = 9216, many k-blocks, multiple tiles per CTA
+    (5, 16, 16, 1024, 1024, 9, 0, 1),    # K = 9216 (144 K-blocks); BN=64 with 160 tiles on 132 SMs, BN=128 on 114
+    # the plans production runs: BN=128 with several tiles per CTA on 114 and 132 SMs
+    (4, 64, 64, 128, 256, 9, 0, 1),      # KB 18: partial last promotion chunk
+    (1, 256, 256, 128, 128, 9, 0, 1),    # level-0 geometry of the 256x256 model: 512 tiles
+    (4, 64, 64, 256, 256, 9, 128, 0),    # fused 1x1 skip operand: KB 36 + 2
+    (8, 32, 32, 512, 512, 9, 0, 2),      # nearest-up residual, KB 72
+    (4, 64, 64, 128, 256, 9, 0, 3),      # 2x2-avg residual
+    (4, 64, 64, 64, 256, 1, 0, 1),       # KB 1: the ring advances once per tile
+    (4, 32, 32, 1024, 1024, 9, 0, 1),    # long K: KB 144
+    (4, 64, 64, 128, 192, 9, 0, 1),      # BN=64 forced by Cout, several tiles per CTA
 ]
 
 
@@ -197,9 +207,9 @@ CONV_CASES = [
 def test_conv_umma(be, case, passes):
     B, H, W, Cin, Cout, taps, Cin2, res_mode = case
     k = 3 if taps == 9 else 1
-    a = rnd((B, H, W, Cin), 50)
-    w, b = rnd((Cout, Cin, k, k), 51, 0.02), rnd((Cout,), 52, 0.1)
-    a_hi, a_lo = (t.to(torch.bfloat16).to(DEV) for t in O.bf16_split(a))
+    a = rnd((B, H, W, Cin), 50).to(DEV)          # fp64 references on the GPU: the large cases take minutes on a CPU
+    w, b = rnd((Cout, Cin, k, k), 51, 0.02).to(DEV), rnd((Cout,), 52, 0.1).to(DEV)
+    a_hi, a_lo = (t.to(torch.bfloat16) for t in O.bf16_split(a))
     w_hi, w_lo = _pack_split(be, w)
     kw = {}
     d64 = torch.float64
@@ -208,39 +218,74 @@ def test_conv_umma(be, case, passes):
     else:
         want = O.op_conv_nhwc(O.bf16_split(a)[0].to(d64), O.bf16_split(w)[0].to(d64), b.to(d64))
     if Cin2:
-        a2, w2, b2 = rnd((B, H, W, Cin2), 53), rnd((Cout, Cin2, 1, 1), 54, 0.02), rnd((Cout,), 55, 0.1)
-        a2_hi, a2_lo = (t.to(torch.bfloat16).to(DEV) for t in O.bf16_split(a2))
+        a2, w2, b2 = (t.to(DEV) for t in (rnd((B, H, W, Cin2), 53), rnd((Cout, Cin2, 1, 1), 54, 0.02), rnd((Cout,), 55, 0.1)))
+        a2_hi, a2_lo = (t.to(torch.bfloat16) for t in O.bf16_split(a2))
         w2_hi, w2_lo = _pack_split(be, w2)
-        kw = dict(Cin2=Cin2, a2_hi=a2_hi, a2_lo=a2_lo, w2_hi=w2_hi, w2_lo=w2_lo, bias2=b2.to(DEV))
+        kw = dict(Cin2=Cin2, a2_hi=a2_hi, a2_lo=a2_lo, w2_hi=w2_hi, w2_lo=w2_lo, bias2=b2)
         want = want + (O.op_conv_split3(a2, w2, b2) if passes == 3 else
                        O.op_conv_nhwc(O.bf16_split(a2)[0].to(d64), O.bf16_split(w2)[0].to(d64), b2.to(d64)))
     res = None
     if res_mode == 1:
-        res = rnd((B, H, W, Cout), 56)
+        res = rnd((B, H, W, Cout), 56).to(DEV)
         want = want + res.double()
     elif res_mode == 2:
-        res = rnd((B, H // 2, W // 2, Cout), 56)
+        res = rnd((B, H // 2, W // 2, Cout), 56).to(DEV)
         want = want + O.op_resample(res, 1).double()
     elif res_mode == 3:
-        res = rnd((B, H * 2, W * 2, Cout), 56)
+        res = rnd((B, H * 2, W * 2, Cout), 56).to(DEV)
         want = want + O.op_resample(res.double(), 2)
     out = torch.full((B, H, W, Cout), float("nan"), device=DEV)
-    oh = torch.empty((B, H, W, Cout), dtype=torch.bfloat16, device=DEV)
-    ol = torch.empty_like(oh)
+    oh = torch.full((B, H, W, Cout), float("nan"), dtype=torch.bfloat16, device=DEV)
+    ol = torch.full_like(oh, float("nan"))
     be.conv_umma(B=B, H=H, W=W, Cin=Cin, Cout=Cout, taps=taps, a_hi=a_hi, a_lo=a_lo, w_hi=w_hi, w_lo=w_lo,
-                 bias=b.to(DEV), residual=None if res is None else res.to(DEV), res_mode=res_mode, out=out,
-                 out_hi=oh, out_lo=ol, passes=passes, **kw)
+                 bias=b, residual=res, res_mode=res_mode, out=out, out_hi=oh, out_lo=ol, passes=passes, **kw)
     torch.cuda.synchronize()
     be.check_fault()
     assert not torch.isnan(out).any()
     # the kernel differs from the fp64 evaluation of the same split products only by fp32 accumulation
     assert rel_dev(out, want) < 6e-6, rel_dev(out, want)
-    if passes == 3:      # and the split scheme itself is fp32-class accurate vs the exact conv
-        exact = O.op_conv_nhwc(a.double(), w.double(), b.double())
-        if Cin2 == 0 and res_mode == 0:
-            assert rel_dev(out, exact) < 3e-5
+    if passes == 3 and Cin2 == 0 and res_mode == 0:      # and the split scheme itself is fp32-class accurate
+        assert rel_dev(out, O.op_conv_nhwc(a.double(), w.double(), b.double())) < 3e-5     # vs the exact conv
     h, l = O.bf16_split(out.cpu())
     assert torch.equal(oh.float().cpu(), h) and torch.equal(ol.float().cpu(), l)
+
+
+def _uniform(shape, seed, lo, hi):
+    g = torch.Generator().manual_seed(seed)
+    return (lo + (hi - lo) * torch.rand(shape, generator=g)).float()
+
+
+@pytest.mark.parametrize("case", [(4, 32, 32, 1024, 1024, 128), (2, 16, 16, 1024, 1024, 64)])
+@pytest.mark.parametrize("passes", [3, 1])
+def test_conv_umma_long_k_positive_operands(be, case, passes):
+    """K = 9216 (144 K-blocks) with strictly positive operands, at both N tiles.  The tensor core's accumulator add
+    truncates; with one sign, those errors add up instead of cancelling, so a chain that is not promoted to the fp32
+    register accumulator every few K-blocks drifts.  Compared with the fp64 evaluation of the same split products;
+    two launches must be bit-identical.  Measured on an H100 80GB HBM3 (132 SMs, 400 W power limit), both N tiles:
+    1.1e-6 at passes 3 and 8.4e-7 at passes 1; with the whole chain left in the wgmma accumulator (no promotion)
+    5.8e-5 and 3.7e-5."""
+    from _conv_plan import conv_plan
+    B, H, W, Cin, Cout, BN = case
+    plan = conv_plan(B, H, W, Cin, Cout, 9, passes=passes)
+    assert plan["BN"] == BN and plan["KB"] == 144
+    a, w = _uniform((B, H, W, Cin), 57, 0.25, 1.25).to(DEV), _uniform((Cout, Cin, 3, 3), 58, 0.0, 0.02).to(DEV)
+    a_hi, a_lo = (t.to(torch.bfloat16) for t in O.bf16_split(a))
+    w_hi, w_lo = _pack_split(be, w)
+    if passes == 3:
+        want = O.op_conv_split3(a, w)
+    else:
+        want = O.op_conv_nhwc(O.bf16_split(a)[0].double(), O.bf16_split(w)[0].double())
+    outs = []
+    for _ in range(2):
+        outs.append(torch.full((B, H, W, Cout), float("nan"), device=DEV))
+        be.conv_umma(B=B, H=H, W=W, Cin=Cin, Cout=Cout, taps=9, a_hi=a_hi, a_lo=a_lo, w_hi=w_hi, w_lo=w_lo,
+                     out=outs[-1], passes=passes)
+    torch.cuda.synchronize()
+    be.check_fault()
+    assert torch.equal(outs[0], outs[1])
+    d = rel_dev(outs[0], want)
+    print(f"\n[conv long K, positive operands, BN={BN} passes={passes}] rel dev {d:.3e}")
+    assert d < 4e-6, d
 
 
 def test_conv_umma_rejects_bad_shapes(be):
@@ -304,8 +349,15 @@ def test_attention_split(be, B, T, heads, D, order):
     assert torch.equal(oh.float().cpu(), h) and torch.equal(ol.float().cpu(), l)
 
 
-@pytest.mark.parametrize("B,H,W,Cin,Cout,c2", [(2, 16, 16, 64, 128, 0), (3, 32, 16, 128, 256, 64), (2, 12, 20, 64, 64, 0),
-                                              (2, 16, 8, 64, 640, 128)])
+GN_STATS_CONV_CASES = [
+    # B, H, W, Cin, Cout, c2
+    (2, 16, 16, 64, 128, 0), (3, 32, 16, 128, 256, 64), (2, 12, 20, 64, 64, 0), (2, 16, 8, 64, 640, 128),
+    (4, 64, 64, 128, 256, 0),      # BN=128, several tiles per CTA: the 128-wide statistics loop
+    (4, 64, 64, 128, 256, 128),    # ... and a concat whose second conv also runs BN=128
+]
+
+
+@pytest.mark.parametrize("B,H,W,Cin,Cout,c2", GN_STATS_CONV_CASES)
 def test_conv_umma_fused_groupnorm_statistics(be, B, H, W, Cin, Cout, c2):
     """GroupNorm partial sums written by the conv epilogue + finalize == statistics of the stored
     tensor (also for the concat of two conv outputs whose groups straddle the boundary)."""
@@ -335,14 +387,21 @@ def test_conv_umma_fused_groupnorm_statistics(be, B, H, W, Cin, Cout, c2):
     assert be.conv_geometry(4, 4)[3] == 0        # tile spans images: caller must use bbdm_gn_stats
 
 
-@pytest.mark.parametrize("B,H,W,Cin,Cout,res", [(2, 8, 8, 64, 64, False), (2, 16, 16, 128, 256, True), (1, 12, 20, 64, 128, False),
-                                                (3, 4, 4, 256, 256, True)])
+UPSAMPLE_CONV_CASES = [
+    # B, H, W, Cin, Cout, res     (H, W: the low-res input)
+    (2, 8, 8, 64, 64, False), (2, 16, 16, 128, 256, True), (1, 12, 20, 64, 128, False), (3, 4, 4, 256, 256, True),
+    (4, 32, 32, 256, 256, True),   # BN=128, several tiles per CTA
+]
+
+
+@pytest.mark.parametrize("B,H,W,Cin,Cout,res", UPSAMPLE_CONV_CASES)
 def test_conv_umma_fused_upsample(be, B, H, W, Cin, Cout, res):
     """nearest-2x + 3x3 conv as 4 phases x 2x2 taps on the low-res operand == conv on the upsampled tensor."""
     from bbdm_b200.weights import upsample_phase_weights
-    a, w, b = rnd((B, H, W, Cin), 100), rnd((Cout, Cin, 3, 3), 101, 0.03), rnd((Cout,), 102, 0.1)
-    a_hi, a_lo = (t.to(torch.bfloat16).to(DEV) for t in O.bf16_split(a))
+    a, w, b = rnd((B, H, W, Cin), 100).to(DEV), rnd((Cout, Cin, 3, 3), 101, 0.03), rnd((Cout,), 102, 0.1).to(DEV)
+    a_hi, a_lo = (t.to(torch.bfloat16) for t in O.bf16_split(a))
     wp = upsample_phase_weights(w).to(DEV)
+    w = w.to(DEV)
     hi = torch.empty((16, Cout, Cin), dtype=torch.bfloat16, device=DEV)
     lo = torch.empty_like(hi)
     be.pack_weight_split_taps(wp, hi, lo)
@@ -350,14 +409,13 @@ def test_conv_umma_fused_upsample(be, B, H, W, Cin, Cout, res):
     want = O.op_conv_nhwc(O.op_resample(a_val, 1), w.double(), b.double())
     r = None
     if res:
-        r = rnd((B, H, W, Cout), 103)
+        r = rnd((B, H, W, Cout), 103).to(DEV)
         want = want + O.op_resample(r.double(), 1)
     rows = 4 * be.conv_geometry(H, W)[3]
     part = torch.full((B * rows, Cout, 2), float("nan"), device=DEV) if rows else None
     out = torch.full((B, 2 * H, 2 * W, Cout), float("nan"), device=DEV)
-    be.conv_umma(B=B, H=H, W=W, Cin=Cin, Cout=Cout, taps=4, a_hi=a_hi, a_lo=a_lo, w_hi=hi, w_lo=lo, bias=b.to(DEV),
-                 residual=None if r is None else r.to(DEV), res_mode=2 if res else 0, out=out, passes=3,
-                 upsample2x=True, stats_partial=part)
+    be.conv_umma(B=B, H=H, W=W, Cin=Cin, Cout=Cout, taps=4, a_hi=a_hi, a_lo=a_lo, w_hi=hi, w_lo=lo, bias=b,
+                 residual=r, res_mode=2 if res else 0, out=out, passes=3, upsample2x=True, stats_partial=part)
     be.check_fault()
     assert not torch.isnan(out).any()
     assert rel_dev(out, want) < 3e-5           # weights are re-split after the tap sums: 2^-17-level difference
@@ -366,6 +424,66 @@ def test_conv_umma_fused_upsample(be, B, H, W, Cin, Cout, res):
         be.gn_finalize_partials(part, rows, None, 0, B, 4 * H * W, 32, 1e-5, mean, rstd)
         m_want, r_want = O.op_gn_stats(out.cpu())
         assert (mean.cpu() - m_want).abs().max() < 3e-6 and rel_dev(rstd, r_want) < 3e-6
+
+
+def test_conv_cases_cover_dispatch_regimes(be):
+    """The conv and weight-gradient cases of the suite, planned for this card, run every kernel instantiation and
+    tile-plan regime the host can choose.  The N-tile and grid rules depend on the SM count; if they change, this
+    fails until the cases are moved back into the regimes they claim."""
+    from _conv_plan import conv_geometry, conv_plan, num_sms, wgrad_plan
+    from test_gpu_training import WG_CASES
+    from test_gpu_winograd import FP16_CONV_CASES
+    sms = num_sms()
+    conv = []
+
+    def add(test, case, plan, passes=3, f16=False, res=0, cin2=False, out_hilo=False, stats=False, up2=False):
+        conv.append(dict(test=test, case=case, passes=passes, f16=f16, res=res, cin2=cin2, out_hilo=out_hilo,
+                         stats=stats, up2=up2, **plan))
+        assert be.conv_geometry(case[1], case[2])[:3] == conv_geometry(case[1], case[2])
+
+    for c in CONV_CASES:
+        B, H, W, Cin, Cout, taps, Cin2, res = c
+        for p in (3, 1):
+            add("conv_umma", c, conv_plan(B, H, W, Cin, Cout, taps, Cin2, passes=p, sms=sms), passes=p, res=res,
+                cin2=Cin2 > 0, out_hilo=True)
+    for c in GN_STATS_CONV_CASES:
+        B, H, W, Cin, Cout, c2 = c
+        for co in (Cout, c2) if c2 else (Cout,):
+            add("gn_stats", c, conv_plan(B, H, W, Cin, co, 9, sms=sms), stats=True)
+    for c in UPSAMPLE_CONV_CASES:
+        B, H, W, Cin, Cout, res = c
+        add("upsample", c, conv_plan(B, H, W, Cin, Cout, 4, up2=True, sms=sms), res=2 if res else 0,
+            stats=be.conv_geometry(H, W)[3] > 0, up2=True)
+    for c in FP16_CONV_CASES:
+        B, H, W, Cin, Cout, p = c
+        add("fp16", c, conv_plan(B, H, W, Cin, Cout, 9, passes=p, sms=sms), passes=p, f16=True)
+    wg = []
+    for c in WG_CASES:
+        B, H, W, Cin, Cout, k = c
+        plan = wgrad_plan(B, H, W, Cin, Cout, k * k, sms=sms)
+        assert be.wgrad_workspace(B, H, W, Cin, Cout, k * k) == (plan["splits_ws"], plan["workspace"])
+        wg.append(dict(case=c, **plan))
+
+    print(f"\n{sms} SMs\n{'test':10} {'case':36} {'p':>2} {'f16':>3} {'BN':>4} {'KB':>4} {'tail':>4} {'tiles':>6} {'/CTA':>4}")
+    for r in conv:
+        print(f"{r['test']:10} {str(r['case']):36} {r['passes']:2} {int(r['f16']):3} {r['BN']:4} {r['KB']:4} "
+              f"{r['kb_tail']:4} {r['tiles']:6} {r['tiles_per_cta']:4}")
+    print(f"{'wgrad':10} {'case':36} {'BN':>4} {'splits':>6} {'kb/split':>8} {'last':>4} {'tail':>4} {'items':>6} {'/CTA':>4}")
+    for r in wg:
+        print(f"{'wgrad':10} {str(r['case']):36} {r['BN']:4} {r['splits']:6} {r['kb_per_split']:8} "
+              f"{r['kb_last_split']:4} {r['kb_tail']:4} {r['items']:6} {r['items_per_cta']:4}")
+
+    assert {(r["BN"], r["passes"], r["f16"]) for r in conv} == \
+        {(bn, p, f) for bn in (64, 128) for p in (3, 1) for f in (False, True)}
+    b128 = [r for r in conv if r["BN"] == 128]
+    assert {1, 2, 3} <= {r["res"] for r in b128}
+    for feature in ("cin2", "out_hilo", "stats", "up2"):
+        assert any(r[feature] for r in b128), feature
+    for bn in (64, 128):
+        assert any(r["BN"] == bn and r["tiles_per_cta"] > 1 and r["kb_tail"] > 0 for r in conv), bn
+        assert any(r["BN"] == bn and r["items_per_cta"] > 1 for r in wg), bn
+    assert any(r["KB"] == 1 for r in conv)
+    assert any(r["kb_tail"] > 0 for r in wg) and any(r["splits"] > 1 for r in wg)
 
 
 @pytest.mark.parametrize("B,T,heads,order", [(1, 128, 1, 0), (2, 256, 4, 0), (1, 1024, 2, 1), (1, 100, 2, 1), (1, 4096, 2, 0),

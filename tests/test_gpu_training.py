@@ -43,26 +43,28 @@ def test_split_grad(be, P, C):
 
 
 WG_CASES = [
-    # B, H, W, Cin, Cout, k
+    # B, H, W, Cin, Cout, k     (N tile BN = 128 couts when Cin % 128 == 0, else 64; plans: tests/_conv_plan.py)
     (2, 8, 8, 64, 64, 3),        # BN = 64 (single MN atom), 64-pixel box = one image
     (1, 16, 16, 128, 128, 3),    # BN = 128: two MN atoms (LBO)
-    (2, 16, 16, 256, 128, 3),    # BN = 256: four MN atoms, 8 promotion warps
-    (2, 64, 64, 64, 192, 3),     # box = one row of 64; Cout tile partially out of range
+    (2, 16, 16, 256, 128, 3),    # BN = 128, two Cin tiles
+    (2, 64, 64, 64, 192, 3),     # box = one row of 64; Cout tile partially out of range; BN 64, 16 splits, 3 items per CTA
     (4, 4, 4, 128, 64, 3),       # box spans 4 images
     (2, 16, 16, 128, 256, 1),    # 1x1
-    (1, 32, 32, 512, 512, 3),    # deeper K split
+    (1, 32, 32, 512, 512, 3),    # two K splits
+    (2, 256, 256, 128, 128, 3),  # 38-44 splits of 47-54 K-blocks (partial last chunk), a short last split, 3 items per CTA
+    (16, 16, 16, 512, 320, 3),   # ragged Cout tiles (n_co = 3), 4 items per CTA
 ]
 
 
 @pytest.mark.parametrize("case", WG_CASES)
 def test_conv_wgrad(be, case):
     B, H, W, Cin, Cout, k = case
-    a = rnd((B, H, W, Cin), 2)
-    g = rnd((B, H, W, Cout), 3, 0.1)
+    a = rnd((B, H, W, Cin), 2).to(DEV)            # fp64 reference on the GPU: the large cases take minutes on a CPU
+    g = rnd((B, H, W, Cout), 3, 0.1).to(DEV)
     P = B * H * W
-    a_hi, a_lo = (t.to(torch.bfloat16).to(DEV) for t in O.bf16_split(a))
+    a_hi, a_lo = (t.to(torch.bfloat16) for t in O.bf16_split(a))
     ht, lt = torch.empty((Cout, P), dtype=torch.bfloat16, device=DEV), torch.empty((Cout, P), dtype=torch.bfloat16, device=DEV)
-    be.split_grad(g.reshape(P, Cout).to(DEV), None, None, ht, lt)
+    be.split_grad(g.reshape(P, Cout), None, None, ht, lt)
     _, fl = be.wgrad_workspace(B, H, W, Cin, Cout, k * k)
     ws = torch.empty(fl, device=DEV)
     dw = torch.full((Cout, Cin, k, k), float("nan"), device=DEV)
@@ -72,10 +74,45 @@ def test_conv_wgrad(be, case):
     # exact gradient for the values the planes carry
     av = sum(O.bf16_split(a)).double().permute(0, 3, 1, 2).requires_grad_(False)
     gv = sum(O.bf16_split(g)).double().permute(0, 3, 1, 2)
-    w = torch.zeros((Cout, Cin, k, k), dtype=torch.float64, requires_grad=True)
+    w = torch.zeros((Cout, Cin, k, k), dtype=torch.float64, device=DEV, requires_grad=True)
     F.conv2d(av, w, padding=k // 2).backward(gv)
     assert not torch.isnan(dw).any()
     assert rel_dev(dw, w.grad) < 2e-5, rel_dev(dw, w.grad)
+
+
+def test_conv_wgrad_long_chain_positive_operands(be):
+    """One split with a 64-K-block chain and strictly positive operands: truncation errors of the tensor core's
+    accumulator add up instead of cancelling unless the chain is promoted to fp32 registers every few K-blocks.
+    Compared with the fp64 sum of the three split products the kernel issues (hi.hi + lo.hi + hi.lo; the dropped
+    lo.lo term would bias a comparison with positive operands by up to ~4e-6); two launches must be bit-identical.
+    Measured on an H100 80GB HBM3 (132 SMs, 400 W power limit): 9.7e-7; with the chain unpromoted, 2.1e-5."""
+    from _conv_plan import wgrad_plan
+    B, H, W, Cin, Cout = 4, 32, 32, 1024, 1024
+    plan = wgrad_plan(B, H, W, Cin, Cout, 9)
+    assert plan["splits"] == 1 and plan["kb_per_split"] == 64 and plan["BN"] == 128
+    gen = torch.Generator().manual_seed(4)
+    a = (0.25 + torch.rand((B, H, W, Cin), generator=gen)).to(DEV)
+    g = (0.02 * torch.rand((B, H, W, Cout), generator=gen)).to(DEV)
+    P = B * H * W
+    a_hi, a_lo = O.bf16_split(a)
+    g_hi, g_lo = O.bf16_split(g)
+    ht, lt = torch.empty((Cout, P), dtype=torch.bfloat16, device=DEV), torch.empty((Cout, P), dtype=torch.bfloat16, device=DEV)
+    be.split_grad(g.reshape(P, Cout), None, None, ht, lt)
+    _, fl = be.wgrad_workspace(B, H, W, Cin, Cout, 9)
+    ws = torch.empty(fl, device=DEV)
+    dws = []
+    for _ in range(2):
+        dws.append(torch.full((Cout, Cin, 3, 3), float("nan"), device=DEV))
+        be.conv_wgrad(ht, lt, a_hi.to(torch.bfloat16), a_lo.to(torch.bfloat16), B, H, W, Cin, Cout, 9, dws[-1], ws)
+    torch.cuda.synchronize()
+    be.check_fault()
+    assert torch.equal(dws[0], dws[1])
+    nchw = lambda t: t.double().permute(0, 3, 1, 2)
+    wgrad = lambda x, dy: torch.nn.grad.conv2d_weight(nchw(x), (Cout, Cin, 3, 3), nchw(dy), padding=1)
+    want = wgrad(a_hi, g_hi) + wgrad(a_hi, g_lo) + wgrad(a_lo, g_hi)
+    d = rel_dev(dws[0], want)
+    print(f"\n[wgrad 64-K-block chain, positive operands] rel dev {d:.3e}")
+    assert d < 4e-6, d
 
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout,k,bias", [(2, 16, 16, 64, 128, 3, True), (1, 32, 32, 128, 64, 3, False),
@@ -194,6 +231,93 @@ def test_gn_act_conv_function_with_resampling(resample):
     assert rel_dev(y, yd) < 3e-5
     for name, a, r in [("x", x, xd), ("gamma", gamma, gd), ("beta", beta, bd), ("w", w, wd), ("b", b, bbd)]:
         assert rel_dev(a.grad, r.grad) < 5e-5, (name, rel_dev(a.grad, r.grad))
+
+
+GN_BWD_CASES = [
+    # B, H, W, C, silu, film      (32 groups; the reduce runs min(64, ...) pixel slices per image)
+    (16, 1, 1, 1536, True, True),     # HW = 1: pixel lanes R and slices S clamp to 1
+    (3, 1, 1, 96, True, False),       # 3 channels per group
+    (16, 2, 2, 96, True, True),
+    (3, 2, 2, 2048, False, True),
+    (1, 2, 2, 1024, True, False),
+    (3, 8, 8, 32, True, True),
+    (1, 8, 8, 320, False, True),
+    (16, 8, 8, 1536, True, True),     # C > 1024: two column passes in the reduce; apply needs > 48 KiB shared memory
+    (3, 64, 64, 1024, True, True),
+    (1, 64, 64, 2048, True, False),
+    (16, 64, 64, 320, True, True),
+    (1, 64, 64, 32, False, False),
+    (1, 256, 256, 128, True, True),   # 65536 pixels per image
+]
+
+
+def _gn_bwd_check(be, B, H, W, C, silu, film, shift=None):
+    """Runs bbdm_gn_bwd_reduce and bbdm_gn_bwd_apply twice, as GNActConv2dFn.backward does, and returns the rel devs
+    of (sum_p dz, sum_p dz*xh, dx) from fp64 after checking that the two runs are bit-identical."""
+    x = (rnd((B, H, W, C), 60, 1.5) + 0.3).to(DEV)
+    da = rnd((B, H, W, C), 61, 0.2).to(DEV)
+    gamma, beta = (1 + 0.1 * rnd((C,), 62)).to(DEV), (0.1 * rnd((C,), 63)).to(DEV)
+    fs = fh = None
+    fstride = 0
+    if film:                 # scale / shift rows inside a wider buffer, as the time-embedding projection writes them
+        fstride = 2 * C + 8
+        fbuf = (0.3 * rnd((B, fstride), 64)).to(DEV)
+        if shift is not None:
+            fbuf[:, C + 4:2 * C + 4] = shift
+        fs, fh = fbuf[:, :C], fbuf[:, C + 4:2 * C + 4]
+    mean, rstd = (t.to(DEV) for t in O.op_gn_stats(x))
+    runs = []
+    for _ in range(2):
+        a12 = torch.full((B, C, 2), float("nan"), device=DEV)
+        ws = torch.full((B * 64 * C * 2,), float("nan"), device=DEV)
+        be.gn_bwd_reduce(x, da, 32, mean, rstd, gamma, beta, fs, fh, fstride, silu, a12, ws)
+        f1 = (1.0 + fs) if film else torch.ones((B, C), device=DEV)
+        gf = gamma * f1
+        s1 = (gf * a12[..., 0]).view(B, 32, C // 32).sum(2).contiguous()
+        s2 = (gf * a12[..., 1]).view(B, 32, C // 32).sum(2).contiguous()
+        dx = torch.full((B, H, W, C), float("nan"), device=DEV)
+        be.gn_bwd_apply(x, da, 32, mean, rstd, gamma, beta, fs, fh, fstride, silu, s1, s2, dx)
+        runs.append((a12, dx))
+    torch.cuda.synchronize()
+    be.check_fault()
+    assert torch.equal(runs[0][0], runs[1][0]) and torch.equal(runs[0][1], runs[1][1])
+    a12, dx = runs[0]
+    assert torch.isfinite(a12).all() and torch.isfinite(dx).all()
+
+    d = torch.float64
+    f1 = (1.0 + fs.to(d)) if film else torch.ones((B, C), dtype=d, device=DEV)
+    f0 = fh.to(d) if film else torch.zeros((B, C), dtype=d, device=DEV)
+    per_c = lambda t: t.to(d).repeat_interleave(C // 32, 1)[:, None, None, :]
+    xh = (x.to(d) - per_c(mean)) * per_c(rstd)                       # from the fp32 statistics the kernels get
+    z = (gamma.to(d) * xh + beta.to(d)) * f1[:, None, None, :] + f0[:, None, None, :]
+    sg = torch.sigmoid(z)
+    dz = da.to(d) * sg * (1 + z * (1 - sg)) if silu else da.to(d)
+    dev_a1, dev_a2 = rel_dev(a12[..., 0], dz.sum((1, 2))), rel_dev(a12[..., 1], (dz * xh).sum((1, 2)))
+    xd = x.to(d).permute(0, 3, 1, 2).requires_grad_(True)
+    h = F.group_norm(xd, 32, gamma.to(d), beta.to(d), 1e-5) * f1[:, :, None, None] + f0[:, :, None, None]
+    (F.silu(h) if silu else h).backward(da.to(d).permute(0, 3, 1, 2))
+    dev_dx = rel_dev(dx, xd.grad.permute(0, 2, 3, 1))
+    print(f"\n[gn_bwd B={B} HW={H}x{W} C={C} silu={silu} film={film}] rel dev a1 {dev_a1:.3e} a2 {dev_a2:.3e} "
+          f"dx {dev_dx:.3e}")
+    return dev_a1, dev_a2, dev_dx
+
+
+@pytest.mark.parametrize("B,H,W,C,silu,film", GN_BWD_CASES)
+def test_gn_bwd_kernels(be, B, H, W, C, silu, film):
+    """GroupNorm(+FiLM)(+SiLU) backward kernels against fp64: the reduce against (sum_p dz, sum_p dz*xh), the apply
+    against the autograd gradient of silu(GN(x)*(1+scale)+shift) w.r.t. x.  Measured on an H100 80GB HBM3 (400 W
+    power limit): at most 2.6e-7 (sums) and 3.2e-7 (dx) over these cases."""
+    dev_a1, dev_a2, dev_dx = _gn_bwd_check(be, B, H, W, C, silu, film)
+    assert dev_a1 < 2e-6 and dev_a2 < 2e-6 and dev_dx < 2e-6
+
+
+def test_gn_bwd_kernels_large_preactivation(be):
+    """FiLM shifts across [-100, 100]: the SiLU derivative's fast exp overflows for z << 0 and saturates for z >> 0;
+    the gradients stay finite and match (measured on an H100: 3.4e-7)."""
+    B, C = 2, 320
+    shift = torch.linspace(-100.0, 100.0, C, device=DEV).repeat(B, 1)
+    dev_a1, dev_a2, dev_dx = _gn_bwd_check(be, B, 8, 8, C, True, True, shift=shift)
+    assert dev_a1 < 2e-6 and dev_a2 < 2e-6 and dev_dx < 2e-6
 
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout,k,need_dx", [(2, 16, 16, 6, 128, 3, False), (2, 16, 16, 128, 3, 3, True),

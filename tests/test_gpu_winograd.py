@@ -137,20 +137,41 @@ def test_wino_conv_chain_vs_fp64_conv(be, case):
     assert rel_dev(mean2, mw) < 1e-5 and rel_dev(rstd2, rw) < 1e-5
 
 
+FP16_CONV_CASES = [
+    # B, H, W, Cin, Cout, passes
+    (2, 16, 16, 128, 128, 3),                                # BN=64, one tile per CTA
+    (2, 16, 16, 128, 128, 1),
+    (4, 64, 64, 128, 256, 3), (4, 64, 64, 128, 256, 1),      # BN=128, several tiles per CTA
+]
+
+
 def test_conv_umma_fp16_operands_direct_conv(be):
     """operand_f16 on the ordinary 3x3 implicit GEMM: split-fp16 planes (22 mantissa bits) instead of split-bf16."""
-    B, H, W, Cin, Cout = 2, 16, 16, 128, 128
-    a, w, b = rnd((B, H, W, Cin), 20), rnd((Cout, Cin, 3, 3), 21, 0.02), rnd((Cout,), 22, 0.1)
+    _check_fp16_direct_conv(be, *FP16_CONV_CASES[0])
+
+
+@pytest.mark.parametrize("B,H,W,Cin,Cout,passes", FP16_CONV_CASES[1:])
+def test_conv_umma_fp16_operands_direct_conv_plans(be, B, H, W, Cin, Cout, passes):
+    """The same at passes 1 and with the BN=128 multi-tile plan."""
+    _check_fp16_direct_conv(be, B, H, W, Cin, Cout, passes)
+
+
+def _check_fp16_direct_conv(be, B, H, W, Cin, Cout, passes):
+    """passes=3 is compared with the exact conv, passes=1 with the fp64 conv of the hi planes it multiplies."""
+    a, w = rnd((B, H, W, Cin), 20).to(DEV), rnd((Cout, Cin, 3, 3), 21, 0.02).to(DEV)
 
     def split16(x):
         h = x.to(torch.float16)
-        return h.to(DEV), (x - h.float()).to(torch.float16).to(DEV)
+        return h, (x - h.float()).to(torch.float16)
     a_hi, a_lo = split16(a)
     w_hi, w_lo = split16((w * 256.0).permute(2, 3, 0, 1).reshape(9, Cout, Cin).contiguous())
-    out = torch.empty((B, H, W, Cout), device=DEV)
+    out = torch.full((B, H, W, Cout), float("nan"), device=DEV)
     be.conv_umma(B=B, H=H, W=W, Cin=Cin, Cout=Cout, taps=9, a_hi=a_hi, a_lo=a_lo, w_hi=w_hi, w_lo=w_lo, out=out,
-                 passes=3, operand_f16=True)
-    want = O.op_conv_nhwc(a.double(), w.double() * 256.0, None)
+                 passes=passes, operand_f16=True)
+    if passes == 3:
+        want = O.op_conv_nhwc(a.double(), w.double() * 256.0, None)
+    else:
+        want = O.op_conv_nhwc(a_hi.double(), (w * 256.0).to(torch.float16).double(), None)
     d = rel_dev(out, want)
-    print(f"\n[direct conv, split-fp16 x3] rel dev vs fp64 conv {d:.3e}")
+    print(f"\n[direct conv, split-fp16 x{passes}] rel dev vs fp64 conv {d:.3e}")
     assert d < 2e-6, d
