@@ -15,7 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BBDM_LIB selects another in-tree build of the same sources (A/B experiments, tools/); the product default is fixed
 LIB_PATH = os.environ.get("BBDM_LIB") or os.path.join(_HERE, "libbbdm_b200.so")
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 OBJ = {"grad": 0, "noise": 1, "ysubx": 2}
 RESAMPLE_NONE, RESAMPLE_UP2, RESAMPLE_DOWN2 = 0, 1, 2
 RES_NONE, RES_SAME, RES_UP2, RES_DOWN2 = 0, 1, 2, 3
@@ -78,7 +78,7 @@ class WinoInputArgs(C.Structure):
 
 
 class WinoOutputArgs(C.Structure):
-    _fields_ = [("m", C.c_void_p), ("B", C.c_int), ("H", C.c_int), ("W", C.c_int), ("Cout", C.c_int),
+    _fields_ = [("m", C.c_void_p), ("inv_wscale", C.c_void_p), ("B", C.c_int), ("H", C.c_int), ("W", C.c_int), ("Cout", C.c_int),
                 ("bias", C.c_void_p), ("residual", C.c_void_p), ("res_mode", C.c_int),
                 ("out", C.c_void_p), ("stats_partial", C.c_void_p)]
 
@@ -142,7 +142,7 @@ def load():
     lib.bbdm_wino_geometry.argtypes = [i, i, i, C.POINTER(i), C.POINTER(i), C.POINTER(i64), C.POINTER(i)]
     lib.bbdm_wino_input.argtypes = [C.POINTER(WinoInputArgs), vp]
     lib.bbdm_wino_output.argtypes = [C.POINTER(WinoOutputArgs), vp]
-    lib.bbdm_wino_pack_weight.argtypes = [vp, i, i, i, vp, vp, vp]
+    lib.bbdm_wino_pack_weight.argtypes = [vp, i, i, i, vp, vp, vp, vp]
     lib.bbdm_denorm_to_uint8.argtypes = [vp, i, i, i, i, i, vp, vp]
     lib.bbdm_spatial_rescale.argtypes = [vp, i, i, i, i, i, vp, vp, i, vp, vp]
     lib.bbdm_layernorm_split.argtypes = [vp, i64, i, vp, vp, f, vp, vp, vp, vp]
@@ -226,6 +226,9 @@ class CudaBackend:
 
     name = "sm_90a"
     requires_cuda = True
+    # wino_pack_weight / wino_output take inv_wscale: per-tensor power-of-two scales of the Winograd weight planes
+    # (a backend without it packs at the fixed 2^8, and the engines call it without a scale)
+    wino_tensor_scale = True
 
     def __init__(self):
         self.lib = load()
@@ -373,18 +376,23 @@ class CudaBackend:
         check(self.lib.bbdm_wino_input(C.byref(a), stream()))
         LAUNCHES["n"] += 1
 
-    def wino_output(self, m, *, B, H, W, Cout, bias=None, residual=None, res_mode=RES_NONE, out, stats_partial=None):
-        a = WinoOutputArgs(ptr(_req(m)), B, H, W, Cout, ptr(bias), ptr(residual), res_mode, ptr(_req(out)),
+    def wino_output(self, m, *, B, H, W, Cout, bias=None, residual=None, res_mode=RES_NONE, out, stats_partial=None,
+                    inv_wscale=None):
+        """inv_wscale: the [1] fp32 device tensor wino_pack_weight wrote for the weight planes of this GEMM (None:
+        planes packed at the fixed 2^8)."""
+        a = WinoOutputArgs(ptr(_req(m)), None if inv_wscale is None else ptr(_req(inv_wscale)), B, H, W, Cout, ptr(bias), ptr(residual), res_mode, ptr(_req(out)),
                            ptr(stats_partial))
         check(self.lib.bbdm_wino_output(C.byref(a), stream()))
         LAUNCHES["n"] += 1
 
-    def wino_pack_weight(self, w, u_hi, u_lo, dgrad=False):
-        """w [Cout,Cin,3,3] fp32 -> u_hi/u_lo fp16 [36, Cout, Cin] (2^8 * G w G^T); dgrad: [36, Cin, Cout] of the
-        flipped / channel-swapped kernel."""
+    def wino_pack_weight(self, w, u_hi, u_lo, dgrad=False, inv_wscale=None):
+        """w [Cout,Cin,3,3] fp32 -> u_hi/u_lo fp16 [36, Cout, Cin] (s * G w G^T); dgrad: [36, Cin, Cout] of the
+        flipped / channel-swapped kernel.  inv_wscale [1] fp32 on the device: s is the per-tensor power of two and
+        1/s is written there (pass it to wino_output); None: the fixed s = 2^8."""
         Cout, Cin = w.shape[0], w.shape[1]
         check(self.lib.bbdm_wino_pack_weight(ptr(_req(w)), Cout, Cin, int(dgrad), ptr(_req(u_hi, torch.float16)),
-                                             ptr(_req(u_lo, torch.float16)), stream()))
+                                             ptr(_req(u_lo, torch.float16)),
+                                             None if inv_wscale is None else ptr(_req(inv_wscale)), stream()))
         LAUNCHES["n"] += 1
 
     # -- SpatialTransformer pieces --------------------------------------------------------------------------

@@ -10,23 +10,40 @@
 //                       split-fp16 planes V_hi, V_lo [36][tiles][C]; optionally also the split-bf16 planes of
 //                       the raw input (A operand of the ResBlock's 1x1 skip conv).  HBM-bound:
 //                       4 B read + 36/16 * 4 B written per input element.
-//   wino_weight_kernel  U = 2^8 * G g G^T (fp64 from the fp32 OIHW weight) -> split-fp16 [36][Cout][Cin].
-//   wino_output_kernel  M [36][tiles][Cout] fp32 -> Y = 2^-8 * A^T M A + bias (+ residual: same / nearest-up /
+//   wino_weight_kernel  U = s * G g G^T (fp64 from the fp32 OIHW weight) -> split-fp16 [36][Cout][Cin], with the
+//                       per-tensor power of two s = 2^(14 - ceil(log2 max|w|)) (wino_wmax_kernel reduces max|w|).
+//   wino_output_kernel  M [36][tiles][Cout] fp32 -> Y = (1/s) * A^T M A + bias (+ residual: same / nearest-up /
 //                       2x2-avg addressed) -> fp32 NHWC + fused GroupNorm partial sums of the result.
 //                       HBM-bound: 36/16 * 4 B read + 4 B written per output element.
 //
 // Numerics (tools/studies/split_formats_accuracy.py): split-FP16 operands carry 22 mantissa bits (bf16 pairs: 16),
 // which pays for the F(4,3) transforms' error amplification; the GEMM promotes the tensor core's truncating
 // accumulator into fp32 registers every 2-4 K-blocks (conv_umma.cu), and tests/test_gpu_winograd.py bounds the chain's
-// deviation from the fp64 conv.  The weight planes are pre-scaled by 2^8 (exact) so that U_lo stays
-// a normal fp16 number; the output transform multiplies by 2^-8.
+// deviation from the fp64 conv.  The weight planes are pre-scaled by the power of two s (exact): every entry of
+// G g G^T is bounded by max|g| (the absolute row sums of G are at most 1), so |s U| <= 2^14 < 65504 and the hi and lo
+// planes of the largest entries stay normal fp16 numbers at any weight magnitude (a fixed scale loses the lo planes to
+// fp16's subnormal range for small weights: 2.5e-5 instead of 6e-6 at weight std 1e-3).  The scale stays on the device
+// (1/s in a caller-provided float that the output transform reads): training repacks every step without a host
+// synchronisation, and sampling replays a captured graph.
 #include "common.cuh"
 #include <cuda_fp16.h>
 #include <stdlib.h>
 
 namespace bbdm {
 
-constexpr float WINO_WSCALE = 256.0f;
+constexpr float WINO_WSCALE_FIXED = 256.0f;    // scale without a scale buffer, and of an all-zero weight tensor
+
+// s = 2^(14 - ceil(log2 m)) from the bit pattern of m = max|w| (a non-negative float), exponent clamped to +-100
+__host__ __device__ inline float wino_wscale(uint32_t mbits) {
+  if (mbits == 0) return WINO_WSCALE_FIXED;
+  const int e = (int)(mbits >> 23) - 127;                  // m = 1.f * 2^e (subnormals: e = -127)
+  int k = 14 - (e + ((mbits & 0x7fffffu) != 0 ? 1 : 0));
+  k = k < -100 ? -100 : (k > 100 ? 100 : k);
+  float s = 1.0f;
+  for (; k > 0; --k) s *= 2.0f;
+  for (; k < 0; ++k) s *= 0.5f;
+  return s;
+}
 
 // ---- 1-D transforms (interpolation points 0, +-1, +-2; Lavin & Gray) -----------------------------
 // B^T (6x6) applied to d[0..5] with stride S in a register array
@@ -341,6 +358,7 @@ wino_input_smem_kernel(const WinoInParams p) {
 // ------------------------------------------------------------------------------------------
 struct WinoOutParams {
   const float* m; int64_t Mtot;
+  const float* inv_wscale;   // 1/s of the weight planes (device scalar written by bbdm_wino_pack_weight), or nullptr: 2^-8
   int B, H, W, Cout, th, tw;
   const float* bias;
   const float* residual; int res_mode;
@@ -358,8 +376,7 @@ struct WinoOutParams {
 // this code on the CPU against a direct fp64 evaluation (tests/test_wino_output_host.py).
 template <int RES>
 __host__ __device__ __forceinline__ void wino_output_tile(const WinoOutParams& p, int b, int ty, int tx, int c, float2 bv,
-                                                          float& sum0, float& sum1, float& sq0, float& sq1) {
-  const float inv = 1.0f / WINO_WSCALE;
+                                                          float inv, float& sum0, float& sum1, float& sq0, float& sq1) {
   const int64_t m = ((int64_t)b * p.th + ty) * p.tw + tx;
   float mx[36], my[36];
 #pragma unroll
@@ -432,8 +449,9 @@ wino_output_kernel(const WinoOutParams p) {
   const int c = cg * 64 + lane * 2;
   float2 bv = make_float2(0.f, 0.f);
   if (p.bias) bv = *reinterpret_cast<const float2*>(p.bias + c);
+  const float inv = p.inv_wscale ? __ldg(p.inv_wscale) : 1.0f / WINO_WSCALE_FIXED;
   float sum0 = 0.f, sum1 = 0.f, sq0 = 0.f, sq1 = 0.f;
-  for (int tx = tl; tx < p.tw; tx += 8) wino_output_tile<RES>(p, b, ty, tx, c, bv, sum0, sum1, sq0, sq1);
+  for (int tx = tl; tx < p.tw; tx += 8) wino_output_tile<RES>(p, b, ty, tx, c, bv, inv, sum0, sum1, sq0, sq1);
   if (p.stats) {
     // fixed-order combine of the 8 tile-column lanes => deterministic partial sums
     red[tl][lane * 2][0] = sum0; red[tl][lane * 2][1] = sq0;
@@ -450,13 +468,31 @@ wino_output_kernel(const WinoOutParams p) {
 }
 
 // ------------------------------------------------------------------------------------------
-// U[q][co][ci] = 2^8 * (G g G^T)[q] in fp64, split into fp16 planes.  One thread per (co, ci).
+// max|w| over the whole tensor: atomicMax on the bit patterns of the non-negative floats |w| (their integer order is
+// their value order), so the result does not depend on the order the blocks run in.  *wmax must be zeroed first.
+__global__ void __launch_bounds__(256)
+wino_wmax_kernel(const float* __restrict__ w, int64_t n, uint32_t* __restrict__ wmax) {
+  uint32_t m = 0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    m = max(m, __float_as_uint(fabsf(w[i])));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0 && m) atomicMax(wmax, m);
+}
+
+// *inv = 1/s, in place over the max|w| bits it is computed from (after the packing kernel has read them)
+__global__ void wino_wscale_store_kernel(float* inv) {
+  *inv = 1.0f / wino_wscale(__float_as_uint(*inv));
+}
+
+// U[q][co][ci] = s * (G g G^T)[q] in fp64, split into fp16 planes.  One thread per (co, ci).
 // dgrad != 0: the data-gradient conv's weights instead -- kernel flipped, channels swapped: U[q][ci][co] from
 // g'[ky][kx] = w[co][ci][2-ky][2-kx] (threads run over co fastest so the stores stay coalesced).
 __global__ void __launch_bounds__(256)
-wino_weight_kernel(const float* __restrict__ w, int Cout, int Cin, int dgrad, __half* __restrict__ u_hi,
-                   __half* __restrict__ u_lo) {
+wino_weight_kernel(const float* __restrict__ w, int Cout, int Cin, int dgrad, const uint32_t* __restrict__ wmax,
+                   __half* __restrict__ u_hi, __half* __restrict__ u_lo) {
   const int64_t n = (int64_t)Cout * Cin;
+  const double s = wmax ? (double)wino_wscale(*wmax) : (double)WINO_WSCALE_FIXED;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < n; idx += (int64_t)gridDim.x * blockDim.x) {
     double g[3][3], t[6][3];
     int64_t src = idx;
@@ -488,7 +524,7 @@ wino_weight_kernel(const float* __restrict__ w, int Cout, int Cin, int dgrad, __
       u[5] = g2;
 #pragma unroll
       for (int j = 0; j < 6; ++j) {
-        const float v = (float)(u[j] * (double)WINO_WSCALE);
+        const float v = (float)(u[j] * s);
         const __half h = __float2half_rn(v);
         const __half l = __float2half_rn(v - __half2float(h));
         const int64_t off = (int64_t)(i * 6 + j) * n + idx;
@@ -576,7 +612,7 @@ int bbdm_wino_input(const BbdmWinoInputArgs* a, void* stream) {
 int bbdm_wino_output(const BbdmWinoOutputArgs* a, void* stream) {
   BBDM_REQUIRE(a && a->m && a->out, "wino_output: null args");
   WinoOutParams p;
-  p.m = a->m;
+  p.m = a->m; p.inv_wscale = a->inv_wscale;
   p.B = a->B; p.H = a->H; p.W = a->W; p.Cout = a->Cout;
   BBDM_REQUIRE(p.B > 0 && p.B <= 65535 && p.H > 0 && p.W > 0 && p.H % 4 == 0 && p.W % 4 == 0,
                "wino_output: H, W must be multiples of 4 (B <= 65535)");
@@ -600,12 +636,23 @@ int bbdm_wino_output(const BbdmWinoOutputArgs* a, void* stream) {
   return BBDM_OK;
 }
 
-int bbdm_wino_pack_weight(const float* w, int Cout, int Cin, int dgrad, void* u_hi, void* u_lo, void* stream) {
+int bbdm_wino_pack_weight(const float* w, int Cout, int Cin, int dgrad, void* u_hi, void* u_lo, float* inv_wscale,
+                          void* stream) {
   BBDM_REQUIRE(w && u_hi && u_lo && Cout > 0 && Cin > 0, "wino_pack_weight: bad args");
+  cudaStream_t st = (cudaStream_t)stream;
   const int64_t n = (int64_t)Cout * Cin;
+  // inv_wscale holds max|w| (as bits) until the packing kernel has read it, then 1/s.  Without it: the fixed 2^8.
+  uint32_t* wmax = reinterpret_cast<uint32_t*>(inv_wscale);
+  if (wmax) {
+    BBDM_CUDA_CHECK(cudaMemsetAsync(wmax, 0, sizeof(uint32_t), st));
+    int64_t g = (n * 9 + 255) / 256;
+    if (g > (int64_t)num_sms() * 8) g = (int64_t)num_sms() * 8;
+    wino_wmax_kernel<<<(unsigned)g, 256, 0, st>>>(w, n * 9, wmax);
+  }
   int64_t g = (n + 255) / 256;
   if (g > (int64_t)num_sms() * 16) g = (int64_t)num_sms() * 16;
-  wino_weight_kernel<<<(unsigned)g, 256, 0, (cudaStream_t)stream>>>(w, Cout, Cin, dgrad, (__half*)u_hi, (__half*)u_lo);
+  wino_weight_kernel<<<(unsigned)g, 256, 0, st>>>(w, Cout, Cin, dgrad, wmax, (__half*)u_hi, (__half*)u_lo);
+  if (wmax) wino_wscale_store_kernel<<<1, 1, 0, st>>>(inv_wscale);
   BBDM_LAUNCH_CHECK();
   return BBDM_OK;
 }

@@ -207,8 +207,9 @@ class KernelExecutor:
         pool.put(v_hi, v_lo)
         out = pool.get((B, H, W, cout))
         part = pool.get((B * th, cout, 2)) if stats else None
+        skw = {} if ent.get("u_inv") is None else dict(inv_wscale=ent["u_inv"])
         be.wino_output(mbuf, B=B, H=H, W=W, Cout=cout, bias=ent["bias"], residual=residual, res_mode=res_mode,
-                       out=out, stats_partial=part)
+                       out=out, stats_partial=part, **skw)
         pool.put(mbuf)
         if part is not None:
             out._gn = (part, th)
@@ -324,7 +325,8 @@ class UNetEngine(KernelExecutor):
                     pack_tensor(blk.ff.net[0].proj.weight, blk.ff.net[0].proj.bias, pre + ".ff.net.0.proj")
                     pack_tensor(blk.ff.net[2].weight, blk.ff.net[2].bias, pre + ".ff.net.2")
         if self.wino:
-            # stride-1 3x3 ResBlock convs: Winograd-domain weight planes U = 2^8 G g G^T, fp16 hi/lo [36][Cout][Cin]
+            # stride-1 3x3 ResBlock convs: Winograd-domain weight planes U = s G g G^T, fp16 hi/lo [36][Cout][Cin], and
+            # 1/s (per-tensor power of two) as a device scalar beside them: a stable address for graph replay
             for name, m in u.named_modules():
                 if not isinstance(m, ResBlock) or not m.use_scale_shift_norm:
                     continue
@@ -335,7 +337,10 @@ class UNetEngine(KernelExecutor):
                         continue
                     uh = buf(cname, "u_hi", (36, ent["cout"], ent["cin"]), torch.float16)
                     ul = buf(cname, "u_lo", (36, ent["cout"], ent["cin"]), torch.float16)
-                    be.wino_pack_weight(conv.weight.detach().contiguous(), uh, ul)
+                    skw = {}
+                    if getattr(be, "wino_tensor_scale", False):
+                        ent["u_inv"] = skw["inv_wscale"] = buf(cname, "u_inv", (1,), torch.float32)
+                    be.wino_pack_weight(conv.weight.detach().contiguous(), uh, ul, **skw)
                     ent["u_hi"], ent["u_lo"] = uh, ul
         for name, m in u.named_modules():
             if isinstance(m, ResBlock) and m.up and m.channels % 64 == 0 and m.out_channels % 64 == 0:

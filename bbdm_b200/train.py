@@ -65,13 +65,17 @@ def _wino_conv(be, xn, weight, *, dgrad, gn=None, act_planes=None, bias=None, re
     be.wino_input(xn, None, v_hi=v_hi, v_lo=v_lo, **kw, **akw)
     u_hi = torch.empty((36, out_channels, C), dtype=torch.float16, device=dev)
     u_lo = torch.empty_like(u_hi)
-    be.wino_pack_weight(weight.detach().contiguous(), u_hi, u_lo, dgrad=dgrad)
+    skw = {}
+    if getattr(be, "wino_tensor_scale", False):
+        # per-tensor scale of the planes: 1/s stays on the device (no host synchronisation)
+        skw["inv_wscale"] = torch.empty((1,), dtype=torch.float32, device=dev)
+    be.wino_pack_weight(weight.detach().contiguous(), u_hi, u_lo, dgrad=dgrad, **skw)
     m = torch.empty((36, mt, out_channels), dtype=torch.float32, device=dev)
     be.conv_umma(B=36, H=mt // 16, W=16, Cin=C, Cout=out_channels, taps=1, a_hi=v_hi, a_lo=v_lo, w_hi=u_hi, w_lo=u_lo,
                  out=m, passes=3, weights_per_image=True, operand_f16=True)
     out = torch.empty((B, H, W, out_channels), dtype=torch.float32, device=dev)
     be.wino_output(m, B=B, H=H, W=W, Cout=out_channels, bias=bias, residual=residual,
-                   res_mode=cabi.RES_NONE if residual is None else cabi.RES_SAME, out=out)
+                   res_mode=cabi.RES_NONE if residual is None else cabi.RES_SAME, out=out, **skw)
     return out
 
 

@@ -70,7 +70,10 @@ class VQGANEngine(KernelExecutor):
                 # ResnetBlock 3x3 convs: Winograd-domain planes (csrc/winograd.cu), like the UNet's ResBlocks
                 ent["u_hi"] = be.empty((36, cout, cin), torch.float16, dev)
                 ent["u_lo"] = be.empty((36, cout, cin), torch.float16, dev)
-                be.wino_pack_weight(wt, ent["u_hi"], ent["u_lo"])
+                skw = {}
+                if getattr(be, "wino_tensor_scale", False):
+                    ent["u_inv"] = skw["inv_wscale"] = be.empty((1,), torch.float32, dev)
+                be.wino_pack_weight(wt, ent["u_hi"], ent["u_lo"], **skw)
             w[name] = ent
 
         for name, m in self.vq.named_modules():

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define BBDM_ABI_VERSION 2
+#define BBDM_ABI_VERSION 3
 
 enum {
   BBDM_OK = 0,
@@ -243,8 +243,11 @@ int bbdm_gn_finalize_partials(const float* part1, int c1, int rows1, const float
 /* ------------------------------------------------------------------------------------------
  * Winograd F(4x4, 3x3) path for the stride-1 3x3 ResBlock convolutions (openaimodel.py:207,233): 4x fewer
  * tensor-core MACs.  conv = wino_input -> bbdm_conv_umma(weights_per_image, operand_f16; B = 36 positions,
- * H = tiles/16, W = 16, taps = 1, out = M) -> wino_output.  Split-FP16 operands keep the deviation from the
- * fp32 reference below the direct split-bf16 kernel's.
+ * H = tiles/16, W = 16, taps = 1, out = M) -> wino_output.  Split-FP16 operands carry 22 mantissa bits; the
+ * deviation of the chain from the fp64 conv is set by the position GEMMs' accumulation, which the output transform
+ * amplifies: on an H100 80GB HBM3 (400 W) 5.6e-6 to 9.6e-6 at every weight std from 2e-2 to 1e-4, against 4.5e-6
+ * for the direct split-bf16 kernel (tests/test_gpu_winograd_range.py).  Promoting every K-block
+ * (BBDM_WINO_CHUNK=1) brings it to the direct kernel's level.
  * ------------------------------------------------------------------------------------------ */
 
 /* tiles_h = H/4, tiles_w = W/4, tiles_total = B*tiles_h*tiles_w; eligible = 1 iff H, W are multiples of 4 and
@@ -256,7 +259,11 @@ int bbdm_wino_geometry(int B, int H, int W, int* tiles_h, int* tiles_w, int64_t*
  * split-fp16 planes v_hi, v_lo [36][tiles_total][C].  raw_hi/raw_lo (optional): split-bf16 NHWC planes of the
  * raw input (A operand of the ResBlock's 1x1 skip convolution, openaimodel.py:244).
  * mean == NULL (silu must be 0): identity -- the tensor is transformed as it is (the data-gradient convolution of
- * the training path transforms dY). */
+ * the training path transforms dY).
+ * Range: V is stored as fp16 (largest finite 65504) and B^T d B amplifies a tile by at most 100, so max|act| <= 655
+ * is finite for every input; on GroupNorm-normalised random inputs the first non-finite result came at
+ * max|act| ~ 4100 (2060 was finite; tools/wino_activation_window.py, H100).  The forward route does not guard
+ * against larger activations: they give inf/NaN. */
 typedef struct {
   const float* src1; int c1;
   const float* src2; int c2;
@@ -272,11 +279,13 @@ typedef struct {
 } BbdmWinoInputArgs;
 int bbdm_wino_input(const BbdmWinoInputArgs* a, void* stream);
 
-/* m [36][tiles_total][Cout] fp32 (the position GEMMs' output) -> out [B,H,W,Cout] = 2^-8 * A^T m A + bias
+/* m [36][tiles_total][Cout] fp32 (the position GEMMs' output) -> out [B,H,W,Cout] = inv_wscale * A^T m A + bias
  * (+ residual, addressed as in BbdmConvArgs.res_mode), and optionally the GroupNorm partial sums of the result:
  * stats_partial [B * tiles_h][Cout][2] (rows_per_image = tiles_h for bbdm_gn_finalize_partials). */
 typedef struct {
   const float* m;
+  const float* inv_wscale;   /* device float 1/s written by bbdm_wino_pack_weight for the weight planes; NULL: the
+                                fixed 2^-8 of planes packed without a scale buffer */
   int B, H, W, Cout;
   const float* bias;
   const float* residual; int res_mode;
@@ -285,10 +294,15 @@ typedef struct {
 } BbdmWinoOutputArgs;
 int bbdm_wino_output(const BbdmWinoOutputArgs* a, void* stream);
 
-/* w [Cout,Cin,3,3] fp32 -> U = 2^8 * G w G^T (fp64 arithmetic), split-fp16 planes u_hi, u_lo [36][Cout][Cin].
- * dgrad != 0: the planes of the data-gradient convolution instead ([36][Cin][Cout], kernel flipped, channels
- * swapped; cf. bbdm_pack_weight_split_dgrad). */
-int bbdm_wino_pack_weight(const float* w, int Cout, int Cin, int dgrad, void* u_hi, void* u_lo, void* stream);
+/* w [Cout,Cin,3,3] fp32 -> U = s * G w G^T (fp64 arithmetic), split-fp16 planes u_hi, u_lo [36][Cout][Cin], with
+ * the per-tensor power of two s = 2^(14 - ceil(log2 max|w|)) (2^8 for an all-zero tensor), so that |U| <= 2^14 and
+ * the planes stay normal fp16 numbers at any weight magnitude.  max|w| is reduced on the device (deterministic) and
+ * 1/s is written to the device float *inv_wscale, which bbdm_wino_output takes: no host synchronisation, and a
+ * stable address for graph replay.  inv_wscale == NULL: the fixed s = 2^8 (exact for N(0, 0.02)-scale weights; the
+ * lo planes of much smaller weights become fp16 subnormals).  dgrad != 0: the planes of the data-gradient convolution instead
+ * ([36][Cin][Cout], kernel flipped, channels swapped; cf. bbdm_pack_weight_split_dgrad). */
+int bbdm_wino_pack_weight(const float* w, int Cout, int Cin, int dgrad, void* u_hi, void* u_lo, float* inv_wscale,
+                          void* stream);
 
 /* General fp32 direct convolution on CUDA cores (any Cin/Cout, k in {1,3}, stride 1 or 2,
  * pad k/2): stem (openaimodel.py:524), head (:690), conv-mode Downsample/Upsample (:109,150)

@@ -2,6 +2,8 @@
 restatements.  It lets the not-gpu suite verify the engine's host logic (block wiring, FiLM
 offsets, concat order, skip/residual modes, buffer lifetimes) without a GPU.  It lives under
 tests/ and is never imported by the product."""
+import math
+
 import torch
 import torch.nn.functional as F
 
@@ -11,6 +13,7 @@ from oracle import bbdm_oracle as O
 class EmuBackend:
     name = "oracle-emulation (tests only)"
     requires_cuda = False
+    wino_tensor_scale = True          # as CudaBackend: per-tensor Winograd weight scales
 
     def __init__(self):
         self.calls = []
@@ -241,19 +244,33 @@ class EmuBackend:
         if raw_hi is not None:
             self._write_split(x, raw_hi, raw_lo)
 
-    def wino_pack_weight(self, w, u_hi, u_lo, dgrad=False):
+    @staticmethod
+    def _wino_wscale(w):
+        """The kernel's per-tensor power of two: 2^(14 - ceil(log2 max|w|)), exponent clamped to +-100; 2^8 for 0."""
+        m = float(w.abs().max())
+        if m == 0.0:
+            return 256.0
+        f, e = math.frexp(m)                                   # m = f * 2^e, f in [0.5, 1)
+        return 2.0 ** min(max(14 - (e - 1 if f == 0.5 else e), -100), 100)
+
+    def wino_pack_weight(self, w, u_hi, u_lo, dgrad=False, inv_wscale=None):
         self.calls.append("wino_pack_weight")
+        s = 256.0 if inv_wscale is None else self._wino_wscale(w)
+        if inv_wscale is not None:
+            inv_wscale.fill_(1.0 / s)
         if dgrad:
             w = w.flip(2, 3).transpose(0, 1)
-        U = torch.einsum("ij,kcjl,ml->imkc", self._G, w.double(), self._G) * 256.0           # [6,6,Cout,Cin]
+        U = torch.einsum("ij,kcjl,ml->imkc", self._G, w.double(), self._G) * s               # [6,6,Cout,Cin]
         self._write_split_f16(U.reshape(u_hi.shape), u_hi, u_lo)
 
-    def wino_output(self, m, *, B, H, W, Cout, bias=None, residual=None, res_mode=0, out, stats_partial=None):
+    def wino_output(self, m, *, B, H, W, Cout, bias=None, residual=None, res_mode=0, out, stats_partial=None,
+                    inv_wscale=None):
         self.calls.append("wino_output")
         assert not torch.isnan(m).any()
         th, tw = H // 4, W // 4
         M = m.double().reshape(6, 6, B, th, tw, Cout)
-        Y = torch.einsum("ij,jlbxyc,ml->bxiymc", self._AT, M, self._AT) / 256.0             # [B,th,4,tw,4,Cout]
+        inv = 1.0 / 256.0 if inv_wscale is None else float(inv_wscale)
+        Y = torch.einsum("ij,jlbxyc,ml->bxiymc", self._AT, M, self._AT) * inv               # [B,th,4,tw,4,Cout]
         o = Y.reshape(B, H, W, Cout).float()
         if bias is not None:
             o = o + bias

@@ -432,7 +432,8 @@ def test_conv_cases_cover_dispatch_regimes(be):
     fails until the cases are moved back into the regimes they claim."""
     from _conv_plan import conv_geometry, conv_plan, num_sms, wgrad_plan
     from test_gpu_training import WG_CASES
-    from test_gpu_winograd import FP16_CONV_CASES
+    from test_gpu_winograd import CHAIN, FP16_CONV_CASES, PROD_CHAIN
+    from test_gpu_winograd_range import SWEEP_CASES
     sms = num_sms()
     conv = []
 
@@ -457,6 +458,20 @@ def test_conv_cases_cover_dispatch_regimes(be):
     for c in FP16_CONV_CASES:
         B, H, W, Cin, Cout, p = c
         add("fp16", c, conv_plan(B, H, W, Cin, Cout, 9, passes=p, sms=sms), passes=p, f16=True)
+    # Winograd position GEMMs: 36 images (transform positions) of tiles/16 x 16 "pixels", one weight plane per position
+    wino = []
+    wino_cases = [(B, H, W, c1 + c2, Cout) for B, H, W, c1, c2, Cout, _ in CHAIN] + \
+        [(B, H, W, c1 + c2, Cout) for B, H, W, c1, c2, Cout in PROD_CHAIN] + SWEEP_CASES
+    for c in wino_cases:
+        B, H, W, Cin, Cout = c
+        mt = be.wino_geometry(B, H, W)[2]
+        assert be.conv_geometry(mt // 16, 16)[:3] == conv_geometry(mt // 16, 16)
+        plan = conv_plan(36, mt // 16, 16, Cin, Cout, 1, wpi=True, sms=sms)
+        per_pos = plan["tiles"] // 36
+        # a CTA walks tiles t, t + grid, ...: does any CTA move on to another position (another weight plane)?
+        plan["pos_change"] = any(t // per_pos != (t + plan["grid"]) // per_pos for t in range(plan["tiles"] - plan["grid"]))
+        wino.append(dict(case=c, **plan))
+
     wg = []
     for c in WG_CASES:
         B, H, W, Cin, Cout, k = c
@@ -468,6 +483,10 @@ def test_conv_cases_cover_dispatch_regimes(be):
     for r in conv:
         print(f"{r['test']:10} {str(r['case']):36} {r['passes']:2} {int(r['f16']):3} {r['BN']:4} {r['KB']:4} "
               f"{r['kb_tail']:4} {r['tiles']:6} {r['tiles_per_cta']:4}")
+    print(f"{'wino':10} {'case':36} {'BN':>4} {'KB':>4} {'chunk':>5} {'tail':>4} {'tiles':>6} {'/CTA':>4} {'pos+':>4}")
+    for r in wino:
+        print(f"{'wino':10} {str(r['case']):36} {r['BN']:4} {r['KB']:4} {r['kb_per_chunk']:5} {r['kb_tail']:4} "
+              f"{r['tiles']:6} {r['tiles_per_cta']:4} {int(r['pos_change']):4}")
     print(f"{'wgrad':10} {'case':36} {'BN':>4} {'splits':>6} {'kb/split':>8} {'last':>4} {'tail':>4} {'items':>6} {'/CTA':>4}")
     for r in wg:
         print(f"{'wgrad':10} {str(r['case']):36} {r['BN']:4} {r['splits']:6} {r['kb_per_split']:8} "
@@ -484,6 +503,11 @@ def test_conv_cases_cover_dispatch_regimes(be):
         assert any(r["BN"] == bn and r["items_per_cta"] > 1 for r in wg), bn
     assert any(r["KB"] == 1 for r in conv)
     assert any(r["kb_tail"] > 0 for r in wg) and any(r["splits"] > 1 for r in wg)
+    assert {r["BN"] for r in wino} == {64, 128}
+    assert any(r["tiles_per_cta"] > 1 for r in wino)
+    for chunk in (2, 4):
+        assert any(r["kb_per_chunk"] == chunk and r["kb_tail"] > 0 for r in wino), chunk
+    assert any(r["tiles_per_cta"] > 1 and r["pos_change"] for r in wino)
 
 
 @pytest.mark.parametrize("B,T,heads,order", [(1, 128, 1, 0), (2, 256, 4, 0), (1, 1024, 2, 1), (1, 100, 2, 1), (1, 4096, 2, 0),

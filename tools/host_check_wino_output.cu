@@ -1,7 +1,7 @@
 // Host-side check of the Winograd output transform's tile routine (bbdm_b200/csrc/winograd.cu,
 // wino_output_tile<RES>, a __host__ __device__ function): the SAME source the kernel runs is executed on the CPU for
 // every (sample, tile, channel pair) and compared with a direct fp64 evaluation of
-//     out = 2^-8 * A^T M A + bias + residual(same | nearest-up | 2x2-average addressed)
+//     out = inv_wscale * A^T M A + bias + residual(same | nearest-up | 2x2-average addressed)
 // plus the per-thread partial sums that feed the fused GroupNorm statistics.  No GPU and no CUDA runtime call is
 // involved.  Build + run (tests/test_wino_output_host.py does this):
 //     nvcc -std=c++17 --expt-relaxed-constexpr -I include -o /tmp/host_check_wino_output tools/host_check_wino_output.cu
@@ -15,7 +15,7 @@
 static const double AT[4][6] = {{1, 1, 1, 1, 1, 0}, {0, 1, -1, 2, -2, 0}, {0, 1, 1, 4, 4, 0}, {0, 1, -1, 8, -8, 1}};
 
 template <int RES>
-static int run(int B, int H, int W, int Cout, bool with_bias) {
+static int run(int B, int H, int W, int Cout, bool with_bias, float inv) {
   using namespace bbdm;
   std::mt19937 rng(1234 + RES * 7 + H);
   std::normal_distribution<float> nd(0.f, 1.f);
@@ -41,7 +41,7 @@ static int run(int B, int H, int W, int Cout, bool with_bias) {
         for (int c = 0; c < Cout; c += 2) {
           float a0 = 0, a1 = 0, q0 = 0, q1 = 0;
           const float2 bv = with_bias ? make_float2(bias[c], bias[c + 1]) : make_float2(0.f, 0.f);
-          wino_output_tile<RES>(p, b, ty, tx, c, bv, a0, a1, q0, q1);
+          wino_output_tile<RES>(p, b, ty, tx, c, bv, inv, a0, a1, q0, q1);
           s1[c] += a0; s1[c + 1] += a1; s2[c] += q0; s2[c + 1] += q1;
         }
   double worst = 0, scale = 0, r1 = 0, r2 = 0;
@@ -55,7 +55,7 @@ static int run(int B, int H, int W, int Cout, bool with_bias) {
           double y = 0;
           for (int k = 0; k < 6; ++k)
             for (int l = 0; l < 6; ++l) y += AT[i][k] * (double)M[((size_t)(k * 6 + l) * Mtot + m) * Cout + c] * AT[j][l];
-          y = y / 256.0 + (with_bias ? (double)bias[c] : 0.0);
+          y = y * (double)inv + (with_bias ? (double)bias[c] : 0.0);
           if (RES == BBDM_RES_SAME) y += res[(((size_t)b * H + hh) * W + ww) * Cout + c];
           if (RES == BBDM_RES_UP2) y += res[(((size_t)b * RH + hh / 2) * RW + ww / 2) * Cout + c];
           if (RES == BBDM_RES_DOWN2) {
@@ -74,21 +74,22 @@ static int run(int B, int H, int W, int Cout, bool with_bias) {
     r2 = std::fmax(r2, std::fabs(s2[c] - w2[c]) / (1.0 + std::fabs(w2[c])));
   }
   const bool ok = worst <= 2e-6 * scale && r1 < 1e-4 && r2 < 1e-4;
-  std::printf("RES=%d B=%d H=%d W=%d Cout=%d bias=%d: max abs dev %.3e (scale %.3e), partial sums %.1e / %.1e -> %s\n", RES, B, H,
-              W, Cout, (int)with_bias, worst, scale, r1, r2, ok ? "ok" : "FAIL");
+  std::printf("RES=%d B=%d H=%d W=%d Cout=%d bias=%d 1/s=%g: max abs dev %.3e (scale %.3e), partial sums %.1e / %.1e -> %s\n",
+              RES, B, H, W, Cout, (int)with_bias, inv, worst, scale, r1, r2, ok ? "ok" : "FAIL");
   return ok ? 0 : 1;
 }
 
 int main() {
   int bad = 0;
-  bad += run<BBDM_RES_NONE>(2, 8, 12, 64, true);
-  bad += run<BBDM_RES_NONE>(1, 4, 4, 128, false);
-  bad += run<BBDM_RES_SAME>(2, 8, 12, 64, true);
-  bad += run<BBDM_RES_SAME>(3, 16, 8, 128, false);
-  bad += run<BBDM_RES_UP2>(2, 8, 12, 64, true);
-  bad += run<BBDM_RES_UP2>(1, 16, 16, 128, false);
-  bad += run<BBDM_RES_DOWN2>(2, 8, 12, 64, true);
-  bad += run<BBDM_RES_DOWN2>(1, 4, 8, 128, false);
+  // 1/s of the weight planes: the all-zero default 2^-8 and the per-tensor scales of small / large weights
+  bad += run<BBDM_RES_NONE>(2, 8, 12, 64, true, 1.0f / 256);
+  bad += run<BBDM_RES_NONE>(1, 4, 4, 128, false, 1.0f / 131072);
+  bad += run<BBDM_RES_SAME>(2, 8, 12, 64, true, 1.0f / 8192);
+  bad += run<BBDM_RES_SAME>(3, 16, 8, 128, false, 1.0f / 256);
+  bad += run<BBDM_RES_UP2>(2, 8, 12, 64, true, 1.0f / 4096);
+  bad += run<BBDM_RES_UP2>(1, 16, 16, 128, false, 1.0f / 256);
+  bad += run<BBDM_RES_DOWN2>(2, 8, 12, 64, true, 1.0f / 256);
+  bad += run<BBDM_RES_DOWN2>(1, 4, 8, 128, false, 1.0f / 16777216);
   std::printf(bad ? "FAILED\n" : "ALL OK\n");
   return bad;
 }

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Time the Winograd transform kernels (and the position GEMM) in isolation for the cfg2 layer shapes.
     python tools/time_wino.py [--once]        # --once: one launch per kernel (for ncu)
-    python tools/time_wino.py --output-only   # only the output transform, without / with a same-size residual"""
+    python tools/time_wino.py --output-only   # only the output transform, without / with a same-size residual
+    python tools/time_wino.py --pack          # weight packing (max|w| reduction + planes), forward and dgrad"""
 import json
 import sys
 import os
@@ -32,15 +33,27 @@ def main():
     be = cabi.CudaBackend()
     dev = "cuda"
     rows = []
+    inv = torch.full((1,), 1.0 / 256, device=dev)        # 1/s of the weight planes (wino_pack_weight writes it)
+    if "--pack" in sys.argv:
+        for Cout, Cin in ((1024, 1024), (512, 512), (512, 1536), (1024, 1536), (512, 640)):
+            w = 0.02 * torch.randn(Cout, Cin, 3, 3, device=dev)
+            row = {"Cout": Cout, "Cin": Cin}
+            for dgrad in (False, True):
+                uh = torch.empty((36, Cin, Cout) if dgrad else (36, Cout, Cin), dtype=torch.float16, device=dev)
+                ul = torch.empty_like(uh)
+                row["dgrad_ms" if dgrad else "fwd_ms"] = timeit(lambda: be.wino_pack_weight(w, uh, ul, inv, dgrad=dgrad), 50)
+            print(json.dumps(row))
+        be.check_fault()
+        return
     if "--output-only" in sys.argv:
         for B, H, W, Cout in ((16, 128, 128, 512), (16, 64, 64, 1024)):
             th, tw, mt, ok = be.wino_geometry(B, H, W)
             m = torch.randn((36, mt, Cout), device=dev)
             out, res = torch.empty((B, H, W, Cout), device=dev), torch.randn((B, H, W, Cout), device=dev)
             part = torch.empty((B * th, Cout, 2), device=dev)
-            t0 = timeit(lambda: be.wino_output(m, B=B, H=H, W=W, Cout=Cout, out=out, stats_partial=part), 10)
-            t1 = timeit(lambda: be.wino_output(m, B=B, H=H, W=W, Cout=Cout, out=out, stats_partial=part, residual=res,
-                                               res_mode=cabi.RES_SAME), 10)
+            t0 = timeit(lambda: be.wino_output(m, inv_wscale=inv, B=B, H=H, W=W, Cout=Cout, out=out, stats_partial=part), 10)
+            t1 = timeit(lambda: be.wino_output(m, inv_wscale=inv, B=B, H=H, W=W, Cout=Cout, out=out, stats_partial=part,
+                                               residual=res, res_mode=cabi.RES_SAME), 10)
             gb = (36 * mt * Cout * 4 + B * H * W * Cout * 4) / 1e9
             print(json.dumps({"B": B, "H": H, "W": W, "Cout": Cout, "tiles": mt, "wino_output_ms": t0,
                               "wino_output_tbps": gb / t0, "wino_output_residual_ms": t1,
@@ -64,7 +77,7 @@ def main():
                                             v_hi=vh, v_lo=vl), n)
         t_g = timeit(lambda: be.conv_umma(B=36, H=mt // 16, W=16, Cin=Cin, Cout=Cout, taps=1, a_hi=vh, a_lo=vl, w_hi=uh,
                                           w_lo=ul, out=m, passes=3, weights_per_image=True, operand_f16=True), n)
-        t_o = timeit(lambda: be.wino_output(m, B=B, H=H, W=W, Cout=Cout, out=out, stats_partial=part), n)
+        t_o = timeit(lambda: be.wino_output(m, inv_wscale=inv, B=B, H=H, W=W, Cout=Cout, out=out, stats_partial=part), n)
         gb_in = (B * H * W * Cin * 4 + 36 * mt * Cin * 4) / 1e9
         gb_out = (36 * mt * Cout * 4 + B * H * W * Cout * 4) / 1e9
         rows.append({"B": B, "H": H, "W": W, "Cin": Cin, "Cout": Cout, "tiles": mt,
