@@ -20,6 +20,8 @@ OBJ = {"grad": 0, "noise": 1, "ysubx": 2}
 RESAMPLE_NONE, RESAMPLE_UP2, RESAMPLE_DOWN2 = 0, 1, 2
 RES_NONE, RES_SAME, RES_UP2, RES_DOWN2 = 0, 1, 2, 3
 GN_MAX_SLICES = 64
+ATTN_HEAD_DIMS = (16, 32, 64, 128)       # head sizes the attention kernels are built for
+ATTN_TC_HEAD_DIMS = (64, 128)            # ... of which bbdm_attention_tc (wgmma) takes these
 
 # every symbol include/bbdm_b200.h declares (tests check the library exports all of them)
 SYMBOLS = [

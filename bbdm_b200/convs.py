@@ -1,0 +1,160 @@
+"""Convolution decisions shared by the UNet and VQGAN executors (engine.py, vqgan_engine.py) and the training
+Functions (train.py): when a 3x3 conv takes the Winograd path, the Winograd launch sequence itself, and the packed
+weight planes the executors cache.
+
+A leaf module (torch, cabi and the torch-only weights helper): train.py is imported by unet.py, which engine.py
+imports, so the shared code cannot live in engine.py.
+"""
+from __future__ import annotations
+
+import os
+
+import torch
+
+from . import cabi
+from .weights import upsample_phase_weights
+
+# Winograd F(4x4,3x3) for the stride-1 3x3 convs with at least WINO_MIN_C input and output channels (parity mode only;
+# below that the transform traffic outweighs the 4x MAC saving).  BBDM_WINOGRAD=0 disables it in the sampling
+# executors, BBDM_WINOGRAD_TRAIN=0 for the training forward and data gradient (the weight gradient is always direct).
+# These are the defaults: each executor copies them into its wino / wino_min_c / wino_min_tiles attributes, and
+# train.py into its WINO_TRAIN / WINO_MIN_C / WINO_MIN_TILES, which is where a caller overrides them.
+WINOGRAD = os.environ.get("BBDM_WINOGRAD", "1") != "0"
+WINOGRAD_TRAIN = os.environ.get("BBDM_WINOGRAD_TRAIN", "1") != "0"
+WINO_MIN_C = int(os.environ.get("BBDM_WINO_MIN_C", "256"))
+# ... and at least this many 4x4 tiles per launch: below it the 36 position GEMMs have too few M tiles each
+# (measured: cfg1, 256 tiles, graph replay 3.9 -> 4.4 ms with Winograd; cfg3, 2048 tiles, 20.2 -> 17.1 ms)
+WINO_MIN_TILES = int(os.environ.get("BBDM_WINO_MIN_TILES", "512"))
+
+
+def wino_channels_ok(cin, cout, min_c):
+    """The channel half of the Winograd rule (the executors apply it when they pack the weight planes)."""
+    return cin % 64 == 0 and cout % 64 == 0 and min(cin, cout) >= min_c
+
+
+def winograd_ok(geometry, cin, cout, min_c, min_tiles):
+    """Whether a stride-1 3x3 conv of cin -> cout channels takes the Winograd path; geometry is the backend's
+    wino_geometry(B, H, W).  At >= 128 tiles per image always (the choice must not depend on the batch size there:
+    batch-size independent, bit-identical results at the pixel resolutions); smaller maps only when the whole batch
+    has enough tiles."""
+    th, tw, tiles, ok = geometry
+    return bool(ok and wino_channels_ok(cin, cout, min_c) and (th * tw >= 128 or tiles >= min_tiles))
+
+
+class FreshBuffers:
+    """The engines' pool interface over plain allocations (training: the buffers live as long as autograd keeps
+    them)."""
+
+    def __init__(self, device):
+        self.device = device
+
+    def get(self, shape, dtype=torch.float32):
+        return torch.empty(shape, dtype=dtype, device=self.device)
+
+    def put(self, *ts):
+        pass
+
+
+def wino_conv(be, pool, geometry, src1, src2, *, cout, planes=None, weight=None, dgrad=False, bias=None,
+              residual=None, res_mode=cabi.RES_NONE, stats=False, **transform):
+    """3x3 conv of cat(src1, src2) (NHWC fp32) on the Winograd path: input transform (``transform`` are the
+    wino_input arguments: GroupNorm affine + FiLM + SiLU, or identity with silu=False; raw_* / act_* side outputs) ->
+    36 position GEMMs in one wgmma launch -> output transform (+ bias, + residual, + GroupNorm partial sums if stats).
+
+    planes = (u_hi, u_lo, u_inv) packed beforehand (WeightPacker.winograd), or weight [Cout, Cin, 3, 3] to pack here
+    (dgrad: the flipped, channel-swapped kernel).  pool: the executors' _Pool or FreshBuffers."""
+    B, H, W, c1 = src1.shape
+    cin = c1 + (0 if src2 is None else src2.shape[3])
+    th, _, mtot, _ = geometry
+    v_hi, v_lo = pool.get((36, mtot, cin), torch.float16), pool.get((36, mtot, cin), torch.float16)
+    be.wino_input(src1, src2, v_hi=v_hi, v_lo=v_lo, **transform)
+    if planes is None:
+        u_hi, u_lo = pool.get((36, cout, cin), torch.float16), pool.get((36, cout, cin), torch.float16)
+        # per-tensor scale of the planes: 1/s stays on the device (no host synchronisation)
+        u_inv = pool.get((1,)) if getattr(be, "wino_tensor_scale", False) else None
+        be.wino_pack_weight(weight.detach().contiguous(), u_hi, u_lo, dgrad=dgrad,
+                            **({} if u_inv is None else dict(inv_wscale=u_inv)))
+    else:
+        u_hi, u_lo, u_inv = planes
+    m = pool.get((36, mtot, cout))
+    be.conv_umma(B=36, H=mtot // 16, W=16, Cin=cin, Cout=cout, taps=1, a_hi=v_hi, a_lo=v_lo, w_hi=u_hi, w_lo=u_lo,
+                 out=m, passes=3, weights_per_image=True, operand_f16=True)
+    pool.put(v_hi, v_lo)
+    out = pool.get((B, H, W, cout))
+    part = pool.get((B * th, cout, 2)) if stats else None
+    be.wino_output(m, B=B, H=H, W=W, Cout=cout, bias=bias, residual=residual, res_mode=res_mode, out=out,
+                   stats_partial=part, **({} if u_inv is None else dict(inv_wscale=u_inv)))
+    pool.put(m)
+    if part is not None:
+        out._gn = (part, th)
+    return out
+
+
+class WeightPacker:
+    """Packs conv weights into the cache entries the executors read.  Buffers of the previous cache (``old``) are
+    re-packed in place when name, field, shape and device match: no reallocation of the planes when EMA weights are
+    swapped in and out, and every address a captured CUDA graph holds stays valid.
+
+    An entry has cout, cin, k, bias, f32 [k*k][Cin][Cout], and split-bf16 hi/lo [k*k][Cout][Cin] when both channel
+    counts are multiples of 64.  The caller decides which convs also get a zero-padded head (padded_head), Winograd
+    planes (winograd) or the fused nearest-2x phase planes (up_phase)."""
+
+    def __init__(self, be, device, old=None):
+        self.be, self.device, self.old, self.w = be, device, old or {}, {}
+
+    def _buf(self, name, field, shape, dtype):
+        ent = self.old.get(name)
+        t = ent.get(field) if isinstance(ent, dict) else None
+        if t is not None and tuple(t.shape) == tuple(shape) and t.device == self.device:
+            return t
+        return self.be.empty(tuple(shape), dtype, self.device)
+
+    def conv(self, name, weight, bias, padded_head=False):
+        """weight [Cout, Cin, k, k] (or Conv1d [Cout, Cin, 1] / Linear [out, in]).  padded_head: a 3x3 conv with
+        Cout < 64 (an image head) gets planes zero-padded to one 64-wide N tile, for the NCHW-storing epilogue."""
+        be, wt = self.be, weight.detach()
+        while wt.dim() < 4:
+            wt = wt.unsqueeze(-1)
+        wt = wt.contiguous()
+        cout, cin, k = wt.shape[0], wt.shape[1], wt.shape[2]
+        ent = {"cout": cout, "cin": cin, "k": k, "bias": None if bias is None else bias.detach()}
+        if cin % 64 == 0 and cout % 64 == 0 and k in (1, 3):
+            ent["hi"] = self._buf(name, "hi", (k * k, cout, cin), torch.bfloat16)
+            ent["lo"] = self._buf(name, "lo", (k * k, cout, cin), torch.bfloat16)
+            be.pack_weight_split(wt, ent["hi"], ent["lo"])
+        elif padded_head and cin % 64 == 0 and cout < 64 and k == 3:
+            prev = self.old[name].get("hi_pad") if isinstance(self.old.get(name), dict) else None
+            hi = self._buf(name, "hi_pad", (k * k, 64, cin), torch.bfloat16)
+            lo = self._buf(name, "lo_pad", (k * k, 64, cin), torch.bfloat16)
+            bp = self._buf(name, "bias_pad", (64,), torch.float32)
+            if hi is not prev:                   # freshly allocated: the padding rows must be zeroed
+                hi.zero_()
+                lo.zero_()
+            bp.zero_()
+            if bias is not None:
+                bp[:cout].copy_(bias.detach())
+            be.pack_weight_split(wt, hi, lo)
+            ent["hi_pad"], ent["lo_pad"], ent["bias_pad"] = hi, lo, bp
+        ent["f32"] = self._buf(name, "f32", (k * k, cin, cout), torch.float32)
+        be.pack_weight_f32(wt, ent["f32"])
+        self.w[name] = ent
+        return ent
+
+    def winograd(self, name, weight):
+        """Winograd-domain planes U = s G g G^T of the packed 3x3 conv ``name``, fp16 hi/lo [36][Cout][Cin], and 1/s
+        (per-tensor power of two) as a device scalar beside them: a stable address for graph replay."""
+        ent = self.w[name]
+        ent["u_hi"] = self._buf(name, "u_hi", (36, ent["cout"], ent["cin"]), torch.float16)
+        ent["u_lo"] = self._buf(name, "u_lo", (36, ent["cout"], ent["cin"]), torch.float16)
+        skw = {}
+        if getattr(self.be, "wino_tensor_scale", False):
+            ent["u_inv"] = skw["inv_wscale"] = self._buf(name, "u_inv", (1,), torch.float32)
+        self.be.wino_pack_weight(weight.detach().contiguous(), ent["u_hi"], ent["u_lo"], **skw)
+
+    def up_phase(self, name, weight):
+        """The 16 phase taps of nearest-2x + the packed 3x3 conv ``name`` (4 output phases x 2x2 taps on the low-res
+        operand)."""
+        ent = self.w[name]
+        ent["up_hi"] = self._buf(name, "up_hi", (16, ent["cout"], ent["cin"]), torch.bfloat16)
+        ent["up_lo"] = self._buf(name, "up_lo", (16, ent["cout"], ent["cin"]), torch.bfloat16)
+        self.be.pack_weight_split_taps(upsample_phase_weights(weight.detach()), ent["up_hi"], ent["up_lo"])

@@ -12,21 +12,16 @@ logic (block wiring, concat order, FiLM offsets, skip modes) on CPU; the product
 """
 from __future__ import annotations
 
-import os
-
 import torch
 import torch.nn as nn
 
-from . import cabi
-from .weights import upsample_phase_weights
+from . import cabi, convs
 from .transformer import SpatialTransformer
 from .unet import (AttentionBlock, Downsample, ResBlock, TimestepEmbedSequential, UNetModel,
                    Upsample, timestep_embedding)
 
 GN_GROUPS = 32
 GN_EPS = 1e-5
-ATTN_HEAD_DIMS = (16, 32, 64, 128)       # head sizes the attention kernels are built for
-ATTN_TC_HEAD_DIMS = (64, 128)            # ... of which bbdm_attention_tc (wgmma) takes these
 
 
 def resample_to_res(resample):
@@ -79,13 +74,9 @@ class KernelExecutor:
         self._pools = {}
         self._gn_ws = None
         self._geom_cache = {}
-        # Winograd F(4x4,3x3) for the stride-1 3x3 convs with at least this many input and output channels
-        # (parity mode only; below that the transform traffic outweighs the 4x MAC saving).  BBDM_WINOGRAD=0 disables.
-        self.wino = precision == "split3" and os.environ.get("BBDM_WINOGRAD", "1") != "0"
-        self.wino_min_c = int(os.environ.get("BBDM_WINO_MIN_C", "256"))
-        # ... and at least this many 4x4 tiles per launch: below it the 36 position GEMMs have too few M tiles each
-        # (measured: cfg1, 256 tiles, graph replay 3.9 -> 4.4 ms with Winograd; cfg3, 2048 tiles, 20.2 -> 17.1 ms)
-        self.wino_min_tiles = int(os.environ.get("BBDM_WINO_MIN_TILES", "512"))
+        # Winograd F(4x4,3x3) convs (parity mode only); the thresholds per executor, defaults from convs
+        self.wino = precision == "split3" and convs.WINOGRAD
+        self.wino_min_c, self.wino_min_tiles = convs.WINO_MIN_C, convs.WINO_MIN_TILES
         self._wino_geom = {}
 
     def _umma_ok(self, cin, cout, w):
@@ -130,38 +121,83 @@ class KernelExecutor:
 
     def _conv(self, pool, ent, *, a_f32=None, a_hi=None, a_lo=None, shape, bias=None, residual=None,
               res_mode=cabi.RES_NONE, second=None, out_split=False, want_f32=True, stride=1, out=None,
-              stats=False):
-        """One convolution.  shape = (B,H,W) of the INPUT; returns (out_f32, out_hi, out_lo)."""
+              stats=False, planes=None, taps=None, upsample2x=False):
+        """One convolution.  shape = (B,H,W) of the INPUT; returns (out_f32, out_hi, out_lo).  On the tensor-core
+        path planes = (w_hi, w_lo) [taps][Cout][Cin] replaces the entry's hi/lo (e.g. its up-phase planes), and
+        upsample2x runs the fused nearest-2x conv (output at twice the input's resolution)."""
         B, H, W = shape
-        cout, cin, k = ent["cout"], ent["cin"], ent["k"]
         bias = ent["bias"] if bias is None else bias
         if a_hi is not None:
+            w_hi, w_lo = (ent["hi"], ent["lo"]) if planes is None else planes
+            taps = ent["k"] ** 2 if taps is None else taps
+            cout, cin = w_hi.shape[1], w_hi.shape[2]
+            f = 2 if upsample2x else 1
+            oshape = (B, f * H, f * W, cout)
             if out is None:
-                out = pool.get((B, H, W, cout)) if want_f32 else None
+                out = pool.get(oshape) if want_f32 else None
             oh = ol = None
             if out_split:
-                oh, ol = pool.get((B, H, W, cout), torch.bfloat16), pool.get((B, H, W, cout), torch.bfloat16)
+                oh, ol = pool.get(oshape, torch.bfloat16), pool.get(oshape, torch.bfloat16)
             kw = {}
             if second is not None:
                 e2, r_hi, r_lo = second
                 kw = dict(Cin2=e2["cin"], a2_hi=r_hi, a2_lo=r_lo, w2_hi=e2["hi"], w2_lo=e2["lo"], bias2=e2["bias"])
             part = None
             if stats and out is not None:
-                rows = self._geom(H, W)
+                rows = f * f * self._geom(H, W)
                 if rows:
                     part = pool.get((B * rows, cout, 2))
-            self.be.conv_umma(B=B, H=H, W=W, Cin=cin, Cout=cout, taps=k * k, a_hi=a_hi, a_lo=a_lo,
-                              w_hi=ent["hi"], w_lo=ent["lo"], bias=bias, residual=residual, res_mode=res_mode,
-                              out=out, out_hi=oh, out_lo=ol, passes=self.passes, stats_partial=part, **kw)
+            self.be.conv_umma(B=B, H=H, W=W, Cin=cin, Cout=cout, taps=taps, a_hi=a_hi, a_lo=a_lo, w_hi=w_hi,
+                              w_lo=w_lo, bias=bias, residual=residual, res_mode=res_mode, out=out, out_hi=oh,
+                              out_lo=ol, passes=self.passes, stats_partial=part, upsample2x=upsample2x, **kw)
             if part is not None:
                 out._gn = (part, rows)
             return out, oh, ol
         assert second is None and res_mode in (cabi.RES_NONE, cabi.RES_SAME) and not out_split
+        cout, k = ent["cout"], ent["k"]
         Ho, Wo = (H + stride - 1) // stride, (W + stride - 1) // stride
         if out is None:
             out = pool.get((B, Ho, Wo, cout))
         self.be.conv_direct(a_f32, ent["f32"], bias, residual, out, cout, k, stride)
         return out, None, None
+
+    def _gn_act(self, pool, x, norm, umma, silu=True, want_raw_split=False, eps=None):
+        """GroupNorm (+ SiLU) of x as a conv operand: (a_f32, a_hi, a_lo, raw_hi, raw_lo)."""
+        mean, rstd = self._stats(pool, x, None, eps=eps)
+        a_f32 = a_hi = a_lo = r_hi = r_lo = None
+        if umma:
+            a_hi, a_lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
+        else:
+            a_f32 = pool.get(x.shape)
+        if want_raw_split:
+            r_hi, r_lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
+        self.be.prep(x, None, groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=norm.weight.detach(),
+                     beta=norm.bias.detach(), silu=silu, resample=cabi.RESAMPLE_NONE, act_f32=a_f32, act_hi=a_hi,
+                     act_lo=a_lo, raw_hi=r_hi, raw_lo=r_lo)
+        pool.put(mean, rstd)
+        return a_f32, a_hi, a_lo, r_hi, r_lo
+
+    def _padded_head(self, pool, h, norm, ent, out):
+        """GroupNorm -> SiLU -> 3x3 conv with Cout < 64 on the tensor-core path: the N tile is zero-padded to 64
+        couts and the epilogue stores the real ones into the NCHW tensor out."""
+        B, H, W, _ = h.shape
+        _, a_hi, a_lo, _, _ = self._gn_act(pool, h, norm, True)
+        self.be.conv_umma(B=B, H=H, W=W, Cin=ent["cin"], Cout=64, taps=9, a_hi=a_hi, a_lo=a_lo, w_hi=ent["hi_pad"],
+                          w_lo=ent["lo_pad"], bias=ent["bias_pad"], out=out, passes=self.passes,
+                          out_nchw_channels=out.shape[1])
+        pool.put(a_hi, a_lo)
+        return out
+
+    def _skip_residual(self, pool, es, src1, id_mode, r_f32, r_hi, r_lo, shape):
+        """The ResBlock skip path as conv2's residual: (residual, res_mode, skip output to release).  The skip conv es
+        runs on the raw input's split planes (tensor-core GEMM) or its fp32 copy; without a skip conv the residual is
+        the raw fp32 input if prep wrote one, else src1 itself, resampled by conv2's epilogue (id_mode)."""
+        if es is not None:
+            skip, _, _ = self._conv(pool, es, a_f32=r_f32, a_hi=r_hi, a_lo=r_lo, shape=shape)
+            return skip, cabi.RES_SAME, skip
+        if r_f32 is not None:
+            return r_f32, cabi.RES_SAME, None
+        return src1, id_mode, None
 
     def _geom(self, H, W):
         key = (H, W)
@@ -180,40 +216,21 @@ class KernelExecutor:
         return g
 
     def _wino_ok(self, ent, B, H, W):
-        if not (self.wino and "u_hi" in ent):
-            return False
-        # >= 128 tiles per image: always (the choice must not depend on the batch size there -- batch-size independent,
-        # bit-identical results at the pixel resolutions); smaller maps: only when the whole batch has enough tiles
-        th, tw, tiles, ok = self._wino_geometry(B, H, W)
-        return bool(ok and (th * tw >= 128 or tiles >= self.wino_min_tiles))
+        return self.wino and "u_hi" in ent and convs.winograd_ok(self._wino_geometry(B, H, W), ent["cin"], ent["cout"],
+                                                                 self.wino_min_c, self.wino_min_tiles)
 
-    def _wino_conv(self, pool, ent, src1, src2, *, mean, rstd, gamma, beta, film=None, silu=True, raw=None,
-                   residual=None, res_mode=cabi.RES_NONE, stats=True):
-        """GroupNorm-affine(+FiLM)+SiLU -> 3x3 conv (+bias, +residual) of cat(src1, src2) on the Winograd path:
-        input transform -> 36 position GEMMs in one wgmma launch -> output transform (+ GN partial sums).
-        raw = (r_hi, r_lo): also emit the raw input's split-bf16 planes (operand of a 1x1 skip conv)."""
-        be = self.be
+    def _wino_ready(self, ent):
+        """Whether refresh_weights gives the packed conv ent Winograd planes."""
+        return self.wino and "hi" in ent and ent["k"] == 3 and convs.wino_channels_ok(ent["cin"], ent["cout"],
+                                                                                     self.wino_min_c)
+
+    def _wino_conv(self, pool, ent, src1, src2, *, residual=None, res_mode=cabi.RES_NONE, **transform):
+        """GroupNorm-affine(+FiLM)+SiLU -> 3x3 conv (+bias, +residual, GN partial sums) of cat(src1, src2) on the
+        Winograd path with the entry's planes; transform: the wino_input arguments (groups, mean, rstd, ...)."""
         B, H, W, _ = src1.shape
-        cin, cout = ent["cin"], ent["cout"]
-        th, tw, mtot, _ = self._wino_geometry(B, H, W)
-        v_hi, v_lo = pool.get((36, mtot, cin), torch.float16), pool.get((36, mtot, cin), torch.float16)
-        fkw = {} if film is None else dict(film_scale=film[0], film_shift=film[1], film_stride=film[2])
-        rkw = {} if raw is None else dict(raw_hi=raw[0], raw_lo=raw[1])
-        be.wino_input(src1, src2, groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=gamma, beta=beta, silu=silu,
-                      v_hi=v_hi, v_lo=v_lo, **fkw, **rkw)
-        mbuf = pool.get((36, mtot, cout))
-        be.conv_umma(B=36, H=mtot // 16, W=16, Cin=cin, Cout=cout, taps=1, a_hi=v_hi, a_lo=v_lo, w_hi=ent["u_hi"],
-                     w_lo=ent["u_lo"], out=mbuf, passes=3, weights_per_image=True, operand_f16=True)
-        pool.put(v_hi, v_lo)
-        out = pool.get((B, H, W, cout))
-        part = pool.get((B * th, cout, 2)) if stats else None
-        skw = {} if ent.get("u_inv") is None else dict(inv_wscale=ent["u_inv"])
-        be.wino_output(mbuf, B=B, H=H, W=W, Cout=cout, bias=ent["bias"], residual=residual, res_mode=res_mode,
-                       out=out, stats_partial=part, **skw)
-        pool.put(mbuf)
-        if part is not None:
-            out._gn = (part, th)
-        return out
+        return convs.wino_conv(self.be, pool, self._wino_geometry(B, H, W), src1, src2, cout=ent["cout"],
+                               planes=(ent["u_hi"], ent["u_lo"], ent.get("u_inv")), bias=ent["bias"],
+                               residual=residual, res_mode=res_mode, stats=True, **transform)
 
 
 class UNetEngine(KernelExecutor):
@@ -224,7 +241,6 @@ class UNetEngine(KernelExecutor):
         self._w = {}
         self._table = None
         self.num_timesteps = 1000
-        self.attention_impl = "tcgen05"      # "mma.sync" selects bbdm_attention_split for head_dim 64/128 too
         self.generation = 0          # bumps whenever cache/parameter ADDRESSES change (graphs key on it)
 
     # ------------------------------------------------------------------------------ weights
@@ -251,52 +267,14 @@ class UNetEngine(KernelExecutor):
         old = self._w or {}
         if self._ptrs(key) != self._ptrs(self._wkey) or not self._w:
             self.generation += 1
-        w = {}
-
-        def buf(name, field, shape, dtype):
-            t = old.get(name, {}).get(field) if isinstance(old.get(name), dict) else None
-            if t is not None and tuple(t.shape) == tuple(shape) and t.device == dev:
-                return t
-            return be.empty(tuple(shape), dtype, dev)
-
-        def pack(conv, name):
-            pack_tensor(conv.weight, conv.bias, name)
-
-        def pack_tensor(weight, bias, name):
-            wt = weight.detach()
-            while wt.dim() < 4:                     # Conv1d [Cout, Cin, 1], Linear [out, in]
-                wt = wt.unsqueeze(-1)
-            wt = wt.contiguous()
-            cout, cin, k = wt.shape[0], wt.shape[1], wt.shape[2]
-            ent = {"cout": cout, "cin": cin, "k": k, "bias": bias.detach() if bias is not None else None}
-            if cin % 64 == 0 and cout % 64 == 0 and k in (1, 3):
-                hi = buf(name, "hi", (k * k, cout, cin), torch.bfloat16)
-                lo = buf(name, "lo", (k * k, cout, cin), torch.bfloat16)
-                be.pack_weight_split(wt, hi, lo)
-                ent["hi"], ent["lo"] = hi, lo
-            elif name == "out.2" and cin % 64 == 0 and cout < 64 and k == 3:
-                # UNet head (Cout = 3..16): zero-padded to one 64-wide N tile of the tensor-core conv
-                prev = old[name].get("hi_pad") if isinstance(old.get(name), dict) else None
-                hi = buf(name, "hi_pad", (k * k, 64, cin), torch.bfloat16)
-                lo = buf(name, "lo_pad", (k * k, 64, cin), torch.bfloat16)
-                made = hi is not prev                 # freshly allocated: the padding rows must be zeroed
-                bp = buf(name, "bias_pad", (64,), torch.float32)
-                if made:
-                    hi.zero_(); lo.zero_()
-                bp.zero_()
-                if bias is not None:
-                    bp[:cout].copy_(bias.detach())
-                be.pack_weight_split(wt, hi, lo)
-                ent["hi_pad"], ent["lo_pad"], ent["bias_pad"] = hi, lo, bp
-            f32 = buf(name, "f32", (k * k, cin, cout), torch.float32)
-            be.pack_weight_f32(wt, f32)
-            ent["f32"] = f32
-            w[name] = ent
+        packer = convs.WeightPacker(be, dev, old)
+        w = packer.w
 
         film_w, film_b, off = [], [], 0
         for name, m in u.named_modules():
             if isinstance(m, (nn.Conv2d, nn.Conv1d)):
-                pack(m, name)
+                # out.2 is the UNet head (Cout = 3..16): zero-padded to one 64-wide N tile of the tensor-core conv
+                packer.conv(name, m.weight, m.bias, padded_head=(name == "out.2"))
             if isinstance(m, ResBlock):
                 lin = m.emb_layers[1]
                 n = lin.weight.shape[0]
@@ -317,40 +295,24 @@ class UNetEngine(KernelExecutor):
                 for j, blk in enumerate(m.transformer_blocks):
                     pre = f"{name}.transformer_blocks.{j}"
                     a1, a2 = blk.attn1, blk.attn2
-                    pack_tensor(torch.cat([a1.to_q.weight, a1.to_k.weight, a1.to_v.weight], 0), None, pre + ".attn1.qkv")
-                    pack_tensor(a1.to_out[0].weight, a1.to_out[0].bias, pre + ".attn1.to_out.0")
-                    pack_tensor(a2.to_q.weight, None, pre + ".attn2.to_q")
-                    pack_tensor(torch.cat([a2.to_k.weight, a2.to_v.weight], 0), None, pre + ".attn2.to_kv")
-                    pack_tensor(a2.to_out[0].weight, a2.to_out[0].bias, pre + ".attn2.to_out.0")
-                    pack_tensor(blk.ff.net[0].proj.weight, blk.ff.net[0].proj.bias, pre + ".ff.net.0.proj")
-                    pack_tensor(blk.ff.net[2].weight, blk.ff.net[2].bias, pre + ".ff.net.2")
-        if self.wino:
-            # stride-1 3x3 ResBlock convs: Winograd-domain weight planes U = s G g G^T, fp16 hi/lo [36][Cout][Cin], and
-            # 1/s (per-tensor power of two) as a device scalar beside them: a stable address for graph replay
-            for name, m in u.named_modules():
-                if not isinstance(m, ResBlock) or not m.use_scale_shift_norm:
-                    continue
-                for cname, conv, skip in ((name + ".in_layers.2", m.in_layers[2], m.up or m.down),
-                                          (name + ".out_layers.3", m.out_layers[3], False)):
-                    ent = w[cname]
-                    if skip or "hi" not in ent or ent["k"] != 3 or min(ent["cin"], ent["cout"]) < self.wino_min_c:
-                        continue
-                    uh = buf(cname, "u_hi", (36, ent["cout"], ent["cin"]), torch.float16)
-                    ul = buf(cname, "u_lo", (36, ent["cout"], ent["cin"]), torch.float16)
-                    skw = {}
-                    if getattr(be, "wino_tensor_scale", False):
-                        ent["u_inv"] = skw["inv_wscale"] = buf(cname, "u_inv", (1,), torch.float32)
-                    be.wino_pack_weight(conv.weight.detach().contiguous(), uh, ul, **skw)
-                    ent["u_hi"], ent["u_lo"] = uh, ul
+                    packer.conv(pre + ".attn1.qkv", torch.cat([a1.to_q.weight, a1.to_k.weight, a1.to_v.weight], 0), None)
+                    packer.conv(pre + ".attn1.to_out.0", a1.to_out[0].weight, a1.to_out[0].bias)
+                    packer.conv(pre + ".attn2.to_q", a2.to_q.weight, None)
+                    packer.conv(pre + ".attn2.to_kv", torch.cat([a2.to_k.weight, a2.to_v.weight], 0), None)
+                    packer.conv(pre + ".attn2.to_out.0", a2.to_out[0].weight, a2.to_out[0].bias)
+                    packer.conv(pre + ".ff.net.0.proj", blk.ff.net[0].proj.weight, blk.ff.net[0].proj.bias)
+                    packer.conv(pre + ".ff.net.2", blk.ff.net[2].weight, blk.ff.net[2].bias)
+        for name, m in u.named_modules():
+            # Winograd planes for the stride-1 3x3 convs of the scale-shift ResBlocks
+            if isinstance(m, ResBlock) and m.use_scale_shift_norm:
+                for cname, conv, resampled in ((name + ".in_layers.2", m.in_layers[2], m.up or m.down),
+                                               (name + ".out_layers.3", m.out_layers[3], False)):
+                    if not resampled and self._wino_ready(w[cname]):
+                        packer.winograd(cname, conv.weight)
         for name, m in u.named_modules():
             if isinstance(m, ResBlock) and m.up and m.channels % 64 == 0 and m.out_channels % 64 == 0:
                 # up-ResBlock in_layers conv: 16 phase taps of the fused nearest-2x + 3x3 conv
-                cname = name + ".in_layers.2"
-                wp = upsample_phase_weights(m.in_layers[2].weight.detach())
-                ph = buf(cname, "up_hi", (16, m.out_channels, m.channels), torch.bfloat16)
-                pl = buf(cname, "up_lo", (16, m.out_channels, m.channels), torch.bfloat16)
-                be.pack_weight_split_taps(wp, ph, pl)
-                w[cname]["up_hi"], w[cname]["up_lo"] = ph, pl
+                packer.up_phase(name + ".in_layers.2", m.in_layers[2].weight)
         if old and old.get("film_n") == off and old["film_w"].device == dev:
             w["film_w"], w["film_b"] = old["film_w"], old["film_b"]
             torch.cat(film_w, 0, out=w["film_w"])
@@ -386,137 +348,95 @@ class UNetEngine(KernelExecutor):
         assert cin == m.channels
         resample = cabi.RESAMPLE_UP2 if m.up else (cabi.RESAMPLE_DOWN2 if m.down else cabi.RESAMPLE_NONE)
         H, W = (Hs * 2, Ws * 2) if m.up else ((Hs // 2, Ws // 2) if m.down else (Hs, Ws))
+        shape, shp = (B, H, W), (B, H, W, cin)
         e1, e2 = w[name + ".in_layers.2"], w[name + ".out_layers.3"]
         skip_conv = isinstance(m.skip_connection, nn.Conv2d)
         es = w[name + ".skip_connection"] if skip_conv else None
         umma1 = self._umma_ok(cin, cout, W)
         umma2 = self._umma_ok(cout, cout, W)
+        # a 1x1 skip conv rides as extra K-blocks of conv2 (or, before a Winograd conv2, as its own GEMM) on the raw
+        # input's split planes; any other skip that is not plain src1 needs the raw (resampled / concatenated) input
         fuse_skip = skip_conv and umma2 and es["k"] == 1 and cin % 64 == 0
         need_raw_f32 = (skip_conv and not fuse_skip) or \
                        (not skip_conv and (src2 is not None or (resample != cabi.RESAMPLE_NONE and not umma2)))
         foff, fn = w[name + "#film"]
+        r_f32 = r_hi = r_lo = None
 
-        # ---- in_layers: GN -> SiLU -> (up/down) -> conv3x3 -------------------------------------
+        # ---- conv1: GN -> SiLU -> (up/down) -> conv3x3 ---------------------------------------------------------
         mean, rstd = self._stats(pool, src1, src2)
         gn = m.in_layers[0]
-        # up-ResBlock on the tensor-core path: never materialise the upsampled activation -- the
-        # conv runs as 4 output phases x 2x2 taps on the low-res operand (2.25x fewer MACs)
-        fused_up = bool(m.up and umma1 and "up_hi" in e1 and Ws >= 4 and m.use_scale_shift_norm
-                        and not need_raw_f32 and not fuse_skip)
-        if fused_up:
+        gkw = dict(groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=gn.weight.detach(), beta=gn.bias.detach(), silu=True)
+        if m.up and umma1 and "up_hi" in e1 and Ws >= 4 and m.use_scale_shift_norm and not need_raw_f32 \
+                and not fuse_skip:
+            # up-ResBlock on the tensor-core path: never materialise the upsampled activation -- the conv runs as
+            # 4 output phases x 2x2 taps on the low-res operand (2.25x fewer MACs)
             a_hi, a_lo = pool.get((B, Hs, Ws, cin), torch.bfloat16), pool.get((B, Hs, Ws, cin), torch.bfloat16)
-            be.prep(src1, src2, groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=gn.weight.detach(),
-                    beta=gn.bias.detach(), silu=True, resample=cabi.RESAMPLE_NONE, act_hi=a_hi, act_lo=a_lo)
+            be.prep(src1, src2, **gkw, resample=cabi.RESAMPLE_NONE, act_hi=a_hi, act_lo=a_lo)
             pool.put(mean, rstd)
-            h1 = pool.get((B, H, W, cout))
-            rows = 4 * self._geom(Hs, Ws)
-            part = pool.get((B * rows, cout, 2)) if rows else None
-            be.conv_umma(B=B, H=Hs, W=Ws, Cin=cin, Cout=cout, taps=4, a_hi=a_hi, a_lo=a_lo, w_hi=e1["up_hi"],
-                         w_lo=e1["up_lo"], bias=e1["bias"], out=h1, passes=self.passes, upsample2x=True,
-                         stats_partial=part)
-            if part is not None:
-                h1._gn = (part, rows)
+            h1, _, _ = self._conv(pool, e1, a_hi=a_hi, a_lo=a_lo, shape=(B, Hs, Ws), planes=(e1["up_hi"], e1["up_lo"]),
+                                  taps=4, upsample2x=True, stats=True)
             pool.put(a_hi, a_lo)
-            return self._resblock_tail(pool, name, m, src1, h1, film, foff, cout, (B, H, W), e2, es, umma2,
-                                       None, cabi.RES_UP2, None, None, None)
-        shp = (B, H, W, cin)
-        a_f32 = a_hi = a_lo = r_f32 = r_hi = r_lo = None
-        if umma1 and resample == cabi.RESAMPLE_NONE and not need_raw_f32 and m.use_scale_shift_norm \
+        elif umma1 and resample == cabi.RESAMPLE_NONE and not need_raw_f32 and m.use_scale_shift_norm \
                 and self._wino_ok(e1, B, H, W):
             # Winograd conv1; the raw split planes for a fused 1x1 skip come out of the same input pass
             if fuse_skip:
                 r_hi, r_lo = pool.get(shp, torch.bfloat16), pool.get(shp, torch.bfloat16)
-            h1 = self._wino_conv(pool, e1, src1, src2, mean=mean, rstd=rstd, gamma=gn.weight.detach(),
-                                 beta=gn.bias.detach(), raw=(r_hi, r_lo) if fuse_skip else None)
+            h1 = self._wino_conv(pool, e1, src1, src2, **gkw, raw_hi=r_hi, raw_lo=r_lo)
             pool.put(mean, rstd)
-            return self._resblock_tail(pool, name, m, src1, h1, film, foff, cout, (B, H, W), e2, es, umma2,
-                                       (es, r_hi, r_lo) if fuse_skip else None, resample_to_res(resample),
-                                       None, r_hi, r_lo, skip_conv=skip_conv, need_raw_f32=False)
-        if umma1:
-            a_hi, a_lo = pool.get(shp, torch.bfloat16), pool.get(shp, torch.bfloat16)
         else:
-            a_f32 = pool.get(shp)
-        if fuse_skip:
-            r_hi, r_lo = pool.get(shp, torch.bfloat16), pool.get(shp, torch.bfloat16)
-        if need_raw_f32:
-            r_f32 = pool.get(shp)
-        be.prep(src1, src2, groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=gn.weight.detach(), beta=gn.bias.detach(),
-                silu=True, resample=resample, act_f32=a_f32, act_hi=a_hi, act_lo=a_lo,
-                raw_f32=r_f32, raw_hi=r_hi, raw_lo=r_lo)
-        pool.put(mean, rstd)
-        if m.use_scale_shift_norm:
-            h1, _, _ = self._conv(pool, e1, a_f32=a_f32, a_hi=a_hi, a_lo=a_lo, shape=(B, H, W), stats=True)
-        else:
-            # conv1 + (bias + emb_out[b]) per sample: per-sample bias rows live in `film`
-            h1 = pool.get((B, H, W, cout))
-            for b in range(B):
-                sl = lambda z: None if z is None else z[b:b + 1]
-                self._conv(pool, e1, a_f32=sl(a_f32), a_hi=sl(a_hi), a_lo=sl(a_lo), shape=(1, H, W),
-                           bias=film[b, foff:foff + fn], out=h1[b:b + 1])
-        pool.put(a_f32, a_hi, a_lo)
+            a_f32 = a_hi = a_lo = None
+            if umma1:
+                a_hi, a_lo = pool.get(shp, torch.bfloat16), pool.get(shp, torch.bfloat16)
+            else:
+                a_f32 = pool.get(shp)
+            if fuse_skip:
+                r_hi, r_lo = pool.get(shp, torch.bfloat16), pool.get(shp, torch.bfloat16)
+            if need_raw_f32:
+                r_f32 = pool.get(shp)
+            be.prep(src1, src2, **gkw, resample=resample, act_f32=a_f32, act_hi=a_hi, act_lo=a_lo,
+                    raw_f32=r_f32, raw_hi=r_hi, raw_lo=r_lo)
+            pool.put(mean, rstd)
+            if m.use_scale_shift_norm:
+                h1, _, _ = self._conv(pool, e1, a_f32=a_f32, a_hi=a_hi, a_lo=a_lo, shape=shape, stats=True)
+            else:
+                # conv1 + (bias + emb_out[b]) per sample: per-sample bias rows live in `film`
+                h1 = pool.get((B, H, W, cout))
+                for b in range(B):
+                    sl = lambda z: None if z is None else z[b:b + 1]
+                    self._conv(pool, e1, a_f32=sl(a_f32), a_hi=sl(a_hi), a_lo=sl(a_lo), shape=(1, H, W),
+                               bias=film[b, foff:foff + fn], out=h1[b:b + 1])
+            pool.put(a_f32, a_hi, a_lo)
 
-        if fuse_skip:
-            second_args = (es, r_hi, r_lo)
-        else:
-            second_args = None
-        return self._resblock_tail(pool, name, m, src1, h1, film, foff, cout, (B, H, W), e2, es, umma2,
-                                   second_args, resample_to_res(resample), r_f32, r_hi, r_lo,
-                                   skip_conv=skip_conv, need_raw_f32=need_raw_f32)
-
-    def _resblock_tail(self, pool, name, m, src1, h1, film, foff, cout, shape, e2, es, umma2, second, id_res_mode,
-                       r_f32, r_hi, r_lo, skip_conv=False, need_raw_f32=False):
-        """out_layers of a ResBlock: GN (+FiLM) -> SiLU -> conv3x3 with the skip path fused in."""
-        be = self.be
-        B, H, W = shape
-        # ---- out_layers: GN (+FiLM) -> SiLU -> conv3x3 (+skip) -----------------------------------
+        # ---- conv2: GN (+FiLM) -> SiLU -> conv3x3 (+skip) ------------------------------------------------------
         mean, rstd = self._stats(pool, h1, None)
         gn2 = m.out_layers[0]
-        shp2 = (B, H, W, cout)
-        b_f32 = b_hi = b_lo = None
+        gkw = dict(groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=gn2.weight.detach(), beta=gn2.bias.detach(), silu=True)
+        if m.use_scale_shift_norm:
+            gkw.update(film_scale=film[:, foff:foff + cout], film_shift=film[:, foff + cout:foff + 2 * cout],
+                       film_stride=film.shape[1])
+        id_mode = resample_to_res(resample)
         if umma2 and m.use_scale_shift_norm and self._wino_ok(e2, B, H, W):
             # Winograd conv2: the 1x1 skip (if any) runs as its own tensor-core GEMM and enters as the residual
-            residual, res_mode, skip_out = None, cabi.RES_NONE, None
-            if second is not None:
-                skip_out, _, _ = self._conv(pool, second[0], a_hi=second[1], a_lo=second[2], shape=(B, H, W))
-                residual, res_mode = skip_out, cabi.RES_SAME
-            elif skip_conv:
-                skip_out, _, _ = self._conv(pool, es, a_f32=r_f32, shape=(B, H, W))
-                residual, res_mode = skip_out, cabi.RES_SAME
-            elif need_raw_f32:
-                residual, res_mode = r_f32, cabi.RES_SAME
+            residual, res_mode, skip_out = self._skip_residual(pool, es, src1, id_mode, r_f32, r_hi, r_lo, shape)
+            out = self._wino_conv(pool, e2, h1, None, **gkw, residual=residual, res_mode=res_mode)
+            pool.put(mean, rstd, h1)
+        else:
+            b_f32 = b_hi = b_lo = None
+            if umma2:
+                b_hi, b_lo = pool.get((B, H, W, cout), torch.bfloat16), pool.get((B, H, W, cout), torch.bfloat16)
             else:
-                residual, res_mode = src1, id_res_mode
-            out = self._wino_conv(pool, e2, h1, None, mean=mean, rstd=rstd, gamma=gn2.weight.detach(),
-                                  beta=gn2.bias.detach(),
-                                  film=(film[:, foff:foff + cout], film[:, foff + cout:foff + 2 * cout], film.shape[1]),
-                                  residual=residual, res_mode=res_mode)
-            pool.put(mean, rstd, h1, r_f32, r_hi, r_lo, skip_out)
-            return out
-        if umma2:
-            b_hi, b_lo = pool.get(shp2, torch.bfloat16), pool.get(shp2, torch.bfloat16)
-        else:
-            b_f32 = pool.get(shp2)
-        fkw = {}
-        if m.use_scale_shift_norm:
-            fkw = dict(film_scale=film[:, foff:foff + cout], film_shift=film[:, foff + cout:foff + 2 * cout],
-                       film_stride=film.shape[1])
-        be.prep(h1, None, groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=gn2.weight.detach(), beta=gn2.bias.detach(),
-                silu=True, resample=cabi.RESAMPLE_NONE, act_f32=b_f32, act_hi=b_hi, act_lo=b_lo, **fkw)
-        pool.put(mean, rstd, h1)
-
-        residual, res_mode, skip_out = None, cabi.RES_NONE, None
-        if second is not None:
-            pass
-        elif skip_conv:
-            skip_out, _, _ = self._conv(pool, es, a_f32=r_f32, shape=(B, H, W))
-            residual, res_mode = skip_out, cabi.RES_SAME
-        elif need_raw_f32:
-            residual, res_mode = r_f32, cabi.RES_SAME
-        else:
-            residual, res_mode = src1, id_res_mode
-        out, _, _ = self._conv(pool, e2, a_f32=b_f32, a_hi=b_hi, a_lo=b_lo, shape=(B, H, W),
-                               residual=residual, res_mode=res_mode, second=second, stats=True)
-        pool.put(b_f32, b_hi, b_lo, r_f32, r_hi, r_lo, skip_out)
+                b_f32 = pool.get((B, H, W, cout))
+            be.prep(h1, None, **gkw, resample=cabi.RESAMPLE_NONE, act_f32=b_f32, act_hi=b_hi, act_lo=b_lo)
+            pool.put(mean, rstd, h1)
+            if fuse_skip:
+                second, residual, res_mode, skip_out = (es, r_hi, r_lo), None, cabi.RES_NONE, None
+            else:
+                second = None
+                residual, res_mode, skip_out = self._skip_residual(pool, es, src1, id_mode, r_f32, r_hi, r_lo, shape)
+            out, _, _ = self._conv(pool, e2, a_f32=b_f32, a_hi=b_hi, a_lo=b_lo, shape=shape, residual=residual,
+                                   res_mode=res_mode, second=second, stats=True)
+            pool.put(b_f32, b_hi, b_lo)
+        pool.put(r_f32, r_hi, r_lo, skip_out)
         return out
 
     def _attention(self, pool, name, m: AttentionBlock, x):
@@ -526,19 +446,10 @@ class UNetEngine(KernelExecutor):
         eq, ep = w[name + ".qkv"], w[name + ".proj_out"]
         heads = m.num_heads
         hd = Cc // heads
-        if hd not in ATTN_HEAD_DIMS:
+        if hd not in cabi.ATTN_HEAD_DIMS:
             raise NotImplementedError(f"attention head_dim {hd}: the sm_90a kernels support 16/32/64/128")
         umma = self._umma_ok(Cc, Cc, W)
-        mean, rstd = self._stats(pool, x, None)
-        a_f32 = a_hi = a_lo = None
-        if umma:
-            a_hi, a_lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
-        else:
-            a_f32 = pool.get(x.shape)
-        be.prep(x, None, groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=m.norm.weight.detach(),
-                beta=m.norm.bias.detach(), silu=False, resample=cabi.RESAMPLE_NONE,
-                act_f32=a_f32, act_hi=a_hi, act_lo=a_lo)
-        pool.put(mean, rstd)
+        a_f32, a_hi, a_lo, _, _ = self._gn_act(pool, x, m.norm, umma, silu=False)
         # qkv 1x1: on the tensor-core path its epilogue writes the split planes the attention core reads
         qkv, q_hi, q_lo = self._conv(pool, eq, a_f32=a_f32, a_hi=a_hi, a_lo=a_lo, shape=(B, H, W),
                                      out_split=umma, want_f32=not umma)
@@ -548,7 +459,7 @@ class UNetEngine(KernelExecutor):
         if umma:
             o_hi, o_lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
             # head_dim 64 (all templates) or 128: warp-specialised wgmma kernel; else the mma.sync one
-            attn = be.attention_tc if (hd in ATTN_TC_HEAD_DIMS and self.attention_impl == "tcgen05") else be.attention_split
+            attn = be.attention_tc if hd in cabi.ATTN_TC_HEAD_DIMS else be.attention_split
             attn(q_hi.view(B, T, 3 * Cc), q_lo.view(B, T, 3 * Cc), heads, order,
                  None, o_hi.view(B, T, Cc), o_lo.view(B, T, Cc))
         else:
@@ -584,17 +495,13 @@ class UNetEngine(KernelExecutor):
         B, H, W, Cc = x.shape
         T, heads, d = H * W, m.n_heads, m.d_head
         inner = heads * d
-        if d not in ATTN_HEAD_DIMS:
+        if d not in cabi.ATTN_HEAD_DIMS:
             raise NotImplementedError(f"SpatialTransformer head_dim {d}: the sm_90a attention kernels take 16/32/64/128")
         if not (self._umma_ok(Cc, inner, W) and inner % 64 == 0):
             raise NotImplementedError("SpatialTransformer: channel counts must be multiples of 64 (tensor-core GEMMs)")
         bf = torch.bfloat16
         tok = (B, H, W, inner)
-        mean, rstd = self._stats(pool, x, None, eps=m.norm.eps)
-        a_hi, a_lo = pool.get(x.shape, bf), pool.get(x.shape, bf)
-        be.prep(x, None, groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=m.norm.weight.detach(), beta=m.norm.bias.detach(),
-                silu=False, resample=cabi.RESAMPLE_NONE, act_hi=a_hi, act_lo=a_lo)
-        pool.put(mean, rstd)
+        _, a_hi, a_lo, _, _ = self._gn_act(pool, x, m.norm, True, silu=False, eps=m.norm.eps)
         h, _, _ = self._conv(pool, w[name + ".proj_in"], a_hi=a_hi, a_lo=a_lo, shape=(B, H, W))
         pool.put(a_hi, a_lo)
 
@@ -616,7 +523,7 @@ class UNetEngine(KernelExecutor):
                                        want_f32=False)
             pool.put(n_hi, n_lo)
             o_hi, o_lo = pool.get(tok, bf), pool.get(tok, bf)
-            attn = be.attention_tc if (d in ATTN_TC_HEAD_DIMS and self.attention_impl == "tcgen05") else be.attention_split
+            attn = be.attention_tc if d in cabi.ATTN_TC_HEAD_DIMS else be.attention_split
             attn(q_hi.view(B, T, 3 * inner), q_lo.view(B, T, 3 * inner), heads, 1, None, o_hi.view(B, T, inner),
                  o_lo.view(B, T, inner))
             pool.put(q_hi, q_lo)
@@ -753,30 +660,19 @@ class UNetEngine(KernelExecutor):
             h = self._run_block(pool, f"output_blocks.{i}", block, h, hs.pop(), film, release_input=True)
 
         # ---- head: GN -> SiLU -> conv3x3 -> NCHW ----------------------------------------------------
-        mean, rstd = self._stats(pool, h, None)
-        gn = u.out[0]
         if out is None:
             out = torch.empty((B, u.out_channels, H, W), dtype=torch.float32, device=dev)
-        eh = w["out.2"]
+        eh, gn = w["out.2"], u.out[0]
         if "hi_pad" in eh and W >= 4:
-            # tensor-core head: N tile padded to 64 couts, epilogue stores the real ones as NCHW
-            a_hi, a_lo = pool.get(h.shape, torch.bfloat16), pool.get(h.shape, torch.bfloat16)
-            be.prep(h, None, groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=gn.weight.detach(), beta=gn.bias.detach(),
-                    silu=True, resample=cabi.RESAMPLE_NONE, act_hi=a_hi, act_lo=a_lo)
-            pool.put(mean, rstd, h)
-            be.conv_umma(B=B, H=H, W=W, Cin=eh["cin"], Cout=64, taps=9, a_hi=a_hi, a_lo=a_lo, w_hi=eh["hi_pad"],
-                         w_lo=eh["lo_pad"], bias=eh["bias_pad"], out=out, passes=self.passes,
-                         out_nchw_channels=u.out_channels)
-            pool.put(a_hi, a_lo, emb, film, self._ctx_nhwc)
-            self._ctx_nhwc = None
-            return out
-        act = pool.get(h.shape)
-        be.prep(h, None, groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=gn.weight.detach(), beta=gn.bias.detach(),
-                silu=True, resample=cabi.RESAMPLE_NONE, act_f32=act)
-        pool.put(mean, rstd, h)
-        y, _, _ = self._conv(pool, eh, a_f32=act, shape=(B, H, W))
-        pool.put(act)
-        be.nhwc_to_nchw(y, out)
-        pool.put(y, emb, film, self._ctx_nhwc)
+            self._padded_head(pool, h, gn, eh, out)
+            pool.put(h)
+        else:
+            act, _, _, _, _ = self._gn_act(pool, h, gn, False)
+            pool.put(h)
+            y, _, _ = self._conv(pool, eh, a_f32=act, shape=(B, H, W))
+            pool.put(act)
+            be.nhwc_to_nchw(y, out)
+            pool.put(y)
+        pool.put(emb, film, self._ctx_nhwc)
         self._ctx_nhwc = None
         return out

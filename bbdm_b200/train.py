@@ -14,20 +14,17 @@ DDP's bucketed NCCL allreduce works unchanged.
 """
 from __future__ import annotations
 
-import os
-
 import torch
 
-from . import cabi
+from . import cabi, convs
 
 _BACKEND = None
 
 # Winograd F(4x4,3x3) for the forward and data-gradient 3x3 convolutions of the training graph (csrc/winograd.cu;
-# same eligibility rule as the sampling engine).  The weight gradient stays the direct wgmma GEMM.
-WINO_TRAIN = os.environ.get("BBDM_WINOGRAD_TRAIN", "1") != "0"
-WINO_MIN_C = int(os.environ.get("BBDM_WINO_MIN_C", "256"))
-WINO_MIN_TILES = int(os.environ.get("BBDM_WINO_MIN_TILES", "512"))
-
+# same eligibility rule as the sampling engines).  The weight gradient stays the direct wgmma GEMM.
+WINO_TRAIN = convs.WINOGRAD_TRAIN
+WINO_MIN_C = convs.WINO_MIN_C
+WINO_MIN_TILES = convs.WINO_MIN_TILES
 
 _WARNED = set()
 
@@ -45,38 +42,8 @@ def _library_path(what, x):
 
 
 def _wino_ok(be, B, H, W, Cin, Cout, k):
-    if not WINO_TRAIN or k != 3 or min(Cin, Cout) < WINO_MIN_C or Cin % 64 or Cout % 64 or not hasattr(be, "wino_geometry"):
-        return False
-    th, tw, tiles, ok = be.wino_geometry(B, H, W)
-    return bool(ok and (th * tw >= 128 or tiles >= WINO_MIN_TILES))
-
-
-def _wino_conv(be, xn, weight, *, dgrad, gn=None, act_planes=None, bias=None, residual=None, out_channels):
-    """3x3 conv of the NHWC tensor xn on the Winograd path: input transform (GroupNorm affine + FiLM + SiLU fused when
-    gn = dict(mean, rstd, gamma, beta, film_scale, film_shift, film_stride, silu); identity for gn None), 36
-    position GEMMs, output transform (+ bias + residual).  dgrad: use the flipped / channel-swapped kernel."""
-    B, H, W, C = xn.shape
-    dev = xn.device
-    _, _, mt, _ = be.wino_geometry(B, H, W)
-    v_hi = torch.empty((36, mt, C), dtype=torch.float16, device=dev)
-    v_lo = torch.empty_like(v_hi)
-    kw = dict(silu=False) if gn is None else gn
-    akw = {} if act_planes is None else dict(act_hi=act_planes[0], act_lo=act_planes[1])
-    be.wino_input(xn, None, v_hi=v_hi, v_lo=v_lo, **kw, **akw)
-    u_hi = torch.empty((36, out_channels, C), dtype=torch.float16, device=dev)
-    u_lo = torch.empty_like(u_hi)
-    skw = {}
-    if getattr(be, "wino_tensor_scale", False):
-        # per-tensor scale of the planes: 1/s stays on the device (no host synchronisation)
-        skw["inv_wscale"] = torch.empty((1,), dtype=torch.float32, device=dev)
-    be.wino_pack_weight(weight.detach().contiguous(), u_hi, u_lo, dgrad=dgrad, **skw)
-    m = torch.empty((36, mt, out_channels), dtype=torch.float32, device=dev)
-    be.conv_umma(B=36, H=mt // 16, W=16, Cin=C, Cout=out_channels, taps=1, a_hi=v_hi, a_lo=v_lo, w_hi=u_hi, w_lo=u_lo,
-                 out=m, passes=3, weights_per_image=True, operand_f16=True)
-    out = torch.empty((B, H, W, out_channels), dtype=torch.float32, device=dev)
-    be.wino_output(m, B=B, H=H, W=W, Cout=out_channels, bias=bias, residual=residual,
-                   res_mode=cabi.RES_NONE if residual is None else cabi.RES_SAME, out=out, **skw)
-    return out
+    return bool(WINO_TRAIN and k == 3 and hasattr(be, "wino_geometry")
+                and convs.winograd_ok(be.wino_geometry(B, H, W), Cin, Cout, WINO_MIN_C, WINO_MIN_TILES))
 
 
 def backend():
@@ -97,16 +64,20 @@ def _on_device(x: torch.Tensor) -> bool:
     return x.is_cuda or (_BACKEND is not None and not getattr(_BACKEND, "requires_cuda", True))
 
 
-def native_ok(conv: torch.nn.Conv2d, x: torch.Tensor) -> bool:
-    """Shapes the tensor-core fwd/dgrad/wgrad kernels take."""
+def _tc_ok(x: torch.Tensor, cin: int, cout: int) -> bool:
+    """Operands the tensor-core fwd/dgrad/wgrad kernels take: fp32 [B, C, H, W] on the device, channel counts that
+    are multiples of 64, and a pixel grid the 64-pixel tile box covers."""
     if not _on_device(x) or x.dtype != torch.float32 or x.dim() != 4:
         return False
-    k = conv.kernel_size
     B, _, H, W = x.shape
+    return cin % 64 == 0 and cout % 64 == 0 and W >= 4 and (B * H * W) % 64 == 0 and _box64_ok(B, H, W)
+
+
+def native_ok(conv: torch.nn.Conv2d, x: torch.Tensor) -> bool:
+    """Convolutions the tensor-core fwd/dgrad/wgrad kernels take."""
+    k = conv.kernel_size
     return (k in ((1, 1), (3, 3)) and conv.stride == (1, 1) and conv.padding == (k[0] // 2, k[0] // 2)
-            and conv.groups == 1 and conv.dilation == (1, 1)
-            and conv.in_channels % 64 == 0 and conv.out_channels % 64 == 0 and W >= 4
-            and (B * H * W) % 64 == 0 and _box64_ok(B, H, W))
+            and conv.groups == 1 and conv.dilation == (1, 1) and _tc_ok(x, conv.in_channels, conv.out_channels))
 
 
 def _box64_ok(B, H, W):
@@ -197,7 +168,8 @@ def _conv_backward(be, ctx_shape, a_hi, a_lo, weight, dy, need_dx, need_dw, need
         # device (no host synchronisation).
         amax = dyn.abs().amax().clamp_min(2.0 ** -100)
         scale = torch.exp2(4.0 - torch.floor(torch.log2(amax)))
-        dxn = _wino_conv(be, (dyn * scale).contiguous(), weight, dgrad=True, out_channels=Cin)
+        dxn = convs.wino_conv(be, convs.FreshBuffers(dev), be.wino_geometry(B, H, W), (dyn * scale).contiguous(), None,
+                              cout=Cin, weight=weight, dgrad=True, silu=False)
         dxn.mul_(1.0 / scale)
     elif need_dx:
         # data gradient = the same conv with the kernel flipped and Cin/Cout swapped
@@ -244,11 +216,12 @@ class GNActConv2dFn(torch.autograd.Function):
         rn = None if residual is None else _nhwc(residual.detach())       # + skip(x), fused in the epilogue
         if resample == 0 and _wino_ok(be, B, H, W, Cin, Cout, k):
             # Winograd forward; the input transform also writes the activated split planes the weight gradient needs
-            gn = dict(groups=32, mean=mean, rstd=rstd, gamma=gamma.detach(), beta=beta.detach(), film_scale=fs,
-                      film_shift=fh, film_stride=0 if fs is None else fs.shape[1], silu=act)
-            out = _wino_conv(be, xn.contiguous(), weight, dgrad=False, gn=gn, act_planes=(a_hi, a_lo),
-                             bias=None if bias is None else bias.detach(), residual=None if rn is None else rn.contiguous(),
-                             out_channels=Cout)
+            out = convs.wino_conv(be, convs.FreshBuffers(dev), be.wino_geometry(B, H, W), xn.contiguous(), None,
+                                  cout=Cout, weight=weight, bias=None if bias is None else bias.detach(),
+                                  residual=None if rn is None else rn.contiguous(),
+                                  res_mode=cabi.RES_NONE if rn is None else cabi.RES_SAME, groups=32, mean=mean,
+                                  rstd=rstd, gamma=gamma.detach(), beta=beta.detach(), film_scale=fs, film_shift=fh,
+                                  film_stride=0 if fs is None else fs.shape[1], silu=act, act_hi=a_hi, act_lo=a_lo)
             wd_hi = wd_lo = None              # the backward re-derives what it needs (Winograd dgrad planes)
         else:
             be.prep(xn, None, groups=32, mean=mean, rstd=rstd, gamma=gamma.detach(), beta=beta.detach(), film_scale=fs,
@@ -386,11 +359,7 @@ def conv1x1(conv1d: torch.nn.Conv1d, x4: torch.Tensor, enabled: bool = True):
     """nn.Conv1d(k=1) of AttentionBlock (qkv / proj_out, openaimodel.py:307,315) applied to a [B,C,H,W]
     tensor as a 1x1 convolution on the tensor-core autograd path; returns [B,Cout,H,W] or None if the
     shape does not qualify (caller falls back to the module)."""
-    B, C, H, W = x4.shape
-    Cout = conv1d.out_channels
-    ok = (enabled and _on_device(x4) and x4.dtype == torch.float32 and conv1d.kernel_size == (1,) and C % 64 == 0
-          and Cout % 64 == 0 and W >= 4 and (B * H * W) % 64 == 0 and _box64_ok(B, H, W))
-    if not ok:
+    if not (enabled and conv1d.kernel_size == (1,) and _tc_ok(x4, x4.shape[1], conv1d.out_channels)):
         return None
     return Conv2dFn.apply(x4, conv1d.weight.unsqueeze(-1), conv1d.bias)
 
@@ -409,7 +378,7 @@ class AttentionCoreFn(torch.autograd.Function):
         dev = qkv.device
         qn = _nhwc(qkv.detach()).contiguous()
         out = torch.empty((B, T, Cc), dtype=torch.float32, device=dev)
-        if Cc // heads in (64, 128):
+        if Cc // heads in cabi.ATTN_TC_HEAD_DIMS:
             q_hi = torch.empty((B, H, W, C3), dtype=torch.bfloat16, device=dev)
             q_lo = torch.empty_like(q_hi)
             be.prep(qn, None, raw_hi=q_hi, raw_lo=q_lo)
@@ -440,7 +409,7 @@ def attention_core(qkv4: torch.Tensor, heads: int, new_order: bool, enabled: boo
     """[B,3C,H,W] -> [B,C,H,W] or None when the native kernels do not take the shape."""
     B, C3, H, W = qkv4.shape
     hd = C3 // 3 // heads
-    if not (enabled and _on_device(qkv4) and qkv4.dtype == torch.float32 and hd in (16, 32, 64, 128) and (C3 // 3) % 4 == 0
+    if not (enabled and _on_device(qkv4) and qkv4.dtype == torch.float32 and hd in cabi.ATTN_HEAD_DIMS and (C3 // 3) % 4 == 0
             and B * heads <= 65535):
         return None
     return AttentionCoreFn.apply(qkv4, heads, 1 if new_order else 0)
@@ -449,11 +418,8 @@ def attention_core(qkv4: torch.Tensor, heads: int, new_order: bool, enabled: boo
 def gn_conv1x1(norm, conv1d: torch.nn.Conv1d, x4: torch.Tensor, enabled: bool = True):
     """conv1d_k1(GroupNorm32(x)) of AttentionBlock (openaimodel.py:307,321) fused like gn_act_conv2d, without
     the activation; None if the shape does not qualify."""
-    B, C, H, W = x4.shape
-    Cout = conv1d.out_channels
-    ok = (enabled and _on_device(x4) and x4.dtype == torch.float32 and conv1d.kernel_size == (1,) and C % 64 == 0
-          and Cout % 64 == 0 and W >= 4 and (B * H * W) % 64 == 0 and _box64_ok(B, H, W) and C <= 4096)
-    if not ok:
+    if not (enabled and conv1d.kernel_size == (1,) and _tc_ok(x4, x4.shape[1], conv1d.out_channels)
+            and x4.shape[1] <= 4096):
         return None
     return GNActConv2dFn.apply(x4, norm.weight, norm.bias, None, None, conv1d.weight.unsqueeze(-1), conv1d.bias,
                                0, None, False)

@@ -21,9 +21,8 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
-from . import cabi
+from . import cabi, convs
 from .engine import GN_GROUPS, KernelExecutor
-from .weights import upsample_phase_weights
 
 
 class VQGANEngine(KernelExecutor):
@@ -45,36 +44,14 @@ class VQGANEngine(KernelExecutor):
             return
         be = self.be
         dev = next(self.vq.parameters()).device
-        w = {}
+        packer = convs.WeightPacker(be, dev, self._w)
+        w = packer.w
 
         def pack(name, wt, bias):
-            wt = wt.detach().contiguous()
-            cout, cin, k = wt.shape[0], wt.shape[1], wt.shape[2]
-            ent = {"cout": cout, "cin": cin, "k": k, "bias": None if bias is None else bias.detach().contiguous()}
-            if cin % 64 == 0 and cout % 64 == 0 and k in (1, 3):
-                ent["hi"] = be.empty((k * k, cout, cin), torch.bfloat16, dev)
-                ent["lo"] = be.empty((k * k, cout, cin), torch.bfloat16, dev)
-                be.pack_weight_split(wt, ent["hi"], ent["lo"])
-            elif cin % 64 == 0 and cout < 64 and k == 3:
-                # image head (Cout = 3): zero-padded to one 64-wide N tile, epilogue stores NCHW
-                ent["hi_pad"] = torch.zeros((k * k, 64, cin), dtype=torch.bfloat16, device=dev)
-                ent["lo_pad"] = torch.zeros((k * k, 64, cin), dtype=torch.bfloat16, device=dev)
-                ent["bias_pad"] = torch.zeros((64,), dtype=torch.float32, device=dev)
-                if bias is not None:
-                    ent["bias_pad"][:cout].copy_(bias.detach())
-                be.pack_weight_split(wt, ent["hi_pad"], ent["lo_pad"])
-            ent["f32"] = be.empty((k * k, cin, cout), torch.float32, dev)
-            be.pack_weight_f32(wt, ent["f32"])
-            if self.wino and "hi" in ent and k == 3 and min(cin, cout) >= self.wino_min_c \
-                    and (name.endswith(".conv1") or name.endswith(".conv2")):
-                # ResnetBlock 3x3 convs: Winograd-domain planes (csrc/winograd.cu), like the UNet's ResBlocks
-                ent["u_hi"] = be.empty((36, cout, cin), torch.float16, dev)
-                ent["u_lo"] = be.empty((36, cout, cin), torch.float16, dev)
-                skw = {}
-                if getattr(be, "wino_tensor_scale", False):
-                    ent["u_inv"] = skw["inv_wscale"] = be.empty((1,), torch.float32, dev)
-                be.wino_pack_weight(wt, ent["u_hi"], ent["u_lo"], **skw)
-            w[name] = ent
+            # any 3x3 conv with Cout < 64 is an image head (Cout = 3): NCHW-storing padded planes
+            ent = packer.conv(name, wt, bias, padded_head=True)
+            if (name.endswith(".conv1") or name.endswith(".conv2")) and self._wino_ready(ent):
+                packer.winograd(name, wt)          # ResnetBlock 3x3 convs, like the UNet's ResBlocks
 
         for name, m in self.vq.named_modules():
             if isinstance(m, nn.Conv2d) and not name.startswith("loss"):
@@ -85,11 +62,7 @@ class VQGANEngine(KernelExecutor):
                      torch.cat([m.q.bias, m.k.bias, m.v.bias], 0))
         for name, m in self.vq.named_modules():          # second pass: the convs above are packed now
             if type(m).__name__ == "Upsample" and m.with_conv and "hi" in w.get(name + ".conv", {}):
-                ent = w[name + ".conv"]
-                wp = upsample_phase_weights(m.conv.weight.detach())
-                ent["up_hi"] = be.empty((16, ent["cout"], ent["cin"]), torch.bfloat16, dev)
-                ent["up_lo"] = be.empty((16, ent["cout"], ent["cin"]), torch.bfloat16, dev)
-                be.pack_weight_split_taps(wp, ent["up_hi"], ent["up_lo"])
+                packer.up_phase(name + ".conv", m.conv.weight)
             if type(m).__name__ == "Downsample" and m.with_conv:
                 # stride-2 3x3 conv on the zero-padded input == 2x2-tap conv over the space-to-depth tensor:
                 # W2[tap=(ty,tx)][co][(a*2+b)*C + ci] = w[co][ci][2ty+a][2tx+b]  (zero where 2ty+a or 2tx+b = 3)
@@ -126,22 +99,6 @@ class VQGANEngine(KernelExecutor):
         out, _, _ = self._conv(pool, ent, a_f32=x, shape=(B, H, W), **kw)
         return out
 
-    def _gn_act(self, pool, x, norm, umma, silu=True, want_raw_split=False):
-        """GroupNorm(eps 1e-6) (+ swish) of x as a conv operand: (a_f32, a_hi, a_lo, raw_hi, raw_lo)."""
-        mean, rstd = self._stats(pool, x, None)
-        a_f32 = a_hi = a_lo = r_hi = r_lo = None
-        if umma:
-            a_hi, a_lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
-        else:
-            a_f32 = pool.get(x.shape)
-        if want_raw_split:
-            r_hi, r_lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
-        self.be.prep(x, None, groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=norm.weight.detach(),
-                     beta=norm.bias.detach(), silu=silu, resample=cabi.RESAMPLE_NONE, act_f32=a_f32, act_hi=a_hi,
-                     act_lo=a_lo, raw_hi=r_hi, raw_lo=r_lo)
-        pool.put(mean, rstd)
-        return a_f32, a_hi, a_lo, r_hi, r_lo
-
     def _resnet(self, pool, name, m, x):
         w = self._w
         B, H, W, cin = x.shape
@@ -158,8 +115,8 @@ class VQGANEngine(KernelExecutor):
             if fuse_skip or skip_umma:
                 r_hi, r_lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
             mean, rstd = self._stats(pool, x, None)
-            h1 = self._wino_conv(pool, e1, x, None, mean=mean, rstd=rstd, gamma=m.norm1.weight.detach(),
-                                 beta=m.norm1.bias.detach(), raw=None if r_hi is None else (r_hi, r_lo))
+            h1 = self._wino_conv(pool, e1, x, None, groups=GN_GROUPS, mean=mean, rstd=rstd,
+                                 gamma=m.norm1.weight.detach(), beta=m.norm1.bias.detach(), raw_hi=r_hi, raw_lo=r_lo)
             pool.put(mean, rstd)
         else:
             a_f32, a_hi, a_lo, r_hi, r_lo = self._gn_act(pool, x, m.norm1, umma1, want_raw_split=fuse_skip or skip_umma)
@@ -167,31 +124,22 @@ class VQGANEngine(KernelExecutor):
             pool.put(a_f32, a_hi, a_lo)
         if wino2:
             # Winograd conv2: the shortcut (1x1 GEMM or identity) enters as the output transform's residual
-            sk = None
-            if es is not None:
-                if "hi" in es and W >= 4 and r_hi is not None:
-                    sk, _, _ = self._conv(pool, es, a_hi=r_hi, a_lo=r_lo, shape=(B, H, W))
-                else:
-                    sk, _, _ = self._conv(pool, es, a_f32=x, shape=(B, H, W))
+            residual, res_mode, sk = self._skip_residual(pool, es, x, cabi.RES_SAME, x, r_hi, r_lo, (B, H, W))
             mean, rstd = self._stats(pool, h1, None)
-            out = self._wino_conv(pool, e2, h1, None, mean=mean, rstd=rstd, gamma=m.norm2.weight.detach(),
-                                  beta=m.norm2.bias.detach(), residual=x if sk is None else sk, res_mode=cabi.RES_SAME)
+            out = self._wino_conv(pool, e2, h1, None, groups=GN_GROUPS, mean=mean, rstd=rstd,
+                                  gamma=m.norm2.weight.detach(), beta=m.norm2.bias.detach(), residual=residual,
+                                  res_mode=res_mode)
             pool.put(mean, rstd, h1, r_hi, r_lo, sk)
             return out
         b_f32, b_hi, b_lo, _, _ = self._gn_act(pool, h1, m.norm2, umma2)
         pool.put(h1)
         kw = dict(a_f32=b_f32, a_hi=b_hi, a_lo=b_lo, shape=(B, H, W), stats=True)
-        sk = None
         if fuse_skip:
+            sk = None
             out, _, _ = self._conv(pool, e2, second=(es, r_hi, r_lo), **kw)
-        elif es is not None:
-            if skip_umma:
-                sk, _, _ = self._conv(pool, es, a_hi=r_hi, a_lo=r_lo, shape=(B, H, W))
-            else:
-                sk, _, _ = self._conv(pool, es, a_f32=x, shape=(B, H, W))
-            out, _, _ = self._conv(pool, e2, residual=sk, res_mode=cabi.RES_SAME, **kw)
         else:
-            out, _, _ = self._conv(pool, e2, residual=x, res_mode=cabi.RES_SAME, **kw)
+            residual, res_mode, sk = self._skip_residual(pool, es, x, cabi.RES_SAME, x, r_hi, r_lo, (B, H, W))
+            out, _, _ = self._conv(pool, e2, residual=residual, res_mode=res_mode, **kw)
         pool.put(b_f32, b_hi, b_lo, r_hi, r_lo, sk)
         return out
 
@@ -251,14 +199,8 @@ class VQGANEngine(KernelExecutor):
                 hi = pool.get((B, H // 2, W // 2, 4 * Cc), torch.bfloat16)
                 lo = pool.get((B, H // 2, W // 2, 4 * Cc), torch.bfloat16)
                 self.be.s2d_split(x, hi, lo)
-                out = pool.get((B, H // 2, W // 2, Cc))
-                rows = self._geom(H // 2, W // 2)
-                part = pool.get((B * rows, Cc, 2)) if rows else None
-                self.be.conv_umma(B=B, H=H // 2, W=W // 2, Cin=4 * Cc, Cout=Cc, taps=4, a_hi=hi, a_lo=lo,
-                                  w_hi=ent["ds_hi"], w_lo=ent["ds_lo"], bias=ent["bias"], out=out, passes=self.passes,
-                                  stats_partial=part)
-                if part is not None:
-                    out._gn = (part, rows)
+                out, _, _ = self._conv(pool, ent, a_hi=hi, a_lo=lo, shape=(B, H // 2, W // 2),
+                                       planes=(ent["ds_hi"], ent["ds_lo"]), taps=4, stats=True)
                 pool.put(hi, lo)
                 return out
             out = pool.get((B, (H + 1 - 3) // 2 + 1, (W + 1 - 3) // 2 + 1, Cc))
@@ -278,13 +220,8 @@ class VQGANEngine(KernelExecutor):
         ent = self._w[name + ".conv"]
         if "up_hi" in ent and W >= 4:
             hi, lo = self._split(pool, x)
-            out = pool.get((B, 2 * H, 2 * W, Cc))
-            rows = 4 * self._geom(H, W)
-            part = pool.get((B * rows, Cc, 2)) if rows else None
-            be.conv_umma(B=B, H=H, W=W, Cin=Cc, Cout=Cc, taps=4, a_hi=hi, a_lo=lo, w_hi=ent["up_hi"], w_lo=ent["up_lo"],
-                         bias=ent["bias"], out=out, passes=self.passes, upsample2x=True, stats_partial=part)
-            if part is not None:
-                out._gn = (part, rows)
+            out, _, _ = self._conv(pool, ent, a_hi=hi, a_lo=lo, shape=(B, H, W), planes=(ent["up_hi"], ent["up_lo"]),
+                                   taps=4, upsample2x=True, stats=True)
             pool.put(hi, lo)
             return out
         up = pool.get((B, 2 * H, 2 * W, Cc))
@@ -309,22 +246,19 @@ class VQGANEngine(KernelExecutor):
         self.be.nchw_to_nhwc_cat(x.contiguous().float(), None, xin)
         return xin
 
-    def _head(self, pool, h, norm, ent, out_channels):
-        """norm_out -> swish -> conv_out; returns (nhwc or None, nchw or None)."""
+    def _head(self, pool, h, norm, ent, out=None):
+        """norm_out -> swish -> conv_out: the NHWC result, or into the NCHW tensor out."""
         B, H, W, _ = h.shape
-        if "hi_pad" in ent and W >= 4:
-            _, a_hi, a_lo, _, _ = self._gn_act(pool, h, norm, True)
-            out = torch.empty((B, out_channels, H, W), dtype=torch.float32, device=h.device)
-            self.be.conv_umma(B=B, H=H, W=W, Cin=ent["cin"], Cout=64, taps=9, a_hi=a_hi, a_lo=a_lo, w_hi=ent["hi_pad"],
-                              w_lo=ent["lo_pad"], bias=ent["bias_pad"], out=out, passes=self.passes,
-                              out_nchw_channels=out_channels)
-            pool.put(a_hi, a_lo)
-            return None, out
-        umma = "hi" in ent and W >= 4
-        a_f32, a_hi, a_lo, _, _ = self._gn_act(pool, h, norm, umma)
+        if out is not None and "hi_pad" in ent and W >= 4:
+            return self._padded_head(pool, h, norm, ent, out)
+        a_f32, a_hi, a_lo, _, _ = self._gn_act(pool, h, norm, "hi" in ent and W >= 4)
         y, _, _ = self._conv(pool, ent, a_f32=a_f32, a_hi=a_hi, a_lo=a_lo, shape=(B, H, W))
         pool.put(a_f32, a_hi, a_lo)
-        return y, None
+        if out is None:
+            return y
+        self.be.nhwc_to_nchw(y, out)
+        pool.put(y)
+        return out
 
     # ------------------------------------------------------------------------------ public
     # activation budget of one pass: 32 images of 256x256 (the cfg3 batch; ~25 GB of pooled NHWC tensors and operand
@@ -359,7 +293,7 @@ class VQGANEngine(KernelExecutor):
             if i != enc.num_resolutions - 1:
                 h = self._step(pool, h, self._downsample, f"encoder.down.{i}.downsample", lvl.downsample)
         h = self._mid(pool, "encoder.mid", enc.mid, h)
-        y, _ = self._head_nhwc(pool, h, enc.norm_out, w["encoder.conv_out"])
+        y = self._head(pool, h, enc.norm_out, w["encoder.conv_out"])
         pool.put(h)
         if quant_conv:
             y = self._step(pool, y, lambda p, t: self._conv_plain(p, w["quant_conv"], t))
@@ -368,14 +302,6 @@ class VQGANEngine(KernelExecutor):
         self.be.nhwc_to_nchw(y, out)
         pool.put(y)
         return out
-
-    def _head_nhwc(self, pool, h, norm, ent):
-        B, H, W, _ = h.shape
-        umma = "hi" in ent and W >= 4
-        a_f32, a_hi, a_lo, _, _ = self._gn_act(pool, h, norm, umma)
-        y, _, _ = self._conv(pool, ent, a_f32=a_f32, a_hi=a_hi, a_lo=a_lo, shape=(B, H, W))
-        pool.put(a_f32, a_hi, a_lo)
-        return y, None
 
     @torch.no_grad()
     def quantize(self, z_nhwc, pool):
@@ -420,11 +346,8 @@ class VQGANEngine(KernelExecutor):
             if i != 0:
                 h = self._step(pool, h, self._upsample, f"decoder.up.{i}.upsample", lvl.upsample)
         ent = w["decoder.conv_out"]
-        y, out = self._head(pool, h, dec.norm_out, ent, ent["cout"])
+        B, H, W, _ = h.shape
+        out = torch.empty((B, ent["cout"], H, W), dtype=torch.float32, device=z.device)
+        self._head(pool, h, dec.norm_out, ent, out)
         pool.put(h)
-        if out is None:
-            B, H, W, Co = y.shape
-            out = torch.empty((B, Co, H, W), dtype=torch.float32, device=z.device)
-            self.be.nhwc_to_nchw(y, out)
-            pool.put(y)
         return (out, indices) if return_indices else out

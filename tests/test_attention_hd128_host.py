@@ -80,16 +80,6 @@ def test_engine_wiring_hd128_matches_reference_fixture(tag):
     assert torch.equal(out, out2)
 
 
-def test_engine_mma_sync_switch_takes_hd128():
-    g = {k: v for k, v in load("mid_hd128").items() if isinstance(v, torch.Tensor)}
-    be = EmuBackend()
-    eng = UNetEngine(build(HD128_CONFIGS["mid_hd128"]), backend=be)
-    eng.attention_impl = "mma.sync"
-    out = eng.forward(g["x"], g["t"], g["y"])
-    assert "attention_split" in be.calls and "attention_tc" not in be.calls
-    assert rel_dev(out, g["unet_out"]) < 6e-5
-
-
 @pytest.mark.parametrize("tag", TAGS)
 def test_engine_rejects_head_dim_256(tag):
     cfg = dict(HD128_CONFIGS[tag], num_heads=1)            # 256 channels / 1 head
