@@ -11,8 +11,13 @@
 //     tap straight from the activation tensor; out-of-image coordinates are zero-filled by the
 //     TMA unit, which IS the conv padding -- no im2col buffer, no halo logic.
 //   * Warp-specialised persistent CTA: warps 0-7 = two consumer warpgroups (wgmma m64nBNk16 on rows
-//     0-63 / 64-127 of the tile, register accumulators, epilogue straight from the fragment), warp 8 =
-//     TMA producer feeding a STAGES-deep shared-memory ring.
+//     0-63 / 64-127 of the tile, register accumulators, epilogue straight from the fragment), warps 8-11 =
+//     producer warpgroup whose first lane feeds a STAGES-deep shared-memory ring with TMA.  384 threads cap
+//     every thread at 168 registers, so the producer warpgroup gives registers to the consumers (setmaxnreg).
+//   * Software-pipelined epilogue: a finished tile's promoted accumulator stays in registers while the
+//     next tile's first chunk runs; after each of that chunk's K blocks is issued, the consumers run one
+//     slice (a group of columns) of the finished tile's epilogue, so it overlaps the tensor core.  Each
+//     element's arithmetic is the same as in a serial epilogue.
 //   * fp32-faithful accumulation: the tensor core's accumulator add truncates (round-toward-zero),
 //     so a K = 9216 chain accumulated entirely inside wgmma drifts by ~3e-5.  The K loop is therefore
 //     cut into chunks of `kb_per_chunk` K-blocks; each chunk starts from a zero wgmma accumulator and is
@@ -26,7 +31,11 @@ namespace bbdm {
 
 constexpr int UM_BM = 128;       // pixels per tile (two m64 warpgroups)
 constexpr int UM_BK = 64;        // K block: 64 input channels of one tap = one 128-byte SWIZZLE_128B row
-constexpr int UM_THREADS = 288;  // 2 consumer warpgroups + 1 producer warp
+constexpr int UM_THREADS = 384;  // 2 consumer warpgroups + 1 producer warpgroup
+// register split (65,536 per SM): 128 x 40 for the producer warpgroup + 256 x 232 for the consumers
+constexpr int UM_PRODUCER_REGS = 40, UM_CONSUMER_REGS = 232;
+static_assert(128 * UM_PRODUCER_REGS + 256 * UM_CONSUMER_REGS <= 65536, "conv_umma: register split");
+constexpr int UM_SLICES = 4;     // epilogue slices per tile, each BN / 32 column blocks of 8
 
 struct ConvParams {
   int B, H, W, Cout;
@@ -64,6 +73,178 @@ __device__ __forceinline__ void conv_mma(float* d, uint64_t da, uint64_t db) {
   } else {
     if (BN == 128) wgmma_n128_bf16<0>(d, da, db, 1u); else wgmma_n64_bf16<0>(d, da, db, 1u);
   }
+}
+
+// ---- tile epilogue: bias / fused-skip bias / residual / store, straight from the fragment ----------------
+// Where a consumer thread's two fragment rows (ri = 0, 1) of a tile land; computed once per tile, kept while
+// the epilogue's slices run.
+struct EpiTile {
+  int nb, tw, th, tb, phase;
+  int bb[2], hh[2], ww[2];
+  bool valid[2];
+  int64_t pix[2];
+};
+
+__device__ __forceinline__ EpiTile epi_tile(const ConvParams& p, int tile, int n_blocks, int warp, int lane) {
+  EpiTile e;
+  e.nb = tile % n_blocks;
+  int mt = tile / n_blocks;
+  e.phase = 0;
+  if (p.up2) { e.phase = mt & 3; mt >>= 2; }
+  e.tw = mt % p.tiles_w; mt /= p.tiles_w;
+  e.th = mt % p.tiles_h;
+  e.tb = mt / p.tiles_h;
+  const int OH = p.up2 ? 2 * p.H : p.H, OW = p.up2 ? 2 * p.W : p.W;
+#pragma unroll
+  for (int ri = 0; ri < 2; ++ri) {
+    const int row = 16 * warp + (lane >> 2) + 8 * ri;        // tile row (warp 0-7 -> rows 0-127)
+    const int ws = e.tw * p.TW + row % p.TW;                  // coordinates in the conv INPUT grid
+    const int hs = e.th * p.TH + (row / p.TW) % p.TH;
+    e.bb[ri] = e.tb * p.TB + row / (p.TW * p.TH);
+    e.valid[ri] = ws < p.W && hs < p.H && e.bb[ri] < p.B;
+    e.hh[ri] = p.up2 ? 2 * hs + (e.phase >> 1) : hs;         // output grid (fused upsample: 2x with phase offset)
+    e.ww[ri] = p.up2 ? 2 * ws + (e.phase & 1) : ws;
+    e.pix[ri] = ((int64_t)e.bb[ri] * OH + e.hh[ri]) * OW + e.ww[ri];
+  }
+  return e;
+}
+
+// Slice s of the epilogue: column blocks jj = JS*s .. JS*s + JS-1 (8 columns each) of both fragment rows.
+// Every bias and residual load of the slice is issued before its first store; each element's residual is
+// read by the thread that writes that element, so out == residual works.  With fused GroupNorm statistics,
+// the slice's per-warp column (sum, sum sq) go to stats_s (sum order: row ri 0, ri 1, lanes xor 4/8/16).
+template <int BN>
+__device__ __forceinline__ void epi_slice(const ConvParams& p, const float* racc, EpiTile e, int s, int warp,
+                                          int lane, float (*stats_s)[BN][2]) {
+  constexpr int JS = BN / 8 / UM_SLICES;
+  // opaque tile coordinates: otherwise the compiler hoists every slice's address arithmetic out of the K loop the
+  // slice runs in, and those addresses would occupy registers (and spill) for the whole loop
+  asm volatile("" : "+r"(e.nb), "+r"(e.bb[0]), "+r"(e.bb[1]), "+r"(e.hh[0]), "+r"(e.hh[1]), "+r"(e.ww[0]),
+               "+r"(e.ww[1]), "+l"(e.pix[0]), "+l"(e.pix[1]));
+  const int OH = p.up2 ? 2 * p.H : p.H, OW = p.up2 ? 2 * p.W : p.W;
+  const int n0 = e.nb * BN + 2 * (lane & 3);
+  // bias terms first, then the residual: the same per-element order of adds as a serial epilogue, with the
+  // residual mode branched on once per slice so that all of its loads can be in flight together
+  float2 v[2][JS];
+#pragma unroll
+  for (int ri = 0; ri < 2; ++ri) {
+#pragma unroll
+    for (int j = 0; j < JS; ++j) {
+      const int jj = JS * s + j;
+      const int nc = n0 + 8 * jj;
+      v[ri][j] = make_float2(racc[4 * jj + 2 * ri], racc[4 * jj + 2 * ri + 1]);
+      if (p.bias) { const float2 b = *reinterpret_cast<const float2*>(p.bias + nc); v[ri][j].x += b.x; v[ri][j].y += b.y; }
+      if (p.bias2) { const float2 b = *reinterpret_cast<const float2*>(p.bias2 + nc); v[ri][j].x += b.x; v[ri][j].y += b.y; }
+    }
+  }
+  if (p.res_mode == BBDM_RES_SAME || p.res_mode == BBDM_RES_UP2) {
+#pragma unroll
+    for (int ri = 0; ri < 2; ++ri) {
+      if (!e.valid[ri]) continue;
+      const int64_t rpix = p.res_mode == BBDM_RES_SAME
+                               ? e.pix[ri]
+                               : ((int64_t)e.bb[ri] * (OH >> 1) + (e.hh[ri] >> 1)) * (OW >> 1) + (e.ww[ri] >> 1);
+      const float* rp = p.residual + rpix * p.Cout + n0 + 8 * JS * s;
+#pragma unroll
+      for (int j = 0; j < JS; ++j) {
+        const float2 t = *reinterpret_cast<const float2*>(rp + 8 * j);
+        v[ri][j].x += t.x; v[ri][j].y += t.y;
+      }
+    }
+  } else if (p.res_mode == BBDM_RES_DOWN2) {
+    const int64_t W2 = (int64_t)OW * 2;
+#pragma unroll
+    for (int ri = 0; ri < 2; ++ri) {
+      if (!e.valid[ri]) continue;
+      const float* rp0 = p.residual + (((int64_t)e.bb[ri] * OH * 2 + e.hh[ri] * 2) * W2 + e.ww[ri] * 2) * p.Cout +
+                         n0 + 8 * JS * s;
+#pragma unroll
+      for (int j = 0; j < JS; ++j) {
+        const float* rp = rp0 + 8 * j;
+        const float2 t0 = *reinterpret_cast<const float2*>(rp), t1 = *reinterpret_cast<const float2*>(rp + p.Cout);
+        const float2 t2 = *reinterpret_cast<const float2*>(rp + W2 * p.Cout);
+        const float2 t3 = *reinterpret_cast<const float2*>(rp + (W2 + 1) * p.Cout);
+        v[ri][j].x += 0.25f * (((t0.x + t1.x) + t2.x) + t3.x);
+        v[ri][j].y += 0.25f * (((t0.y + t1.y) + t2.y) + t3.y);
+      }
+    }
+  }
+  float ssum[2 * JS], ssq[2 * JS];           // per (column block, parity): sums over this thread's 2 rows
+#pragma unroll
+  for (int j = 0; j < 2 * JS; ++j) { ssum[j] = 0.f; ssq[j] = 0.f; }
+#pragma unroll
+  for (int ri = 0; ri < 2; ++ri) {
+    if (!e.valid[ri]) continue;
+    const int bb = e.bb[ri], hh = e.hh[ri], ww = e.ww[ri];
+    const int64_t pix = e.pix[ri];
+#pragma unroll
+    for (int j = 0; j < JS; ++j) {
+      const int nc = n0 + 8 * (JS * s + j);
+      const float2 w = v[ri][j];
+      if (p.out_nchw_c > 0) {
+        // head: first out_nchw_c couts straight into the NCHW result
+        if (nc < p.out_nchw_c) p.out[(((int64_t)bb * p.out_nchw_c + nc) * OH + hh) * OW + ww] = w.x;
+        if (nc + 1 < p.out_nchw_c) p.out[(((int64_t)bb * p.out_nchw_c + nc + 1) * OH + hh) * OW + ww] = w.y;
+      } else if (p.out) {
+        *reinterpret_cast<float2*>(p.out + pix * p.Cout + nc) = w;
+      }
+      if (p.out_hi) {
+        uint32_t h, l;
+        split2x(w.x, w.y, h, l);
+        *reinterpret_cast<uint32_t*>(p.out_hi + pix * p.Cout + nc) = h;
+        *reinterpret_cast<uint32_t*>(p.out_lo + pix * p.Cout + nc) = l;
+      }
+      ssum[2 * j] += w.x; ssq[2 * j] += w.x * w.x;
+      ssum[2 * j + 1] += w.y; ssq[2 * j + 1] += w.y * w.y;
+    }
+  }
+  if (p.stats) {
+    // rows of a warp: lanes with equal lane % 4 hold the same columns
+#pragma unroll
+    for (int j = 0; j < 2 * JS; ++j) {
+#pragma unroll
+      for (int off = 4; off < 32; off <<= 1) {
+        ssum[j] += __shfl_xor_sync(0xffffffffu, ssum[j], off);
+        ssq[j] += __shfl_xor_sync(0xffffffffu, ssq[j], off);
+      }
+    }
+    if (lane < 4) {
+#pragma unroll
+      for (int j = 0; j < 2 * JS; ++j) {
+        const int c = 8 * (JS * s + (j >> 1)) + 2 * lane + (j & 1);
+        stats_s[warp][c][0] = ssum[j];
+        stats_s[warp][c][1] = ssq[j];
+      }
+    }
+  }
+}
+
+// After a tile's last slice: fused GroupNorm statistics of the tensor just written, per-channel (sum, sum sq)
+// over each 32-row quarter of the tile (tile lies inside one image: TB == 1); a quarter is warps (2q, 2q + 1).
+template <int BN>
+__device__ __forceinline__ void epi_stats_out(const ConvParams& p, const EpiTile& e, float (*stats_s)[BN][2]) {
+  if (!p.stats) return;
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  const int64_t tile_lin =
+      (((int64_t)e.tb * p.tiles_w * p.tiles_h + e.th * p.tiles_w + e.tw) * (p.up2 ? 4 : 1) + e.phase) * 4;
+  int i0 = threadIdx.x;
+  asm volatile("" : "+r"(i0));   // keeps this loop's per-thread indices from being held across the tile loop
+  for (int i = i0; i < 4 * BN; i += 256) {
+    const int q = i / BN, c = i % BN;
+    const float s = stats_s[2 * q][c][0] + stats_s[2 * q + 1][c][0];
+    const float sq = stats_s[2 * q][c][1] + stats_s[2 * q + 1][c][1];
+    *reinterpret_cast<float2*>(p.stats + ((tile_lin + q) * p.Cout + e.nb * BN + c) * 2) = make_float2(s, sq);
+  }
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+}
+
+// slices s_begin .. s_end - 1 (s is a run-time index; each slice's register indices must be compile-time)
+template <int BN>
+__device__ __forceinline__ void epi_slices(const ConvParams& p, const float* racc, const EpiTile& e, int s_begin,
+                                           int s_end, int warp, int lane, float (*stats_s)[BN][2]) {
+#pragma unroll
+  for (int s = 0; s < UM_SLICES; ++s)
+    if (s >= s_begin && s < s_end) epi_slice<BN>(p, racc, e, s, warp, lane, stats_s);
 }
 
 template <int BN, int PASSES, bool F16>
@@ -105,9 +286,10 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
   const int total_tiles = p.n_tiles * n_blocks * (p.up2 ? 4 : 1);
   const int KB = p.K1 + p.K2;
 
-  if (warp == 8) {
+  if (warp >= 8) {
     // ================================ TMA producer ==========================================
-    if (lane == 0) {
+    setmaxnreg_dec<UM_PRODUCER_REGS>();
+    if (warp == 8 && lane == 0) {
       int stage = 0;
       uint32_t phase_bit = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -155,14 +337,18 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
   }
 
   // ================================ consumer warpgroups: MMA + epilogue ========================
+  setmaxnreg_inc<UM_CONSUMER_REGS>();
   const int wg = warp >> 2;                    // rows 64*wg .. 64*wg + 63 of the tile
   const uint32_t a_off = (uint32_t)wg * 64 * 128;
   int stage = 0;
   uint32_t phase_bit = 0;
+  // racc: the tile's fp32 accumulator.  From the end of a tile until the end of the next tile's first chunk it
+  // holds the finished tile (epilogue `pend`, slices done so far `slice`).
+  float racc[NR];
+  EpiTile pend;
+  bool pending = false;
+  int slice = 0;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-    float racc[NR];
-#pragma unroll
-    for (int j = 0; j < NR; ++j) racc[j] = 0.f;
     for (int kb0 = 0; kb0 < KB; kb0 += p.kb_per_chunk) {
       const int kb1 = kb0 + p.kb_per_chunk < KB ? kb0 + p.kb_per_chunk : KB;
       float acc[NR];
@@ -191,107 +377,37 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
         if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase_bit ^= 1; }
+        if (pending) {
+          // the previous tile's epilogue, one slice per K block while its wgmmas run; the chunk's last K block
+          // takes the slices left over
+          const int s_end = kb + 1 < kb1 ? slice + 1 : UM_SLICES;
+          epi_slices<BN>(p, racc, pend, slice, s_end, warp, lane, stats_s);
+          slice = s_end;
+        }
+      }
+      if (pending) {
+        epi_stats_out<BN>(p, pend, stats_s);
+        pending = false;
       }
       wgmma_wait<0>();
       reg_fence<NR>(acc);
       if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
+      if (kb0 == 0) {
 #pragma unroll
-      for (int j = 0; j < NR; ++j) racc[j] += acc[j];
-    }
-
-    // ---- tile epilogue: bias / fused-skip bias / residual / store, straight from the fragment ----------
-    const int nb = tile % n_blocks;
-    int mt = tile / n_blocks;
-    int phase = 0;
-    if (p.up2) { phase = mt & 3; mt >>= 2; }
-    const int tw = mt % p.tiles_w; mt /= p.tiles_w;
-    const int th = mt % p.tiles_h;
-    const int tb = mt / p.tiles_h;
-    const int OH = p.up2 ? 2 * p.H : p.H, OW = p.up2 ? 2 * p.W : p.W;
-    const int n0 = nb * BN + 2 * (lane & 3);
-    float ssum[NR / 2], ssq[NR / 2];           // per (column block, parity): sums over this thread's 2 rows
+        for (int j = 0; j < NR; ++j) racc[j] = 0.f + acc[j];
+      } else {
 #pragma unroll
-    for (int j = 0; j < NR / 2; ++j) { ssum[j] = 0.f; ssq[j] = 0.f; }
-#pragma unroll
-    for (int ri = 0; ri < 2; ++ri) {
-      const int row = 16 * warp + (lane >> 2) + 8 * ri;     // tile row (warp 0-7 -> rows 0-127)
-      const int ws = tw * p.TW + row % p.TW;                 // coordinates in the conv INPUT grid
-      const int hs = th * p.TH + (row / p.TW) % p.TH;
-      const int bb = tb * p.TB + row / (p.TW * p.TH);
-      const bool valid = ws < p.W && hs < p.H && bb < p.B;
-      const int hh = p.up2 ? 2 * hs + (phase >> 1) : hs;     // output grid (fused upsample: 2x with phase offset)
-      const int ww = p.up2 ? 2 * ws + (phase & 1) : ws;
-      const int64_t pix = ((int64_t)bb * OH + hh) * OW + ww;
-      if (!valid) continue;
-#pragma unroll
-      for (int jj = 0; jj < BN / 8; ++jj) {
-        const int nc = n0 + 8 * jj;
-        float2 v = make_float2(racc[4 * jj + 2 * ri], racc[4 * jj + 2 * ri + 1]);
-        if (p.bias) { const float2 b = *reinterpret_cast<const float2*>(p.bias + nc); v.x += b.x; v.y += b.y; }
-        if (p.bias2) { const float2 b = *reinterpret_cast<const float2*>(p.bias2 + nc); v.x += b.x; v.y += b.y; }
-        if (p.res_mode == BBDM_RES_SAME) {
-          const float2 t = *reinterpret_cast<const float2*>(p.residual + pix * p.Cout + nc);
-          v.x += t.x; v.y += t.y;
-        } else if (p.res_mode == BBDM_RES_UP2) {
-          const float2 t = *reinterpret_cast<const float2*>(
-              p.residual + (((int64_t)bb * (OH >> 1) + (hh >> 1)) * (OW >> 1) + (ww >> 1)) * p.Cout + nc);
-          v.x += t.x; v.y += t.y;
-        } else if (p.res_mode == BBDM_RES_DOWN2) {
-          const int64_t W2 = (int64_t)OW * 2;
-          const float* rp = p.residual + (((int64_t)bb * OH * 2 + hh * 2) * W2 + ww * 2) * p.Cout + nc;
-          const float2 t0 = *reinterpret_cast<const float2*>(rp), t1 = *reinterpret_cast<const float2*>(rp + p.Cout);
-          const float2 t2 = *reinterpret_cast<const float2*>(rp + W2 * p.Cout);
-          const float2 t3 = *reinterpret_cast<const float2*>(rp + (W2 + 1) * p.Cout);
-          v.x += 0.25f * (((t0.x + t1.x) + t2.x) + t3.x);
-          v.y += 0.25f * (((t0.y + t1.y) + t2.y) + t3.y);
-        }
-        if (p.out_nchw_c > 0) {
-          // head: first out_nchw_c couts straight into the NCHW result
-          if (nc < p.out_nchw_c) p.out[(((int64_t)bb * p.out_nchw_c + nc) * OH + hh) * OW + ww] = v.x;
-          if (nc + 1 < p.out_nchw_c) p.out[(((int64_t)bb * p.out_nchw_c + nc + 1) * OH + hh) * OW + ww] = v.y;
-        } else if (p.out) {
-          *reinterpret_cast<float2*>(p.out + pix * p.Cout + nc) = v;
-        }
-        if (p.out_hi) {
-          uint32_t h, l;
-          split2x(v.x, v.y, h, l);
-          *reinterpret_cast<uint32_t*>(p.out_hi + pix * p.Cout + nc) = h;
-          *reinterpret_cast<uint32_t*>(p.out_lo + pix * p.Cout + nc) = l;
-        }
-        ssum[2 * jj] += v.x; ssq[2 * jj] += v.x * v.x;
-        ssum[2 * jj + 1] += v.y; ssq[2 * jj + 1] += v.y * v.y;
+        for (int j = 0; j < NR; ++j) racc[j] += acc[j];
       }
     }
-    if (p.stats) {
-      // fused GroupNorm statistics of the tensor just written: per-channel (sum, sum sq) over each
-      // 32-row quarter of the tile (tile lies inside one image: TB == 1).  Rows of a warp: lanes with
-      // equal lane % 4 hold the same columns; a quarter is warps (2q, 2q + 1).
-#pragma unroll
-      for (int j = 0; j < NR / 2; ++j) {
-#pragma unroll
-        for (int off = 4; off < 32; off <<= 1) {
-          ssum[j] += __shfl_xor_sync(0xffffffffu, ssum[j], off);
-          ssq[j] += __shfl_xor_sync(0xffffffffu, ssq[j], off);
-        }
-      }
-      if (lane < 4) {
-#pragma unroll
-        for (int j = 0; j < NR / 2; ++j) {
-          const int c = 8 * (j >> 1) + 2 * lane + (j & 1);
-          stats_s[warp][c][0] = ssum[j];
-          stats_s[warp][c][1] = ssq[j];
-        }
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      const int64_t tile_lin = (((int64_t)tb * p.tiles_w * p.tiles_h + th * p.tiles_w + tw) * (p.up2 ? 4 : 1) + phase) * 4;
-      for (int e = threadIdx.x; e < 4 * BN; e += 256) {
-        const int q = e / BN, c = e % BN;
-        const float s = stats_s[2 * q][c][0] + stats_s[2 * q + 1][c][0];
-        const float sq = stats_s[2 * q][c][1] + stats_s[2 * q + 1][c][1];
-        *reinterpret_cast<float2*>(p.stats + ((tile_lin + q) * p.Cout + nb * BN + c) * 2) = make_float2(s, sq);
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-    }
+    pend = epi_tile(p, tile, n_blocks, warp, lane);
+    pending = true;
+    slice = 0;
+  }
+  if (pending) {
+    // a CTA's last tile: nothing left to overlap with
+    epi_slices<BN>(p, racc, pend, 0, UM_SLICES, warp, lane, stats_s);
+    epi_stats_out<BN>(p, pend, stats_s);
   }
 }
 
