@@ -450,13 +450,16 @@ int bbdm_ema_multi(const void* const* params, const int64_t* numel, const int64_
  *   order 0 (QKVAttentionLegacy, openaimodel.py:350-375): [head][q|k|v][head_dim]
  *   order 1 (QKVAttention, :382-413):                      [q|k|v][head][head_dim]
  * out: fp32 [B,T,C] and/or split bf16 (A operand of the proj_out GEMM).
- * Split-bf16 tensor-core products with fp32 accumulation.  head_dim in {16,32,64,128}. */
+ * Split-bf16 tensor-core products with fp32 accumulation: q and k are scaled by s, then split; expf softmax.
+ * Runs on the mma.sync kernel of bbdm_attention_split, which copies the fp32 K/V tiles with cp.async and splits
+ * them in shared memory.  head_dim in {16,32,64,128}. */
 int bbdm_attention(const float* qkv, int B, int T, int C, int heads, int order,
                    float* out_f32, void* out_hi, void* out_lo, void* stream);
 
 /* Same attention core on PRE-SPLIT bf16 planes qkv_hi/qkv_lo [B,T,3C] (written by the qkv
  * conv's epilogue, BbdmConvArgs.out_hi/out_lo): no conversion or re-splitting of K/V per query
- * tile; cp.async double-buffered KV tiles, ldmatrix fragments, 128 queries per CTA.  head_dim in {16,32,64,128}. */
+ * tile; cp.async double-buffered KV tiles, ldmatrix fragments, 128 queries per CTA; S is scaled by D^-1/2 after the
+ * products and the softmax runs on ex2.approx.  head_dim in {16,32,64,128}. */
 int bbdm_attention_split(const void* qkv_hi, const void* qkv_lo, int B, int T, int C, int heads,
                          int order, float* out_f32, void* out_hi, void* out_lo, void* stream);
 

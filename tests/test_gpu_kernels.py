@@ -703,6 +703,23 @@ def test_attention_cross(be, B, Tq, Tkv, heads, D):
     assert torch.equal(oh.float().cpu(), h) and torch.equal(ol.float().cpu(), l)
 
 
+def test_attention_mma_bit_pinned(be):
+    """The mma.sync attention entry points reproduce tests/golden/attention_mma.npz bit for bit: the fp32-qkv form
+    keeps its own arithmetic (q, k scaled before the split, expf softmax), the split-plane forms theirs."""
+    import json
+    import numpy as np
+    from golden import make_golden_attention_mma as G
+    fx = np.load(os.path.join(os.path.dirname(__file__), "golden", "attention_mma.npz"))
+    cases = json.loads(str(fx["cases"]))
+    assert cases == G.CASES
+    for i, case in enumerate(cases):
+        got = G.run(be, case)
+        assert sorted(got) == sorted(k.split("_", 1)[1] for k in fx.files if k.startswith(f"{i}_")), case
+        for k, v in got.items():
+            want = torch.from_numpy(fx[f"{i}_{k}"])
+            assert torch.equal(v.view(torch.int16) if v.dtype == torch.bfloat16 else v, want), (case, k)
+
+
 # ------------------------------------------------------------------------------------ stem
 @pytest.mark.parametrize("B,H,W,Cin,Cout", [(2, 32, 64, 6, 128), (1, 16, 32, 3, 64), (3, 8, 32, 16, 128), (2, 40, 96, 4, 32)])
 def test_conv_stem_equals_conv_direct_and_fuses_gn_partials(be, B, H, W, Cin, Cout):

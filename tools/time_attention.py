@@ -1,12 +1,14 @@
 #!/usr/bin/env python
 """Time the attention kernels alone with CUDA events, per head_dim at equal FLOPs.
 
-    python tools/time_attention.py [--head-dims 64 128] [--B 16 --T 4096 --C 1024] [--out FILE]
+    python tools/time_attention.py [--head-dims 64 128] [--B 16 --T 4096 --C 1024] [--kernels ...] [--out FILE]
     python tools/time_attention.py B T C heads          # one head layout, head_dim = C / heads
 
 Default: the cfg2 middle-block shape (B=16, T=4096, C=1024) as 16 heads x 64 and as 8 heads x 128.  For each
-head_dim it times bbdm_attention_tc (split-bf16 planes in, split planes out) and bbdm_attention_bwd (exact fp32),
-alternating the variants over rounds and reporting the median.  Algorithmic FLOPs: forward 4 B T^2 C (QK^T, PV),
+head_dim it times the --kernels (default: bbdm_attention_tc with split-bf16 planes in and split planes out, and
+bbdm_attention_bwd in exact fp32; also available: the mma.sync forwards bbdm_attention, fp32 qkv in and fp32 out, and
+bbdm_attention_split, split planes in and out, for head_dim 16 / 32 / 64 / 128), alternating the variants over
+rounds and reporting the median.  Algorithmic FLOPs: forward 4 B T^2 C (QK^T, PV),
 backward 10 B T^2 C (the five T x T x D products of FlashAttention's backward), whatever the kernels recompute.
 One JSON line per (kernel, head_dim), each tagged with the card's name and power limit read in the same run."""
 import argparse
@@ -53,6 +55,8 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--fwd-iters", type=int, default=10)
     ap.add_argument("--bwd-iters", type=int, default=2)
+    ap.add_argument("--kernels", nargs="+", default=["attention_tc", "attention_bwd"],
+                    choices=["attention_tc", "attention_bwd", "attention", "attention_split"])
     ap.add_argument("--out", default=None, help="also append the JSON lines to this file")
     a = ap.parse_args()
     if a.shape:
@@ -73,32 +77,35 @@ def main():
     dout = torch.randn(B, T, C, device="cuda", generator=g)
     dqkv = torch.empty_like(qkv)
 
-    runs = {}
+    runs = []                                                      # (kernel, head_dim, heads, fn, iters, flops)
     for d in a.head_dims:
         assert C % d == 0, (C, d)
         heads = C // d
         lse = torch.empty(B * heads * T, device="cuda")
         delta = torch.empty_like(lse)
-        fwd = lambda h=heads: be.attention_tc(hi, lo, h, 0, None, o_hi, o_lo)
-        bwd = lambda h=heads, l=lse, dl=delta: be.attention_bwd(qkv, out, dout, h, 0, dqkv, l, dl)
-        be.attention_tc(hi, lo, heads, 0, out, None, None)      # the forward output the backward is given
-        fwd(); bwd()                                               # warm up every shape timed below
+        fns = {"attention_tc": (lambda h=heads: be.attention_tc(hi, lo, h, 0, None, o_hi, o_lo), a.fwd_iters, 4.0),
+               "attention_bwd": (lambda h=heads, l=lse, dl=delta: be.attention_bwd(qkv, out, dout, h, 0, dqkv, l, dl),
+                                 a.bwd_iters, 10.0),
+               "attention": (lambda h=heads: be.attention(qkv, h, 0, out, None, None), a.fwd_iters, 4.0),
+               "attention_split": (lambda h=heads: be.attention_split(hi, lo, h, 0, None, o_hi, o_lo), a.fwd_iters, 4.0)}
+        if "attention_bwd" in a.kernels:
+            be.attention_tc(hi, lo, heads, 0, out, None, None)     # the forward output the backward is given
+        for k in a.kernels:
+            fns[k][0]()                                            # warm up every shape timed below
+            runs.append((k, d, heads, *fns[k], []))
         torch.cuda.synchronize()
-        runs[d] = (heads, fwd, bwd, {"fwd": [], "bwd": []})
     info = card()
     for _ in range(a.rounds):                                      # alternate the variants
-        for d, (heads, fwd, bwd, ms) in runs.items():
-            ms["fwd"].append(event_ms(fwd, a.fwd_iters))
-            ms["bwd"].append(event_ms(bwd, a.bwd_iters))
+        for k, d, heads, fn, iters, fl, ms in runs:
+            ms.append(event_ms(fn, iters))
     be.check_fault()
 
     lines = []
-    for d, (heads, _, _, ms) in runs.items():
-        for kern, key, fl in (("attention_tc", "fwd", 4.0), ("attention_bwd", "bwd", 10.0)):
-            med = statistics.median(ms[key])
-            lines.append(json.dumps({"kernel": kern, "B": B, "T": T, "C": C, "heads": heads, "head_dim": d,
-                                     "ms": round(med, 4), "ms_rounds": [round(x, 4) for x in ms[key]],
-                                     "algo_tflops": round(fl * B * T * T * C / med / 1e9, 2), **info}))
+    for k, d, heads, fn, iters, fl, ms in runs:
+        med = statistics.median(ms)
+        lines.append(json.dumps({"kernel": k, "B": B, "T": T, "C": C, "heads": heads, "head_dim": d,
+                                 "ms": round(med, 4), "ms_rounds": [round(x, 4) for x in ms],
+                                 "algo_tflops": round(fl * B * T * T * C / med / 1e9, 2), **info}))
     for ln in lines:
         print(ln)
     if a.out:
