@@ -34,6 +34,7 @@ SYMBOLS = [
     "bbdm_split_grad", "bbdm_conv_wgrad_workspace", "bbdm_conv_wgrad", "bbdm_gn_bwd_reduce", "bbdm_gn_bwd_apply",
     "bbdm_conv_wgrad_direct", "bbdm_attention_bwd", "bbdm_conv_direct_pad", "bbdm_softmax_rows_split", "bbdm_vq_nearest", "bbdm_s2d_split", "bbdm_pack_weight_split_both",
     "bbdm_wino_geometry", "bbdm_wino_input", "bbdm_wino_output", "bbdm_wino_pack_weight",
+    "bbdm_wino6_geometry", "bbdm_wino6_input", "bbdm_wino6_output", "bbdm_wino6_pack_weight",
     "bbdm_optim_chunk_elems", "bbdm_adam_multi", "bbdm_ema_multi", "bbdm_denorm_to_uint8",
     "bbdm_layernorm_split", "bbdm_geglu_split", "bbdm_attention_cross", "bbdm_conv_stem", "bbdm_spatial_rescale",
 ]
@@ -145,6 +146,10 @@ def load():
     lib.bbdm_wino_input.argtypes = [C.POINTER(WinoInputArgs), vp]
     lib.bbdm_wino_output.argtypes = [C.POINTER(WinoOutputArgs), vp]
     lib.bbdm_wino_pack_weight.argtypes = [vp, i, i, i, vp, vp, vp, vp]
+    lib.bbdm_wino6_geometry.argtypes = lib.bbdm_wino_geometry.argtypes
+    lib.bbdm_wino6_input.argtypes = lib.bbdm_wino_input.argtypes
+    lib.bbdm_wino6_output.argtypes = lib.bbdm_wino_output.argtypes
+    lib.bbdm_wino6_pack_weight.argtypes = lib.bbdm_wino_pack_weight.argtypes
     lib.bbdm_denorm_to_uint8.argtypes = [vp, i, i, i, i, i, vp, vp]
     lib.bbdm_spatial_rescale.argtypes = [vp, i, i, i, i, i, vp, vp, i, vp, vp]
     lib.bbdm_layernorm_split.argtypes = [vp, i64, i, vp, vp, f, vp, vp, vp, vp]
@@ -231,6 +236,8 @@ class CudaBackend:
     # wino_pack_weight / wino_output take inv_wscale: per-tensor power-of-two scales of the Winograd weight planes
     # (a backend without it packs at the fixed 2^8, and the engines call it without a scale)
     wino_tensor_scale = True
+    # Winograd output tile sizes: F(4x4,3x3) and F(6x6,3x3) (the wino_* methods' tile argument)
+    wino_tiles = (4, 6)
 
     def __init__(self):
         self.lib = load()
@@ -360,41 +367,45 @@ class CudaBackend:
         check(self.lib.bbdm_conv_umma_geometry(H, W, *[C.byref(z) for z in v]))
         return tuple(z.value for z in v)
 
-    # -- Winograd F(4x4,3x3) path ------------------------------------------------------------------
-    def wino_geometry(self, B, H, W):
-        """(tiles_h, tiles_w, tiles_total, eligible)."""
+    # -- Winograd F(4x4,3x3) / F(6x6,3x3) path ------------------------------------------------------
+    def _wino(self, name, tile):
+        assert tile in self.wino_tiles, tile
+        return getattr(self.lib, f"bbdm_wino{'' if tile == 4 else tile}_{name}")
+
+    def wino_geometry(self, B, H, W, tile=4):
+        """(tiles_h, tiles_w, tiles_total, eligible); F(6,3): tiles_total padded to a multiple of 16."""
         th, tw, el, tot = C.c_int(0), C.c_int(0), C.c_int(0), C.c_int64(0)
-        check(self.lib.bbdm_wino_geometry(B, H, W, C.byref(th), C.byref(tw), C.byref(tot), C.byref(el)))
+        check(self._wino("geometry", tile)(B, H, W, C.byref(th), C.byref(tw), C.byref(tot), C.byref(el)))
         return th.value, tw.value, tot.value, bool(el.value)
 
     def wino_input(self, src1, src2, *, groups=32, mean=None, rstd=None, gamma=None, beta=None, film_scale=None,
                    film_shift=None, film_stride=0, silu=True, v_hi, v_lo, raw_hi=None, raw_lo=None, act_hi=None,
-                   act_lo=None):
+                   act_lo=None, tile=4):
         B, H, W, c1 = src1.shape
         a = WinoInputArgs(ptr(_req(src1)), c1, ptr(src2), 0 if src2 is None else src2.shape[3], B, H, W, groups,
                           ptr(mean), ptr(rstd), ptr(gamma), ptr(beta), ptr(film_scale), ptr(film_shift), film_stride,
                           int(silu), ptr(_req(v_hi, torch.float16)), ptr(_req(v_lo, torch.float16)),
                           ptr(raw_hi), ptr(raw_lo), ptr(act_hi), ptr(act_lo))
-        check(self.lib.bbdm_wino_input(C.byref(a), stream()))
+        check(self._wino("input", tile)(C.byref(a), stream()))
         LAUNCHES["n"] += 1
 
     def wino_output(self, m, *, B, H, W, Cout, bias=None, residual=None, res_mode=RES_NONE, out, stats_partial=None,
-                    inv_wscale=None):
+                    inv_wscale=None, tile=4):
         """inv_wscale: the [1] fp32 device tensor wino_pack_weight wrote for the weight planes of this GEMM (None:
         planes packed at the fixed 2^8)."""
         a = WinoOutputArgs(ptr(_req(m)), None if inv_wscale is None else ptr(_req(inv_wscale)), B, H, W, Cout, ptr(bias), ptr(residual), res_mode, ptr(_req(out)),
                            ptr(stats_partial))
-        check(self.lib.bbdm_wino_output(C.byref(a), stream()))
+        check(self._wino("output", tile)(C.byref(a), stream()))
         LAUNCHES["n"] += 1
 
-    def wino_pack_weight(self, w, u_hi, u_lo, dgrad=False, inv_wscale=None):
-        """w [Cout,Cin,3,3] fp32 -> u_hi/u_lo fp16 [36, Cout, Cin] (s * G w G^T); dgrad: [36, Cin, Cout] of the
-        flipped / channel-swapped kernel.  inv_wscale [1] fp32 on the device: s is the per-tensor power of two and
-        1/s is written there (pass it to wino_output); None: the fixed s = 2^8."""
+    def wino_pack_weight(self, w, u_hi, u_lo, dgrad=False, inv_wscale=None, tile=4):
+        """w [Cout,Cin,3,3] fp32 -> u_hi/u_lo fp16 [(tile+2)^2, Cout, Cin] (s * G w G^T); dgrad: [.., Cin, Cout] of
+        the flipped / channel-swapped kernel.  inv_wscale [1] fp32 on the device: s is the per-tensor power of two
+        and 1/s is written there (pass it to wino_output); None: the fixed s = 2^8."""
         Cout, Cin = w.shape[0], w.shape[1]
-        check(self.lib.bbdm_wino_pack_weight(ptr(_req(w)), Cout, Cin, int(dgrad), ptr(_req(u_hi, torch.float16)),
-                                             ptr(_req(u_lo, torch.float16)),
-                                             None if inv_wscale is None else ptr(_req(inv_wscale)), stream()))
+        check(self._wino("pack_weight", tile)(ptr(_req(w)), Cout, Cin, int(dgrad), ptr(_req(u_hi, torch.float16)),
+                                              ptr(_req(u_lo, torch.float16)),
+                                              None if inv_wscale is None else ptr(_req(inv_wscale)), stream()))
         LAUNCHES["n"] += 1
 
     # -- SpatialTransformer pieces --------------------------------------------------------------------------

@@ -32,13 +32,25 @@ def wino_channels_ok(cin, cout, min_c):
     return cin % 64 == 0 and cout % 64 == 0 and min(cin, cout) >= min_c
 
 
-def winograd_ok(geometry, cin, cout, min_c, min_tiles):
+def wino_tile(H, W):
+    """Output tile size of the sampling executor's Winograd convs at an HxW map: 6 (F(6x6,3x3), 64 transform
+    positions per 6x6 tile, edge tiles zero-padded) where its position-GEMM MACs are at most 0.9x those of F(4x4,3x3)
+    (36 positions per 4x4 tile): 48x48 and larger maps (0.84x at 64x64 and 128x128, 0.80x at 256x256), else 4
+    (32x32: 1.11x)."""
+    f6 = 64 * (-(-H // 6)) * (-(-W // 6))
+    f4 = 36 * (H / 4) * (W / 4)
+    return 6 if f6 <= 0.9 * f4 else 4
+
+
+def winograd_ok(geometry, cin, cout, min_c, min_tiles, tile=4):
     """Whether a stride-1 3x3 conv of cin -> cout channels takes the Winograd path; geometry is the backend's
-    wino_geometry(B, H, W).  At >= 128 tiles per image always (the choice must not depend on the batch size there:
-    batch-size independent, bit-identical results at the pixel resolutions); smaller maps only when the whole batch
-    has enough tiles."""
+    wino_geometry(B, H, W, tile).  The size clauses count output pixels of the tile grid (tile^2 per tile), so they mean
+    the same at both tile sizes: at >= 128 F(4,3) tiles' worth of pixels per image always (the choice must not depend
+    on the batch size there: batch-size independent, bit-identical results at the pixel resolutions); smaller maps
+    only when the whole batch has min_tiles F(4,3) tiles' worth."""
     th, tw, tiles, ok = geometry
-    return bool(ok and wino_channels_ok(cin, cout, min_c) and (th * tw >= 128 or tiles >= min_tiles))
+    px = tile * tile
+    return bool(ok and wino_channels_ok(cin, cout, min_c) and (th * tw * px >= 128 * 16 or tiles * px >= min_tiles * 16))
 
 
 class FreshBuffers:
@@ -56,34 +68,38 @@ class FreshBuffers:
 
 
 def wino_conv(be, pool, geometry, src1, src2, *, cout, planes=None, weight=None, dgrad=False, bias=None,
-              residual=None, res_mode=cabi.RES_NONE, stats=False, **transform):
+              residual=None, res_mode=cabi.RES_NONE, stats=False, tile=4, **transform):
     """3x3 conv of cat(src1, src2) (NHWC fp32) on the Winograd path: input transform (``transform`` are the
     wino_input arguments: GroupNorm affine + FiLM + SiLU, or identity with silu=False; raw_* / act_* side outputs) ->
-    36 position GEMMs in one wgmma launch -> output transform (+ bias, + residual, + GroupNorm partial sums if stats).
+    (tile+2)^2 position GEMMs in one wgmma launch -> output transform (+ bias, + residual, + GroupNorm partial sums if
+    stats).  tile: 4 (F(4x4,3x3)) or 6 (F(6x6,3x3)); geometry is the backend's wino_geometry for that tile.
 
-    planes = (u_hi, u_lo, u_inv) packed beforehand (WeightPacker.winograd), or weight [Cout, Cin, 3, 3] to pack here
-    (dgrad: the flipped, channel-swapped kernel).  pool: the executors' _Pool or FreshBuffers."""
+    planes = (u_hi, u_lo, u_inv) packed beforehand (WeightPacker.winograd, same tile), or weight [Cout, Cin, 3, 3] to
+    pack here (dgrad: the flipped, channel-swapped kernel).  pool: the executors' _Pool or FreshBuffers."""
     B, H, W, c1 = src1.shape
     cin = c1 + (0 if src2 is None else src2.shape[3])
     th, _, mtot, _ = geometry
-    v_hi, v_lo = pool.get((36, mtot, cin), torch.float16), pool.get((36, mtot, cin), torch.float16)
-    be.wino_input(src1, src2, v_hi=v_hi, v_lo=v_lo, **transform)
+    npos = (tile + 2) ** 2
+    tkw = {} if tile == 4 else dict(tile=tile)
+    v_hi, v_lo = pool.get((npos, mtot, cin), torch.float16), pool.get((npos, mtot, cin), torch.float16)
+    be.wino_input(src1, src2, v_hi=v_hi, v_lo=v_lo, **transform, **tkw)
     if planes is None:
-        u_hi, u_lo = pool.get((36, cout, cin), torch.float16), pool.get((36, cout, cin), torch.float16)
+        u_hi, u_lo = pool.get((npos, cout, cin), torch.float16), pool.get((npos, cout, cin), torch.float16)
         # per-tensor scale of the planes: 1/s stays on the device (no host synchronisation)
         u_inv = pool.get((1,)) if getattr(be, "wino_tensor_scale", False) else None
         be.wino_pack_weight(weight.detach().contiguous(), u_hi, u_lo, dgrad=dgrad,
-                            **({} if u_inv is None else dict(inv_wscale=u_inv)))
+                            **({} if u_inv is None else dict(inv_wscale=u_inv)), **tkw)
     else:
         u_hi, u_lo, u_inv = planes
-    m = pool.get((36, mtot, cout))
-    be.conv_umma(B=36, H=mtot // 16, W=16, Cin=cin, Cout=cout, taps=1, a_hi=v_hi, a_lo=v_lo, w_hi=u_hi, w_lo=u_lo,
+        assert u_hi.shape[0] == npos, (u_hi.shape, tile)
+    m = pool.get((npos, mtot, cout))
+    be.conv_umma(B=npos, H=mtot // 16, W=16, Cin=cin, Cout=cout, taps=1, a_hi=v_hi, a_lo=v_lo, w_hi=u_hi, w_lo=u_lo,
                  out=m, passes=3, weights_per_image=True, operand_f16=True)
     pool.put(v_hi, v_lo)
     out = pool.get((B, H, W, cout))
     part = pool.get((B * th, cout, 2)) if stats else None
     be.wino_output(m, B=B, H=H, W=W, Cout=cout, bias=bias, residual=residual, res_mode=res_mode, out=out,
-                   stats_partial=part, **({} if u_inv is None else dict(inv_wscale=u_inv)))
+                   stats_partial=part, **({} if u_inv is None else dict(inv_wscale=u_inv)), **tkw)
     pool.put(m)
     if part is not None:
         out._gn = (part, th)
@@ -140,13 +156,16 @@ class WeightPacker:
         self.w[name] = ent
         return ent
 
-    def winograd(self, name, weight):
-        """Winograd-domain planes U = s G g G^T of the packed 3x3 conv ``name``, fp16 hi/lo [36][Cout][Cin], and 1/s
-        (per-tensor power of two) as a device scalar beside them: a stable address for graph replay."""
+    def winograd(self, name, weight, tile=4):
+        """Winograd-domain planes U = s G g G^T of the packed 3x3 conv ``name`` for F(tile x tile, 3x3), fp16 hi/lo
+        [(tile+2)^2][Cout][Cin], and 1/s (per-tensor power of two) as a device scalar beside them: a stable address for
+        graph replay.  ent["u_tile"] records the tile size."""
         ent = self.w[name]
-        ent["u_hi"] = self._buf(name, "u_hi", (36, ent["cout"], ent["cin"]), torch.float16)
-        ent["u_lo"] = self._buf(name, "u_lo", (36, ent["cout"], ent["cin"]), torch.float16)
-        skw = {}
+        npos = (tile + 2) ** 2
+        ent["u_hi"] = self._buf(name, "u_hi", (npos, ent["cout"], ent["cin"]), torch.float16)
+        ent["u_lo"] = self._buf(name, "u_lo", (npos, ent["cout"], ent["cin"]), torch.float16)
+        ent["u_tile"] = tile
+        skw = {} if tile == 4 else dict(tile=tile)
         if getattr(self.be, "wino_tensor_scale", False):
             ent["u_inv"] = skw["inv_wscale"] = self._buf(name, "u_inv", (1,), torch.float32)
         self.be.wino_pack_weight(weight.detach().contiguous(), ent["u_hi"], ent["u_lo"], **skw)

@@ -58,6 +58,9 @@ int bbdm_check_device_fault(void* stream, unsigned long long* fault_word) {
   if (h) {
     if ((h >> 28) == 0xBull)
       bbdm::set_error("device fault word 0x%llx: timestep index out of range (the reference's gather raises IndexError)", h);
+    else if ((h >> 28) == 0xCull)
+      bbdm::set_error("device fault word 0x%llx: Winograd F(6x6,3x3) input transform of a %llu-channel conv left the "
+                      "fp16 range (activations above ~290, or non-finite)", h, h & 0xFFFFFFFull);
     else
       bbdm::set_error("device fault word 0x%llx (kernel-side wait timeout)", h);
     return BBDM_E_DEVICE;

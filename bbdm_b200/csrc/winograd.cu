@@ -16,6 +16,12 @@
 //                       2x2-avg addressed) -> fp32 NHWC + fused GroupNorm partial sums of the result.
 //                       HBM-bound: 36/16 * 4 B read + 4 B written per output element.
 //
+// F(6x6, 3x3) (interpolation points 0, +-1, +-2, +-1/2; bbdm_wino6_*): the same three kernels over 8x8 input tiles at
+// stride 6 and 64 position GEMMs -- 64/36 positions per 36/16 output pixels, 0.79x the MACs and the V / M bytes of
+// F(4,3), for the large maps of the UNet sampling executor (convs.wino_tile).  Its transforms amplify rounding more
+// (tools/studies/winograd_f63_accuracy.py: the chain sits at the direct split-bf16 kernel's deviation, about 1.5x
+// F(4,3)'s) and B^T d B grows a tile by up to 225 (F(4,3): 100), so fp16 V is finite for max|act| <= 291.
+//
 // Numerics (tools/studies/split_formats_accuracy.py): split-FP16 operands carry 22 mantissa bits (bf16 pairs: 16),
 // which pays for the F(4,3) transforms' error amplification; the GEMM promotes the tensor core's truncating
 // accumulator into fp32 registers every 2-4 K-blocks (conv_umma.cu), and tests/test_gpu_winograd.py bounds the chain's
@@ -68,6 +74,38 @@ __host__ __device__ __forceinline__ void wino_at6(const float* m, float* y) {
   y[3 * T] = fmaf(8.0f, d34, d12) + m[5 * S];
 }
 
+// ---- F(6x6,3x3): interpolation points 0, +-1, +-2, +-1/2 (and infinity) -----------------------
+// B^T (8x8) applied to d[0..7] with stride S.  Absolute row sums reach 15 (F(4,3): 10): |V| <= 225 max|d|.
+template <int S>
+__device__ __forceinline__ void wino_bt8(float* d) {
+  const float d0 = d[0], d1 = d[S], d2 = d[2 * S], d3 = d[3 * S], d4 = d[4 * S], d5 = d[5 * S], d6 = d[6 * S],
+              d7 = d[7 * S];
+  const float e1 = fmaf(-4.25f, d4, d2 + d6), o1 = fmaf(-4.25f, d3, d1 + d5);
+  const float e3 = fmaf(0.25f, d2, fmaf(-1.25f, d4, d6)), o3 = fmaf(0.5f, d1, fmaf(-2.5f, d3, 2.0f * d5));
+  const float e5 = fmaf(4.0f, d2, fmaf(-5.0f, d4, d6)), o5 = fmaf(2.0f, d1, fmaf(-2.5f, d3, 0.5f * d5));
+  d[0] = fmaf(5.25f, d4 - d2, d0 - d6);
+  d[S] = e1 + o1;
+  d[2 * S] = e1 - o1;
+  d[3 * S] = e3 + o3;
+  d[4 * S] = e3 - o3;
+  d[5 * S] = e5 + o5;
+  d[6 * S] = e5 - o5;
+  d[7 * S] = fmaf(5.25f, d3 - d5, d7 - d1);
+}
+// A^T (6x8) applied to m[0..7] (stride S) -> y[0..5] (stride T)
+template <int S, int T>
+__host__ __device__ __forceinline__ void wino_at8(const float* m, float* y) {
+  const float a = m[S] + m[2 * S], b = m[S] - m[2 * S];
+  const float c = m[3 * S] + m[4 * S], d = m[3 * S] - m[4 * S];
+  const float e = m[5 * S] + m[6 * S], f = m[5 * S] - m[6 * S];
+  y[0] = ((m[0] + a) + c) + e;
+  y[T] = fmaf(2.0f, d, fmaf(0.5f, f, b));
+  y[2 * T] = fmaf(4.0f, c, fmaf(0.25f, e, a));
+  y[3 * T] = fmaf(8.0f, d, fmaf(0.125f, f, b));
+  y[4 * T] = fmaf(16.0f, c, fmaf(0.0625f, e, a));
+  y[5 * T] = fmaf(32.0f, d, fmaf(0.03125f, f, b)) + m[7 * S];
+}
+
 __device__ __forceinline__ void split2_f16(float a, float b, uint32_t& hi, uint32_t& lo) {
   const __half2 h = __floats2half2_rn(a, b);
   const float2 hf = __half22float2(h);
@@ -81,14 +119,17 @@ struct WinoInParams {
   const float* src1; int c1;
   const float* src2; int c2;
   int B, H, W, C, groups, cpg, th, tw;
-  int64_t Mtot;
+  int64_t Mtot;              // rows of the V planes: B*th*tw tiles (F(6,3): padded to a multiple of 16, zero rows)
   const float* mean; const float* rstd; const float* gamma; const float* beta;
   const float* fscale; const float* fshift; int64_t fstride;
   int silu;
   __half* v_hi; __half* v_lo;
   __nv_bfloat16* raw_hi; __nv_bfloat16* raw_lo;
   __nv_bfloat16* act_hi; __nv_bfloat16* act_lo;   // optional split-bf16 planes of the ACTIVATED tensor (wgrad operand)
+  unsigned long long* fault;   // F(6,3): device fault word, set when a V value is not a finite fp16 number
 };
+
+constexpr unsigned long long WINO6_RANGE_FAULT = 0xC0000000ull;   // | C: channel count of the failing launch
 
 // One CTA per (sample b, tile row ty, chunk of 256*VEC channels): every thread owns VEC channels and walks the tile
 // row left to right, keeping the two activated pixel columns it shares with the next tile in registers (24 instead of
@@ -211,35 +252,59 @@ wino_input_kernel(const WinoInParams p) {
 
 // ------------------------------------------------------------------------------------------
 // Shared-memory staged input transform (the default): one CTA per (sample b, tile row ty, 64-channel chunk) walks the
-// tile row in segments of 8 tiles.  Per segment: (1) cp.async stages the 6 x 34 pixel x 64 channel input patch
-// (double buffered: the next segment's loads fly while this one is transformed -- the register variant above is
-// bound by exposed load latency, ncu: 65 % long-scoreboard stalls, 29 % issue utilisation); (2) every pixel is
+// tile row in segments of TX tiles.  Per segment: (1) cp.async stages the N x (T*TX+2) pixel x 64 channel input patch
+// (N = T+2 rows; double buffered: the next segment's loads fly while this one is transformed -- the register variant
+// above is bound by exposed load latency, ncu: 65 % long-scoreboard stalls, 29 % issue utilisation); (2) every pixel is
 // activated ONCE in place (GroupNorm affine x FiLM, SiLU; out-of-image pixels become exact zeros = the conv padding
-// of the activated tensor); (3) thread (tile, channel pair) reads its 6x6 tile with conflict-free 8-byte LDS,
-// transforms, splits to fp16 hi/lo and stores (128 contiguous bytes per warp, position and plane).
-constexpr int WI_CC = 64;                 // channels per CTA
-constexpr int WI_TX = 8;                  // tiles per segment
-constexpr int WI_COLS = 4 * WI_TX + 2;    // patch columns
-constexpr int WI_PATCH = 6 * WI_COLS * WI_CC;          // floats per buffer
-constexpr size_t WI_SMEM = 2 * (size_t)WI_PATCH * sizeof(float);
+// of the activated tensor); (3) F(4,3): thread (tile, channel pair) reads its 6x6 tile with conflict-free 8-byte LDS,
+// transforms, splits to fp16 hi/lo and stores (128 contiguous bytes per warp, position and plane).  F(6,3): thread
+// (tile, channel) does the same for its 8x8 tile (64 floats of state, not 128: the kernel stays spill-free at 2 CTAs
+// per SM), 64 contiguous bytes per warp, position and plane.
+template <int T>
+struct WinoIn {
+  static constexpr int N = T + 2;                    // input tile side
+  static constexpr int CC = 64;                      // channels per CTA
+  static constexpr int TX = T == 4 ? 8 : 4;          // tiles per segment: 256 threads in phase 3, 2 buffers x 2 CTAs/SM
+  static constexpr int COLS = T * TX + 2;            // patch columns (>= 16: phases 1/2 step 16 pixels at a time)
+  static constexpr int PATCH = N * COLS * CC;        // floats per buffer
+  static constexpr size_t SMEM = 2 * (size_t)PATCH * sizeof(float);
+};
+static_assert(WinoIn<4>::SMEM == 2 * 6 * 34 * 64 * 4 && WinoIn<6>::SMEM * 2 <= 227 * 1024, "staged patch budget");
 
 __device__ __forceinline__ void cp_async16(uint32_t saddr, const void* g) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(saddr), "l"(g) : "memory");
 }
 
+template <int T>
 __global__ void __launch_bounds__(256, 2)
 wino_input_smem_kernel(const WinoInParams p) {
-  extern __shared__ __align__(16) float patch[];          // [2][6][WI_COLS][WI_CC]
+  using K = WinoIn<T>;
+  constexpr int N = K::N, CC = K::CC, TX = K::TX, COLS = K::COLS;
+  extern __shared__ __align__(16) float patch[];          // [2][N][COLS][CC]
   const int b = blockIdx.x / p.th, ty = blockIdx.x % p.th;
-  const int cbase = blockIdx.y * WI_CC;                    // first channel of this CTA (in the concatenation)
+  const int cbase = blockIdx.y * CC;                       // first channel of this CTA (in the concatenation)
   const float* base;
   int cs, cc0;
   if (cbase < p.c1) { base = p.src1; cs = p.c1; cc0 = cbase; } else { base = p.src2; cs = p.c2; cc0 = cbase - p.c1; }
-  const int y0 = 4 * ty - 1;
+  const int y0 = T * ty - 1;
   const int tid = threadIdx.x;
   const int ch4 = tid & 15;                                // this thread's 4-channel group in phases 1/2
   const int pix0 = tid >> 4;                               // first patch pixel of this thread (stride 16 pixels)
-  constexpr int NPIX = 6 * WI_COLS;                        // 204 pixels per patch
+  constexpr int NPIX = N * COLS;                           // pixels per patch
+
+  if constexpr (T == 6) {
+    // the GEMM's padding rows (tile count rounded up to 16): exact zeros, written by the CTAs of tile row 0
+    if (blockIdx.x == 0) {
+      const int64_t tiles = (int64_t)p.B * p.th * p.tw;
+      const int npad = (int)(p.Mtot - tiles);
+      for (int k = tid; k < N * N * npad * CC; k += 256) {
+        const int c = k % CC, r = (k / CC) % npad, q = k / (CC * npad);
+        const int64_t off = ((int64_t)q * p.Mtot + tiles + r) * p.C + cbase + c;
+        p.v_hi[off] = __float2half_rn(0.f);
+        p.v_lo[off] = __float2half_rn(0.f);
+      }
+    }
+  }
 
   // GroupNorm affine x FiLM for the 4 channels this thread activates
   float sc[4], sh[4];
@@ -257,17 +322,17 @@ wino_input_smem_kernel(const WinoInParams p) {
       sh[v] = fmaf(h0, f1, f0);
     }
   }
-  const int nseg = (p.tw + WI_TX - 1) / WI_TX;
+  const int nseg = (p.tw + TX - 1) / TX;
   const uint32_t patch_s = (uint32_t)__cvta_generic_to_shared(patch);
 
   auto stage = [&](int seg, int buf) {
-    const int x0 = 4 * WI_TX * seg - 1;
-    int i = 0, j = pix0;                                  // pix0 < 16 < WI_COLS: row 0
+    const int x0 = T * TX * seg - 1;
+    int i = 0, j = pix0;                                  // pix0 < 16 <= COLS: row 0
     for (int px = pix0; px < NPIX; px += 16, j += 16) {
-      if (j >= WI_COLS) { j -= WI_COLS; ++i; }
+      if (j >= COLS) { j -= COLS; ++i; }
       const int iy = y0 + i, ix = x0 + j;
       if (iy >= 0 && iy < p.H && ix >= 0 && ix < p.W)
-        cp_async16(patch_s + (uint32_t)(((buf * NPIX + px) * WI_CC + ch4 * 4) * 4),
+        cp_async16(patch_s + (uint32_t)(((buf * NPIX + px) * CC + ch4 * 4) * 4),
                    base + (((int64_t)b * p.H + iy) * p.W + ix) * cs + cc0 + ch4 * 4);
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
@@ -283,18 +348,18 @@ wino_input_smem_kernel(const WinoInParams p) {
       asm volatile("cp.async.wait_group 0;" ::: "memory");
     }
     __syncthreads();
-    float* pb = patch + buf * WI_PATCH;
-    const int x0 = 4 * WI_TX * seg - 1;
+    float* pb = patch + buf * K::PATCH;
+    const int x0 = T * TX * seg - 1;
     // ---- phase 2: activate every staged pixel once, in place ------------------------------------------------
     int i = 0, j = pix0;
     for (int px = pix0; px < NPIX; px += 16, j += 16) {
-      if (j >= WI_COLS) { j -= WI_COLS; ++i; }
+      if (j >= COLS) { j -= COLS; ++i; }
       const int iy = y0 + i, ix = x0 + j;
-      float4* q = reinterpret_cast<float4*>(pb + px * WI_CC + ch4 * 4);
+      float4* q = reinterpret_cast<float4*>(pb + px * CC + ch4 * 4);
       float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
       if (iy >= 0 && iy < p.H && ix >= 0 && ix < p.W) {
         const float4 x = *q;
-        if (p.raw_hi && i >= 1 && i <= 4 && j >= 1 && j <= 4 * WI_TX) {
+        if (p.raw_hi && i >= 1 && i <= T && j >= 1 && j <= T * TX) {
           // pixels this segment owns: raw split-bf16 planes for the 1x1 skip conv
           uint2 h, l;
           split4(x, h, l);
@@ -308,7 +373,7 @@ wino_input_smem_kernel(const WinoInParams p) {
           a.x = __fdividef(a.x, 1.0f + __expf(-a.x)); a.y = __fdividef(a.y, 1.0f + __expf(-a.y));
           a.z = __fdividef(a.z, 1.0f + __expf(-a.z)); a.w = __fdividef(a.w, 1.0f + __expf(-a.w));
         }
-        if (p.act_hi && i >= 1 && i <= 4 && j >= 1 && j <= 4 * WI_TX) {
+        if (p.act_hi && i >= 1 && i <= T && j >= 1 && j <= T * TX) {
           // training: the activated tensor's split-bf16 planes are the weight-gradient GEMM's operand
           uint2 h, l;
           split4(a, h, l);
@@ -320,35 +385,66 @@ wino_input_smem_kernel(const WinoInParams p) {
       *q = a;                                              // out of the image: exact zero (padding of the activation)
     }
     __syncthreads();
-    // ---- phase 3: one (tile, channel pair) per thread -------------------------------------------------------
-    const int txl = tid >> 5, c0 = (tid & 31) * 2;
-    const int tx = WI_TX * seg + txl;
-    if (tx < p.tw) {
-      float t0[36], t1[36];
+    // ---- phase 3: one (tile, channel pair) [F(4,3)] or (tile, channel) [F(6,3)] per thread ----------------------
+    const int64_t plane = p.Mtot * p.C;
+    if constexpr (T == 4) {
+      const int txl = tid >> 5, c0 = (tid & 31) * 2;
+      const int tx = TX * seg + txl;
+      if (tx < p.tw) {
+        float t0[36], t1[36];
 #pragma unroll
-      for (int i = 0; i < 6; ++i)
+        for (int i = 0; i < 6; ++i)
 #pragma unroll
-        for (int j = 0; j < 6; ++j) {
-          const float2 v = *reinterpret_cast<const float2*>(pb + ((i * WI_COLS + 4 * txl + j) * WI_CC + c0));
-          t0[i * 6 + j] = v.x;
-          t1[i * 6 + j] = v.y;
+          for (int j = 0; j < 6; ++j) {
+            const float2 v = *reinterpret_cast<const float2*>(pb + ((i * COLS + 4 * txl + j) * CC + c0));
+            t0[i * 6 + j] = v.x;
+            t1[i * 6 + j] = v.y;
+          }
+#pragma unroll
+        for (int j = 0; j < 6; ++j) { wino_bt6<6>(t0 + j); wino_bt6<6>(t1 + j); }
+#pragma unroll
+        for (int i = 0; i < 6; ++i) { wino_bt6<1>(t0 + 6 * i); wino_bt6<1>(t1 + 6 * i); }
+        const int64_t m = ((int64_t)b * p.th + ty) * p.tw + tx;
+        __half* ph = p.v_hi + m * p.C + cbase + c0;
+        __half* pl = p.v_lo + m * p.C + cbase + c0;
+#pragma unroll
+        for (int q = 0; q < 36; ++q) {
+          uint32_t h, l;
+          split2_f16(t0[q], t1[q], h, l);
+          *reinterpret_cast<uint32_t*>(ph) = h;
+          *reinterpret_cast<uint32_t*>(pl) = l;
+          ph += plane;
+          pl += plane;
         }
+      }
+    } else {
+      const int txl = tid >> 6, c = tid & 63;
+      const int tx = TX * seg + txl;
+      if (tx < p.tw) {
+        float t[64];
 #pragma unroll
-      for (int j = 0; j < 6; ++j) { wino_bt6<6>(t0 + j); wino_bt6<6>(t1 + j); }
+        for (int i = 0; i < 8; ++i)
 #pragma unroll
-      for (int i = 0; i < 6; ++i) { wino_bt6<1>(t0 + 6 * i); wino_bt6<1>(t1 + 6 * i); }
-      const int64_t m = ((int64_t)b * p.th + ty) * p.tw + tx;
-      const int64_t plane = p.Mtot * p.C;
-      __half* ph = p.v_hi + m * p.C + cbase + c0;
-      __half* pl = p.v_lo + m * p.C + cbase + c0;
+          for (int j = 0; j < 8; ++j) t[i * 8 + j] = pb[(i * COLS + 6 * txl + j) * CC + c];
 #pragma unroll
-      for (int q = 0; q < 36; ++q) {
-        uint32_t h, l;
-        split2_f16(t0[q], t1[q], h, l);
-        *reinterpret_cast<uint32_t*>(ph) = h;
-        *reinterpret_cast<uint32_t*>(pl) = l;
-        ph += plane;
-        pl += plane;
+        for (int j = 0; j < 8; ++j) wino_bt8<8>(t + j);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) wino_bt8<1>(t + 8 * i);
+        const int64_t m = ((int64_t)b * p.th + ty) * p.tw + tx;
+        __half* ph = p.v_hi + m * p.C + cbase + c;
+        __half* pl = p.v_lo + m * p.C + cbase + c;
+        // |V| <= 225 max|act|: past max|act| ~ 291 the fp16 planes overflow -- reported, never silent
+        bool finite = true;
+#pragma unroll
+        for (int q = 0; q < 64; ++q) {
+          const __half h = __float2half_rn(t[q]);
+          finite &= fabsf(t[q]) < 65520.0f;              // rounds to at most 65504 (false for NaN too)
+          *ph = h;
+          *pl = __float2half_rn(t[q] - __half2float(h));
+          ph += plane;
+          pl += plane;
+        }
+        if (!finite) atomicExch(p.fault, WINO6_RANGE_FAULT | (unsigned)(p.C & 0xFFFFFFF));
       }
     }
     __syncthreads();          // all reads of this buffer done before the cp.async of segment seg+2 lands in it
@@ -467,6 +563,97 @@ wino_output_kernel(const WinoOutParams p) {
   }
 }
 
+// F(6x6,3x3): one output tile (6x6 pixels) of ONE channel (64 M values instead of 2 x 36: one channel per thread keeps
+// the F(4,3) kernel's register budget).  Tiles run over ceil(H/6) x ceil(W/6): pixels, residual reads and partial sums
+// past H or W are masked.  __host__ __device__: tools/host_check_wino6_output.cu runs it on the CPU.
+template <int RES>
+__host__ __device__ __forceinline__ void wino6_output_tile(const WinoOutParams& p, int b, int ty, int tx, int c, float bv,
+                                                           float inv, float& sum, float& sq) {
+  const int64_t m = ((int64_t)b * p.th + ty) * p.tw + tx;
+  float mm[64];
+#pragma unroll
+  for (int q = 0; q < 64; ++q) mm[q] = p.m[((int64_t)q * p.Mtot + m) * p.Cout + c];
+  // Y = A^T M A: columns (8 -> 6 rows), then rows (8 -> 6 columns)
+  float t6[48], y[36];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) wino_at8<8, 8>(mm + j, t6 + j);
+#pragma unroll
+  for (int i = 0; i < 6; ++i) wino_at8<1, 1>(t6 + 8 * i, y + 6 * i);
+  const int h0 = 6 * ty, w0 = 6 * tx;
+  float rup[RES == BBDM_RES_UP2 ? 9 : 1];
+  if constexpr (RES == BBDM_RES_UP2) {
+    // output pixels (6ty+i, 6tx+j) read source pixel (3ty + i/2, 3tx + j/2): 3x3 distinct values per tile
+    const int H2 = p.H >> 1, W2 = p.W >> 1;
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int j = 0; j < 3; ++j)
+        rup[i * 3 + j] = 3 * ty + i < H2 && 3 * tx + j < W2
+                             ? p.residual[(((int64_t)b * H2 + 3 * ty + i) * W2 + 3 * tx + j) * p.Cout + c] : 0.f;
+  }
+  // three output rows at a time: their residual values (same / 2x2-average addressed) are fetched as one batch ahead
+  // of their stores
+  const int64_t pix0 = ((int64_t)b * p.H + h0) * p.W + w0;          // first pixel of the tile
+#pragma unroll
+  for (int i0 = 0; i0 < 6; i0 += 3) {
+    float rs[18];
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int j = 0; j < 6; ++j) {
+        rs[i * 6 + j] = 0.f;
+        if (h0 + i0 + i >= p.H || w0 + j >= p.W) continue;
+        if constexpr (RES == BBDM_RES_SAME) {
+          rs[i * 6 + j] = p.residual[(pix0 + (int64_t)(i0 + i) * p.W + j) * p.Cout + c];
+        } else if constexpr (RES == BBDM_RES_DOWN2) {
+          const int64_t W2 = (int64_t)p.W * 2;
+          const float* rp = p.residual + (((int64_t)b * p.H * 2 + (h0 + i0 + i) * 2) * W2 + (w0 + j) * 2) * p.Cout + c;
+          rs[i * 6 + j] = 0.25f * (((rp[0] + rp[p.Cout]) + rp[W2 * p.Cout]) + rp[(W2 + 1) * p.Cout]);
+        }
+      }
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int j = 0; j < 6; ++j) {
+        if (h0 + i0 + i >= p.H || w0 + j >= p.W) continue;
+        float r = fmaf(y[(i0 + i) * 6 + j], inv, bv);
+        if constexpr (RES == BBDM_RES_SAME || RES == BBDM_RES_DOWN2) r += rs[i * 6 + j];
+        else if constexpr (RES == BBDM_RES_UP2) r += rup[((i0 + i) >> 1) * 3 + (j >> 1)];
+        p.out[(pix0 + (int64_t)(i0 + i) * p.W + j) * p.Cout + c] = r;
+        sum += r;
+        sq = fmaf(r, r, sq);
+      }
+  }
+}
+
+// One CTA per (64-channel group, tile row ty, sample b): 64 channels x 4 tile-column lanes (a warp reads 128
+// contiguous bytes of M per position).
+// The same-addressed and 2x2-averaged residual modes need more than 128 registers (ptxas: spills at 2 CTAs per SM).
+template <int RES>
+__global__ void __launch_bounds__(256, RES == BBDM_RES_SAME || RES == BBDM_RES_DOWN2 ? 1 : 2)
+wino6_output_kernel(const WinoOutParams p) {
+  __shared__ float red[4][64][2];
+  const int cg = blockIdx.x, ty = blockIdx.y, b = blockIdx.z;
+  const int cl = threadIdx.x & 63, tl = threadIdx.x >> 6;
+  const int c = cg * 64 + cl;
+  const float bv = p.bias ? p.bias[c] : 0.f;
+  const float inv = p.inv_wscale ? __ldg(p.inv_wscale) : 1.0f / WINO_WSCALE_FIXED;
+  float sum = 0.f, sq = 0.f;
+  for (int tx = tl; tx < p.tw; tx += 4) wino6_output_tile<RES>(p, b, ty, tx, c, bv, inv, sum, sq);
+  if (p.stats) {
+    // fixed-order combine of the 4 tile-column lanes => deterministic partial sums
+    red[tl][cl][0] = sum; red[tl][cl][1] = sq;
+    __syncthreads();
+    if (threadIdx.x < 64) {
+      float a = 0.f, q = 0.f;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) { a += red[k][threadIdx.x][0]; q += red[k][threadIdx.x][1]; }
+      const int64_t prow = (int64_t)b * p.th + ty;
+      *reinterpret_cast<float2*>(p.stats + (prow * p.Cout + cg * 64 + threadIdx.x) * 2) = make_float2(a, q);
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------
 // max|w| over the whole tensor: atomicMax on the bit patterns of the non-negative floats |w| (their integer order is
 // their value order), so the result does not depend on the order the blocks run in.  *wmax must be zeroed first.
@@ -485,16 +672,41 @@ __global__ void wino_wscale_store_kernel(float* inv) {
   *inv = 1.0f / wino_wscale(__float_as_uint(*inv));
 }
 
-// U[q][co][ci] = s * (G g G^T)[q] in fp64, split into fp16 planes.  One thread per (co, ci).
+// G (N x 3) applied to g0..g2 in fp64 -> u[0..N-1].  F(4,3): absolute row sums <= 1; F(6,3): <= 56/45, so
+// |s U| <= (56/45)^2 2^14 < 65504 with the same power-of-two scale.
+template <int T>
+__device__ __forceinline__ void wino_g(double g0, double g1, double g2, double* u) {
+  if constexpr (T == 4) {
+    u[0] = g0 / 4.0;
+    u[1] = -(g0 + g1 + g2) / 6.0;
+    u[2] = -(g0 - g1 + g2) / 6.0;
+    u[3] = g0 / 24.0 + g1 / 12.0 + g2 / 6.0;
+    u[4] = g0 / 24.0 - g1 / 12.0 + g2 / 6.0;
+    u[5] = g2;
+  } else {
+    u[0] = g0;
+    u[1] = -2.0 * (g0 + g1 + g2) / 9.0;
+    u[2] = -2.0 * (g0 - g1 + g2) / 9.0;
+    u[3] = g0 / 90.0 + g1 / 45.0 + 2.0 * g2 / 45.0;
+    u[4] = g0 / 90.0 - g1 / 45.0 + 2.0 * g2 / 45.0;
+    u[5] = 32.0 * g0 / 45.0 + 16.0 * g1 / 45.0 + 8.0 * g2 / 45.0;
+    u[6] = 32.0 * g0 / 45.0 - 16.0 * g1 / 45.0 + 8.0 * g2 / 45.0;
+    u[7] = g2;
+  }
+}
+
+// U[q][co][ci] = s * (G g G^T)[q] in fp64, split into fp16 planes ((T+2)^2 positions q).  One thread per (co, ci).
 // dgrad != 0: the data-gradient conv's weights instead -- kernel flipped, channels swapped: U[q][ci][co] from
 // g'[ky][kx] = w[co][ci][2-ky][2-kx] (threads run over co fastest so the stores stay coalesced).
+template <int T>
 __global__ void __launch_bounds__(256)
 wino_weight_kernel(const float* __restrict__ w, int Cout, int Cin, int dgrad, const uint32_t* __restrict__ wmax,
                    __half* __restrict__ u_hi, __half* __restrict__ u_lo) {
+  constexpr int N = T + 2;
   const int64_t n = (int64_t)Cout * Cin;
   const double s = wmax ? (double)wino_wscale(*wmax) : (double)WINO_WSCALE_FIXED;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < n; idx += (int64_t)gridDim.x * blockDim.x) {
-    double g[3][3], t[6][3];
+    double g[3][3], t[N][3];
     int64_t src = idx;
     if (dgrad) { const int64_t ci = idx / Cout, co = idx - ci * Cout; src = co * Cin + ci; }
 #pragma unroll
@@ -504,30 +716,21 @@ wino_weight_kernel(const float* __restrict__ w, int Cout, int Cin, int dgrad, co
     }
 #pragma unroll
     for (int j = 0; j < 3; ++j) {
-      const double g0 = g[0][j], g1 = g[1][j], g2 = g[2][j];
-      t[0][j] = g0 / 4.0;
-      t[1][j] = -(g0 + g1 + g2) / 6.0;
-      t[2][j] = -(g0 - g1 + g2) / 6.0;
-      t[3][j] = g0 / 24.0 + g1 / 12.0 + g2 / 6.0;
-      t[4][j] = g0 / 24.0 - g1 / 12.0 + g2 / 6.0;
-      t[5][j] = g2;
+      double u[N];
+      wino_g<T>(g[0][j], g[1][j], g[2][j], u);
+#pragma unroll
+      for (int i = 0; i < N; ++i) t[i][j] = u[i];
     }
 #pragma unroll
-    for (int i = 0; i < 6; ++i) {
-      const double g0 = t[i][0], g1 = t[i][1], g2 = t[i][2];
-      double u[6];
-      u[0] = g0 / 4.0;
-      u[1] = -(g0 + g1 + g2) / 6.0;
-      u[2] = -(g0 - g1 + g2) / 6.0;
-      u[3] = g0 / 24.0 + g1 / 12.0 + g2 / 6.0;
-      u[4] = g0 / 24.0 - g1 / 12.0 + g2 / 6.0;
-      u[5] = g2;
+    for (int i = 0; i < N; ++i) {
+      double u[N];
+      wino_g<T>(t[i][0], t[i][1], t[i][2], u);
 #pragma unroll
-      for (int j = 0; j < 6; ++j) {
+      for (int j = 0; j < N; ++j) {
         const float v = (float)(u[j] * s);
         const __half h = __float2half_rn(v);
         const __half l = __float2half_rn(v - __half2float(h));
-        const int64_t off = (int64_t)(i * 6 + j) * n + idx;
+        const int64_t off = (int64_t)(i * N + j) * n + idx;
         u_hi[off] = h;
         u_lo[off] = l;
       }
@@ -539,21 +742,29 @@ wino_weight_kernel(const float* __restrict__ w, int Cout, int Cin, int dgrad, co
 
 using namespace bbdm;
 
-extern "C" {
+namespace {
 
-int bbdm_wino_geometry(int B, int H, int W, int* tiles_h, int* tiles_w, int64_t* tiles_total, int* eligible) {
+// Tile grid of a T x T output tiling.  F(4,3): H, W multiples of 4, tiles_total = B*th*tw.  F(6,3): ceil(H/6) x
+// ceil(W/6) tiles (edge tiles past H or W read zero padding and store nothing there), tiles_total padded with zero V
+// rows to the GEMM's multiple of 16 and to at least one 128-row M block, so that eligibility never depends on the
+// batch size (a 64x64 image has 121 tiles).  The GEMM views the tile axis as rows of 16 with 128-tile M blocks inside
+// one transform position.
+template <int T>
+int wino_geometry_t(int B, int H, int W, int* tiles_h, int* tiles_w, int64_t* tiles_total, int* eligible) {
   BBDM_REQUIRE(B > 0 && H > 0 && W > 0, "wino_geometry: bad shape");
-  const int th = H / 4, tw = W / 4;
-  const int64_t mtot = (int64_t)B * th * tw;
+  const int th = T == 4 ? H / 4 : (H + 5) / 6, tw = T == 4 ? W / 4 : (W + 5) / 6;
+  int64_t mtot = (int64_t)B * th * tw;
+  if (T == 6) mtot = mtot < 128 ? 128 : (mtot + 15) / 16 * 16;
   if (tiles_h) *tiles_h = th;
   if (tiles_w) *tiles_w = tw;
   if (tiles_total) *tiles_total = mtot;
-  // the GEMM views the tile axis as rows of 16 with 128-tile M blocks inside one transform position
-  if (eligible) *eligible = (H % 4 == 0 && W % 4 == 0 && mtot % 16 == 0 && mtot >= 128) ? 1 : 0;
+  const bool aligned = T == 6 || (H % 4 == 0 && W % 4 == 0);
+  if (eligible) *eligible = (aligned && mtot % 16 == 0 && mtot >= 128) ? 1 : 0;
   return BBDM_OK;
 }
 
-int bbdm_wino_input(const BbdmWinoInputArgs* a, void* stream) {
+template <int T>
+int wino_input_t(const BbdmWinoInputArgs* a, void* stream) {
   BBDM_REQUIRE(a && a->src1 && a->v_hi && a->v_lo, "wino_input: null args");
   WinoInParams p;
   p.src1 = a->src1; p.c1 = a->c1;
@@ -561,7 +772,10 @@ int bbdm_wino_input(const BbdmWinoInputArgs* a, void* stream) {
   p.B = a->B; p.H = a->H; p.W = a->W;
   p.C = p.c1 + p.c2;
   p.groups = a->groups;
-  BBDM_REQUIRE(p.B > 0 && p.H > 0 && p.W > 0 && p.H % 4 == 0 && p.W % 4 == 0, "wino_input: H, W must be multiples of 4");
+  if (T == 4)
+    BBDM_REQUIRE(p.B > 0 && p.H > 0 && p.W > 0 && p.H % 4 == 0 && p.W % 4 == 0, "wino_input: H, W must be multiples of 4");
+  else
+    BBDM_REQUIRE(p.B > 0 && p.H > 0 && p.W > 0, "wino6_input: bad shape");
   BBDM_REQUIRE(p.c1 % 2 == 0 && p.c2 % 2 == 0 && p.C > 0, "wino_input: channel counts must be even");
   if (a->mean) {
     BBDM_REQUIRE(a->rstd && a->gamma && a->beta && p.groups > 0 && p.C % p.groups == 0, "wino_input: incomplete GroupNorm args");
@@ -573,29 +787,38 @@ int bbdm_wino_input(const BbdmWinoInputArgs* a, void* stream) {
   BBDM_REQUIRE((a->film_scale == nullptr) == (a->film_shift == nullptr), "wino_input: film scale/shift mismatch");
   BBDM_REQUIRE((a->raw_hi == nullptr) == (a->raw_lo == nullptr), "wino_input: raw hi/lo must come in pairs");
   p.cpg = p.C / p.groups;
-  p.th = p.H / 4; p.tw = p.W / 4;
-  p.Mtot = (int64_t)p.B * p.th * p.tw;
+  wino_geometry_t<T>(p.B, p.H, p.W, &p.th, &p.tw, &p.Mtot, nullptr);
   p.mean = a->mean; p.rstd = a->rstd; p.gamma = a->gamma; p.beta = a->beta;
   p.fscale = a->film_scale; p.fshift = a->film_shift; p.fstride = a->film_stride;
   p.silu = a->silu;
   p.v_hi = (__half*)a->v_hi; p.v_lo = (__half*)a->v_lo;
   p.raw_hi = (__nv_bfloat16*)a->raw_hi; p.raw_lo = (__nv_bfloat16*)a->raw_lo;
   p.act_hi = (__nv_bfloat16*)a->act_hi; p.act_lo = (__nv_bfloat16*)a->act_lo;
+  p.fault = nullptr;
+  if (T == 6) {
+    p.fault = device_fault_ptr();
+    BBDM_REQUIRE(p.fault != nullptr, "wino6_input: device fault word unavailable");
+  }
   const bool smem_only = a->mean == nullptr || a->act_hi != nullptr;      // features only the staged kernel has
   const int64_t ctas = (int64_t)p.B * p.th;
   BBDM_REQUIRE(ctas < (1ll << 31), "wino_input: too many tile rows");
+  constexpr int CC = WinoIn<T>::CC;
   // default: the shared-memory staged kernel (needs 64-channel chunks inside one source tensor);
-  // BBDM_WINO_IN_VEC=1|2 selects the register-only variant with 1 or 2 channels per thread (fallback / A-B switch)
+  // BBDM_WINO_IN_VEC=1|2 selects the register-only F(4,3) variant with 1 or 2 channels per thread (fallback / A-B
+  // switch).  F(6,3) has the staged kernel only.
   static int vec = -1;
   if (vec < 0) { const char* e = getenv("BBDM_WINO_IN_VEC"); vec = e ? (atoi(e) == 2 ? 2 : 1) : 0; }
-  if (vec == 0 && p.c1 % WI_CC == 0 && p.c2 % WI_CC == 0) {
+  if ((T == 6 || vec == 0) && p.c1 % CC == 0 && p.c2 % CC == 0) {
     static DeviceOnce configured;
     if (configured.need()) {
-      BBDM_CUDA_CHECK(cudaFuncSetAttribute(wino_input_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WI_SMEM));
+      BBDM_CUDA_CHECK(cudaFuncSetAttribute(wino_input_smem_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)WinoIn<T>::SMEM));
       configured.mark();
     }
-    dim3 grid((unsigned)ctas, p.C / WI_CC);
-    wino_input_smem_kernel<<<grid, 256, WI_SMEM, (cudaStream_t)stream>>>(p);
+    dim3 grid((unsigned)ctas, p.C / CC);
+    wino_input_smem_kernel<T><<<grid, 256, WinoIn<T>::SMEM, (cudaStream_t)stream>>>(p);
+  } else if (T == 6) {
+    BBDM_REQUIRE(false, "wino6_input: channel counts must be multiples of 64");
   } else if (smem_only) {
     BBDM_REQUIRE(false, "wino_input: identity mode / act planes need channel counts that are multiples of 64");
   } else if (vec == 2 || (vec == 0 && p.c1 % 2 == 0 && p.c2 % 2 == 0)) {
@@ -609,35 +832,48 @@ int bbdm_wino_input(const BbdmWinoInputArgs* a, void* stream) {
   return BBDM_OK;
 }
 
-int bbdm_wino_output(const BbdmWinoOutputArgs* a, void* stream) {
+template <int T>
+int wino_output_t(const BbdmWinoOutputArgs* a, void* stream) {
   BBDM_REQUIRE(a && a->m && a->out, "wino_output: null args");
   WinoOutParams p;
   p.m = a->m; p.inv_wscale = a->inv_wscale;
   p.B = a->B; p.H = a->H; p.W = a->W; p.Cout = a->Cout;
-  BBDM_REQUIRE(p.B > 0 && p.B <= 65535 && p.H > 0 && p.W > 0 && p.H % 4 == 0 && p.W % 4 == 0,
-               "wino_output: H, W must be multiples of 4 (B <= 65535)");
+  if (T == 4)
+    BBDM_REQUIRE(p.B > 0 && p.B <= 65535 && p.H > 0 && p.W > 0 && p.H % 4 == 0 && p.W % 4 == 0,
+                 "wino_output: H, W must be multiples of 4 (B <= 65535)");
+  else
+    BBDM_REQUIRE(p.B > 0 && p.B <= 65535 && p.H > 0 && p.W > 0, "wino6_output: bad shape (B <= 65535)");
   BBDM_REQUIRE(p.Cout > 0 && p.Cout % 64 == 0, "wino_output: Cout %% 64 != 0");
   BBDM_REQUIRE(a->res_mode >= 0 && a->res_mode <= 3 && (a->res_mode == 0 || a->residual), "wino_output: bad residual");
   if (a->res_mode == BBDM_RES_UP2) BBDM_REQUIRE(p.H % 2 == 0 && p.W % 2 == 0, "wino_output: RES_UP2 needs even H, W");
-  p.th = p.H / 4; p.tw = p.W / 4;
+  wino_geometry_t<T>(p.B, p.H, p.W, &p.th, &p.tw, &p.Mtot, nullptr);
   BBDM_REQUIRE(p.th <= 65535, "wino_output: too many tile rows");
-  p.Mtot = (int64_t)p.B * p.th * p.tw;
   p.bias = a->bias; p.residual = a->residual; p.res_mode = a->res_mode;
   p.out = a->out; p.stats = a->stats_partial;
   dim3 grid(p.Cout / 64, p.th, p.B);
   cudaStream_t st = (cudaStream_t)stream;
-  switch (p.res_mode) {
-    case BBDM_RES_SAME: wino_output_kernel<BBDM_RES_SAME><<<grid, 256, 0, st>>>(p); break;
-    case BBDM_RES_UP2: wino_output_kernel<BBDM_RES_UP2><<<grid, 256, 0, st>>>(p); break;
-    case BBDM_RES_DOWN2: wino_output_kernel<BBDM_RES_DOWN2><<<grid, 256, 0, st>>>(p); break;
-    default: wino_output_kernel<BBDM_RES_NONE><<<grid, 256, 0, st>>>(p); break;
+  if constexpr (T == 4) {
+    switch (p.res_mode) {
+      case BBDM_RES_SAME: wino_output_kernel<BBDM_RES_SAME><<<grid, 256, 0, st>>>(p); break;
+      case BBDM_RES_UP2: wino_output_kernel<BBDM_RES_UP2><<<grid, 256, 0, st>>>(p); break;
+      case BBDM_RES_DOWN2: wino_output_kernel<BBDM_RES_DOWN2><<<grid, 256, 0, st>>>(p); break;
+      default: wino_output_kernel<BBDM_RES_NONE><<<grid, 256, 0, st>>>(p); break;
+    }
+  } else {
+    switch (p.res_mode) {
+      case BBDM_RES_SAME: wino6_output_kernel<BBDM_RES_SAME><<<grid, 256, 0, st>>>(p); break;
+      case BBDM_RES_UP2: wino6_output_kernel<BBDM_RES_UP2><<<grid, 256, 0, st>>>(p); break;
+      case BBDM_RES_DOWN2: wino6_output_kernel<BBDM_RES_DOWN2><<<grid, 256, 0, st>>>(p); break;
+      default: wino6_output_kernel<BBDM_RES_NONE><<<grid, 256, 0, st>>>(p); break;
+    }
   }
   BBDM_LAUNCH_CHECK();
   return BBDM_OK;
 }
 
-int bbdm_wino_pack_weight(const float* w, int Cout, int Cin, int dgrad, void* u_hi, void* u_lo, float* inv_wscale,
-                          void* stream) {
+template <int T>
+int wino_pack_weight_t(const float* w, int Cout, int Cin, int dgrad, void* u_hi, void* u_lo, float* inv_wscale,
+                       void* stream) {
   BBDM_REQUIRE(w && u_hi && u_lo && Cout > 0 && Cin > 0, "wino_pack_weight: bad args");
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t n = (int64_t)Cout * Cin;
@@ -651,10 +887,34 @@ int bbdm_wino_pack_weight(const float* w, int Cout, int Cin, int dgrad, void* u_
   }
   int64_t g = (n + 255) / 256;
   if (g > (int64_t)num_sms() * 16) g = (int64_t)num_sms() * 16;
-  wino_weight_kernel<<<(unsigned)g, 256, 0, st>>>(w, Cout, Cin, dgrad, wmax, (__half*)u_hi, (__half*)u_lo);
+  wino_weight_kernel<T><<<(unsigned)g, 256, 0, st>>>(w, Cout, Cin, dgrad, wmax, (__half*)u_hi, (__half*)u_lo);
   if (wmax) wino_wscale_store_kernel<<<1, 1, 0, st>>>(inv_wscale);
   BBDM_LAUNCH_CHECK();
   return BBDM_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int bbdm_wino_geometry(int B, int H, int W, int* tiles_h, int* tiles_w, int64_t* tiles_total, int* eligible) {
+  return wino_geometry_t<4>(B, H, W, tiles_h, tiles_w, tiles_total, eligible);
+}
+int bbdm_wino_input(const BbdmWinoInputArgs* a, void* stream) { return wino_input_t<4>(a, stream); }
+int bbdm_wino_output(const BbdmWinoOutputArgs* a, void* stream) { return wino_output_t<4>(a, stream); }
+int bbdm_wino_pack_weight(const float* w, int Cout, int Cin, int dgrad, void* u_hi, void* u_lo, float* inv_wscale,
+                          void* stream) {
+  return wino_pack_weight_t<4>(w, Cout, Cin, dgrad, u_hi, u_lo, inv_wscale, stream);
+}
+
+int bbdm_wino6_geometry(int B, int H, int W, int* tiles_h, int* tiles_w, int64_t* tiles_total, int* eligible) {
+  return wino_geometry_t<6>(B, H, W, tiles_h, tiles_w, tiles_total, eligible);
+}
+int bbdm_wino6_input(const BbdmWinoInputArgs* a, void* stream) { return wino_input_t<6>(a, stream); }
+int bbdm_wino6_output(const BbdmWinoOutputArgs* a, void* stream) { return wino_output_t<6>(a, stream); }
+int bbdm_wino6_pack_weight(const float* w, int Cout, int Cin, int dgrad, void* u_hi, void* u_lo, float* inv_wscale,
+                           void* stream) {
+  return wino_pack_weight_t<6>(w, Cout, Cin, dgrad, u_hi, u_lo, inv_wscale, stream);
 }
 
 }  // extern "C"

@@ -208,16 +208,23 @@ class KernelExecutor:
 
 
     # ---- Winograd F(4x4,3x3) path (csrc/winograd.cu) ----------------------------------------------------------
-    def _wino_geometry(self, B, H, W):
-        key = (B, H, W)
+    def _wino_geometry(self, B, H, W, tile=4):
+        key = (B, H, W, tile)
         g = self._wino_geom.get(key)
         if g is None:
-            g = self._wino_geom[key] = self.be.wino_geometry(B, H, W)
+            g = self._wino_geom[key] = self.be.wino_geometry(B, H, W, **({} if tile == 4 else dict(tile=tile)))
         return g
 
-    def _wino_ok(self, ent, B, H, W):
-        return self.wino and "u_hi" in ent and convs.winograd_ok(self._wino_geometry(B, H, W), ent["cin"], ent["cout"],
-                                                                 self.wino_min_c, self.wino_min_tiles)
+    def _wino_ok(self, ent, B, H, W, c1=None):
+        """c1: channels of the first tensor of a concatenated input -- the F(6,3) input transform takes 64-channel
+        chunks inside each tensor (cin % 64 == 0 alone does not give that)."""
+        if not (self.wino and "u_hi" in ent):
+            return False
+        tile = ent["u_tile"]
+        if tile == 6 and c1 is not None and c1 % 64:
+            return False
+        return convs.winograd_ok(self._wino_geometry(B, H, W, tile), ent["cin"], ent["cout"], self.wino_min_c,
+                                 self.wino_min_tiles, tile)
 
     def _wino_ready(self, ent):
         """Whether refresh_weights gives the packed conv ent Winograd planes."""
@@ -228,9 +235,10 @@ class KernelExecutor:
         """GroupNorm-affine(+FiLM)+SiLU -> 3x3 conv (+bias, +residual, GN partial sums) of cat(src1, src2) on the
         Winograd path with the entry's planes; transform: the wino_input arguments (groups, mean, rstd, ...)."""
         B, H, W, _ = src1.shape
-        return convs.wino_conv(self.be, pool, self._wino_geometry(B, H, W), src1, src2, cout=ent["cout"],
+        tile = ent["u_tile"]
+        return convs.wino_conv(self.be, pool, self._wino_geometry(B, H, W, tile), src1, src2, cout=ent["cout"],
                                planes=(ent["u_hi"], ent["u_lo"], ent.get("u_inv")), bias=ent["bias"],
-                               residual=residual, res_mode=res_mode, stats=True, **transform)
+                               residual=residual, res_mode=res_mode, stats=True, tile=tile, **transform)
 
 
 class UNetEngine(KernelExecutor):
@@ -302,13 +310,18 @@ class UNetEngine(KernelExecutor):
                     packer.conv(pre + ".attn2.to_out.0", a2.to_out[0].weight, a2.to_out[0].bias)
                     packer.conv(pre + ".ff.net.0.proj", blk.ff.net[0].proj.weight, blk.ff.net[0].proj.bias)
                     packer.conv(pre + ".ff.net.2", blk.ff.net[2].weight, blk.ff.net[2].bias)
+        sizes = self._resblock_sizes()
         for name, m in u.named_modules():
-            # Winograd planes for the stride-1 3x3 convs of the scale-shift ResBlocks
+            # Winograd planes for the stride-1 3x3 convs of the scale-shift ResBlocks: F(6x6,3x3) for the convs that
+            # run on a large map at the UNet's image_size (convs.wino_tile), else F(4x4,3x3); a forward at another
+            # size runs the form that is packed
             if isinstance(m, ResBlock) and m.use_scale_shift_norm:
+                hw = sizes[name]
+                tile = convs.wino_tile(hw, hw) if 6 in getattr(be, "wino_tiles", (4,)) else 4
                 for cname, conv, resampled in ((name + ".in_layers.2", m.in_layers[2], m.up or m.down),
                                                (name + ".out_layers.3", m.out_layers[3], False)):
                     if not resampled and self._wino_ready(w[cname]):
-                        packer.winograd(cname, conv.weight)
+                        packer.winograd(cname, conv.weight, tile)
         for name, m in u.named_modules():
             if isinstance(m, ResBlock) and m.up and m.channels % 64 == 0 and m.out_channels % 64 == 0:
                 # up-ResBlock in_layers conv: 16 phase taps of the fused nearest-2x + 3x3 conv
@@ -323,6 +336,21 @@ class UNetEngine(KernelExecutor):
         w["film_n"] = off
         self._w = w
         self._wkey = key
+
+    def _resblock_sizes(self):
+        """{ResBlock name: side of the map its convs write} at the UNet's nominal image_size (the input side)."""
+        u, side, out = self.unet, int(self.unet.image_size), {}
+        for prefix, blocks in (("input_blocks", u.input_blocks), ("middle_block", [u.middle_block]),
+                               ("output_blocks", u.output_blocks)):
+            for i, block in enumerate(blocks):
+                for j, layer in enumerate(block):
+                    if isinstance(layer, Downsample) or (isinstance(layer, ResBlock) and layer.down):
+                        side //= 2
+                    elif isinstance(layer, Upsample) or (isinstance(layer, ResBlock) and layer.up):
+                        side *= 2
+                    if isinstance(layer, ResBlock):
+                        out[f"{prefix}.{j}" if prefix == "middle_block" else f"{prefix}.{i}.{j}"] = side
+        return out
 
     def _embedding_table(self, dev):
         """Rows 0..T-1 of the sinusoidal embedding (host-built with the reference's own expression,
@@ -377,7 +405,7 @@ class UNetEngine(KernelExecutor):
                                   taps=4, upsample2x=True, stats=True)
             pool.put(a_hi, a_lo)
         elif umma1 and resample == cabi.RESAMPLE_NONE and not need_raw_f32 and m.use_scale_shift_norm \
-                and self._wino_ok(e1, B, H, W):
+                and self._wino_ok(e1, B, H, W, c1):
             # Winograd conv1; the raw split planes for a fused 1x1 skip come out of the same input pass
             if fuse_skip:
                 r_hi, r_lo = pool.get(shp, torch.bfloat16), pool.get(shp, torch.bfloat16)

@@ -40,7 +40,8 @@ const char* bbdm_last_error(void);
 /* Fills sm count / compute capability of the current device; 0 on success. */
 int bbdm_device_info(int* sm_count, int* cc_major, int* cc_minor);
 /* Reads (and clears) the device-side fault word written by kernels whose mbarrier waits
- * timed out; synchronises `stream`.  0 = no fault. */
+ * timed out, by a timestep index out of range (0xB...) or by a Winograd F(6x6,3x3) input transform
+ * that left the fp16 range (0xC...); synchronises `stream`.  0 = no fault. */
 int bbdm_check_device_fault(void* stream, unsigned long long* fault_word);
 
 /* ------------------------------------------------------------------------------------------
@@ -303,6 +304,25 @@ int bbdm_wino_output(const BbdmWinoOutputArgs* a, void* stream);
  * ([36][Cin][Cout], kernel flipped, channels swapped; cf. bbdm_pack_weight_split_dgrad). */
 int bbdm_wino_pack_weight(const float* w, int Cout, int Cin, int dgrad, void* u_hi, void* u_lo, float* inv_wscale,
                           void* stream);
+
+/* Winograd F(6x6, 3x3) forms of the four calls above (interpolation points 0, +-1, +-2, +-1/2): 64 transform
+ * positions per 6x6 output tile, 0.79x the position-GEMM MACs of F(4,3) per output pixel, for the large maps.
+ * The arguments are the same; what differs:
+ *   geometry     tiles_h = ceil(H/6), tiles_w = ceil(W/6) (any H, W: edge tiles read the zero padding of the
+ *                activated tensor and store nothing past H or W); tiles_total = B*tiles_h*tiles_w rounded up to a
+ *                multiple of 16 and to at least 128 -- the rows of V and M, the GEMM's H = tiles_total/16
+ *                (wino6_input writes the padding rows as zeros); eligible = 1 for every shape.
+ *   input        v_hi, v_lo [64][tiles_total][C]; c1 and c2 must be multiples of 64.  Range: B^T d B amplifies a
+ *                tile by at most 225 (F(4,3): 100), so max|act| <= 291 is finite for every input; a V value
+ *                that is not a finite fp16 number sets the device fault word to 0xC0000000 | C
+ *                (bbdm_check_device_fault reports it).
+ *   output       m [64][tiles_total][Cout]; stats_partial [B * tiles_h][Cout][2].
+ *   pack_weight  u_hi, u_lo [64][Cout][Cin] (dgrad: [64][Cin][Cout]); the same scale s (|s U| <= 1.55 * 2^14). */
+int bbdm_wino6_geometry(int B, int H, int W, int* tiles_h, int* tiles_w, int64_t* tiles_total, int* eligible);
+int bbdm_wino6_input(const BbdmWinoInputArgs* a, void* stream);
+int bbdm_wino6_output(const BbdmWinoOutputArgs* a, void* stream);
+int bbdm_wino6_pack_weight(const float* w, int Cout, int Cin, int dgrad, void* u_hi, void* u_lo, float* inv_wscale,
+                           void* stream);
 
 /* General fp32 direct convolution on CUDA cores (any Cin/Cout, k in {1,3}, stride 1 or 2,
  * pad k/2): stem (openaimodel.py:524), head (:690), conv-mode Downsample/Upsample (:109,150)
