@@ -22,6 +22,12 @@ RES_NONE, RES_SAME, RES_UP2, RES_DOWN2 = 0, 1, 2, 3
 GN_MAX_SLICES = 64
 ATTN_HEAD_DIMS = (16, 32, 64, 128)       # head sizes the attention kernels are built for
 ATTN_TC_HEAD_DIMS = (64, 128)            # ... of which bbdm_attention_tc (wgmma) takes these
+LN_MAX_C = 2048                          # bbdm_layernorm_split / _bwd: C even, <= this
+
+
+def layernorm_bwd_workspace(rows, C):
+    """floats of bbdm_layernorm_bwd's workspace: one [2, C] partial per 64 rows"""
+    return -(-rows // 64) * 2 * C
 
 # every symbol include/bbdm_b200.h declares (tests check the library exports all of them)
 SYMBOLS = [
@@ -37,6 +43,7 @@ SYMBOLS = [
     "bbdm_wino6_geometry", "bbdm_wino6_input", "bbdm_wino6_output", "bbdm_wino6_pack_weight",
     "bbdm_optim_chunk_elems", "bbdm_adam_multi", "bbdm_ema_multi", "bbdm_denorm_to_uint8",
     "bbdm_layernorm_split", "bbdm_geglu_split", "bbdm_attention_cross", "bbdm_conv_stem", "bbdm_spatial_rescale",
+    "bbdm_layernorm_bwd", "bbdm_geglu_bwd", "bbdm_attention_cross_bwd",
 ]
 
 
@@ -155,6 +162,9 @@ def load():
     lib.bbdm_layernorm_split.argtypes = [vp, i64, i, vp, vp, f, vp, vp, vp, vp]
     lib.bbdm_geglu_split.argtypes = [vp, i64, i, vp, vp, vp, vp]
     lib.bbdm_attention_cross.argtypes = [vp, vp, vp, vp, i, i, i, i, i, vp, vp, vp, vp]
+    lib.bbdm_layernorm_bwd.argtypes = [vp, vp, i64, i, vp, f, vp, vp, vp, vp, vp]
+    lib.bbdm_geglu_bwd.argtypes = [vp, vp, i64, i, vp, vp]
+    lib.bbdm_attention_cross_bwd.argtypes = [vp, vp, vp, vp, i, i, i, i, i, vp, vp, vp, vp, vp]
     lib.bbdm_optim_chunk_elems.argtypes = []
     lib.bbdm_adam_multi.argtypes = [vp, vp, vp, vp, vp, vp, i, vp, vp, f, f, f, f, f, i64, vp, C.c_double, vp]
     lib.bbdm_ema_multi.argtypes = [vp, vp, vp, vp, vp, i, vp, C.c_double, i, vp]
@@ -428,6 +438,26 @@ class CudaBackend:
                                             ptr(_req(kv_hi, torch.bfloat16)), ptr(_req(kv_lo, torch.bfloat16)), B, Tq, Tkv,
                                             Cc, heads, ptr(out_f32), ptr(out_hi), ptr(out_lo), stream()))
         LAUNCHES["n"] += 1
+
+    def layernorm_bwd(self, x, dy, gamma, eps, dx, dgamma, dbeta, workspace):
+        """workspace: layernorm_bwd_workspace(rows, C) floats."""
+        Cc = x.shape[-1]
+        check(self.lib.bbdm_layernorm_bwd(ptr(_req(x)), ptr(_req(dy)), x.numel() // Cc, Cc, ptr(_req(gamma)), eps,
+                                          ptr(_req(dx)), ptr(_req(dgamma)), ptr(_req(dbeta)), ptr(_req(workspace)),
+                                          stream()))
+        LAUNCHES["n"] += 2
+
+    def geglu_bwd(self, u, dy, du):
+        N2 = u.shape[-1]
+        check(self.lib.bbdm_geglu_bwd(ptr(_req(u)), ptr(_req(dy)), u.numel() // N2, N2 // 2, ptr(_req(du)), stream()))
+        LAUNCHES["n"] += 1
+
+    def attention_cross_bwd(self, q, kv, out, dout, heads, dq, dkv, lse, delta):
+        B, Tq, Cc = q.shape
+        check(self.lib.bbdm_attention_cross_bwd(ptr(_req(q)), ptr(_req(kv)), ptr(_req(out)), ptr(_req(dout)), B, Tq,
+                                                kv.shape[1], Cc, heads, ptr(_req(dq)), ptr(_req(dkv)), ptr(_req(lse)),
+                                                ptr(_req(delta)), stream()))
+        LAUNCHES["n"] += 2
 
     # -- sample_to_eval output path ------------------------------------------------------------------------
     def denorm_to_uint8(self, images, to_normal, out):

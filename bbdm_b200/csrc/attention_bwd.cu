@@ -21,16 +21,22 @@ namespace bbdm {
 constexpr int AB_T = 64;           // tile edge (queries and keys)
 constexpr int AB_LD = AB_T + 4;    // row stride of the P / dS tiles (float4-aligned, conflict-free)
 
+// Queries come from q [B, Tq, ldq], keys and values from kv [B, Tkv, ldkv] (the same tensor for self-attention);
+// head h reads columns q_base + h*q_hstride (q), k_base / v_base + h*kv_hstride (k, v) and its gradients go to the
+// same columns of dq / dkv, whose row strides equal ldq / ldkv.
 struct AttnBwdParams {
-  const float* qkv; const float* o; const float* dout; float* dqkv;
-  float* lse; float* delta;        // [B*heads, T]
-  int T, C, heads, order;
+  const float* q; const float* kv; const float* o; const float* dout; float* dq; float* dkv;
+  float* lse; float* delta;        // [B*heads, Tq]
+  int Tq, Tkv, C, heads;
+  int64_t ldq, ldkv;
+  int q_base, k_base, v_base, q_hstride, kv_hstride;
   float scale2, scale_log2;
 };
 
-__device__ __forceinline__ void head_offsets(const AttnBwdParams& p, int head, int D, int& qoff, int& koff, int& voff) {
-  if (p.order == 0) { qoff = head * 3 * D; koff = qoff + D; voff = qoff + 2 * D; }
-  else { qoff = head * D; koff = p.C + head * D; voff = 2 * p.C + head * D; }
+__device__ __forceinline__ void head_offsets(const AttnBwdParams& p, int head, int& qoff, int& koff, int& voff) {
+  qoff = p.q_base + head * p.q_hstride;
+  koff = p.k_base + head * p.kv_hstride;
+  voff = p.v_base + head * p.kv_hstride;
 }
 
 // 64 rows x D columns of a [*, ld] fp32 matrix -> transposed tile dst_t[D][64] (and row-major dst_r[64][D])
@@ -98,21 +104,21 @@ attn_bwd_dq_kernel(const AttnBwdParams p) {
   const int bh = blockIdx.y, b = bh / p.heads, head = bh % p.heads;
   const int q0 = blockIdx.x * AB_T;
   int qoff, koff, voff;
-  head_offsets(p, head, D, qoff, koff, voff);
-  const int64_t ld3 = 3 * (int64_t)p.C;
-  const float* qkv_b = p.qkv + (int64_t)b * p.T * ld3;
-  const float* do_b = p.dout + (int64_t)b * p.T * p.C + head * D;
-  const float* o_b = p.o + (int64_t)b * p.T * p.C + head * D;
-  const int n_tiles = (p.T + AB_T - 1) / AB_T;
+  head_offsets(p, head, qoff, koff, voff);
+  const float* q_b = p.q + (int64_t)b * p.Tq * p.ldq;
+  const float* kv_b = p.kv + (int64_t)b * p.Tkv * p.ldkv;
+  const float* do_b = p.dout + (int64_t)b * p.Tq * p.C + head * D;
+  const float* o_b = p.o + (int64_t)b * p.Tq * p.C + head * D;
+  const int n_tiles = (p.Tkv + AB_T - 1) / AB_T;
 
-  load_tile<D>(qkv_b + qoff, ld3, q0, p.T, Qt, nullptr);
-  load_tile<D>(do_b, p.C, q0, p.T, dOt, nullptr);
+  load_tile<D>(q_b + qoff, p.ldq, q0, p.Tq, Qt, nullptr);
+  load_tile<D>(do_b, p.C, q0, p.Tq, dOt, nullptr);
   __syncthreads();
   {
     // delta_i = <dO_i, O_i>: 4 threads per row
     const int row = tid >> 2, part = tid & 3;
     float s = 0.f;
-    if (q0 + row < p.T) {
+    if (q0 + row < p.Tq) {
       const float* orow = o_b + (int64_t)(q0 + row) * p.C;
       for (int d = part * (D / 4); d < (part + 1) * (D / 4); ++d) s = fmaf(dOt[d * AB_T + row], orow[d], s);
     }
@@ -120,7 +126,7 @@ attn_bwd_dq_kernel(const AttnBwdParams p) {
     s += __shfl_xor_sync(0xffffffffu, s, 2);
     if (part == 0) {
       delta_s[row] = s;
-      if (q0 + row < p.T) p.delta[(int64_t)bh * p.T + q0 + row] = s;
+      if (q0 + row < p.Tq) p.delta[(int64_t)bh * p.Tq + q0 + row] = s;
     }
   }
 
@@ -131,7 +137,7 @@ attn_bwd_dq_kernel(const AttnBwdParams p) {
   for (int j = 0; j < n_tiles; ++j) {
     const int k0 = j * AB_T;
     __syncthreads();
-    load_tile<D>(qkv_b + koff, ld3, k0, p.T, Kt, nullptr);
+    load_tile<D>(kv_b + koff, p.ldkv, k0, p.Tkv, Kt, nullptr);
     __syncthreads();
     float s[4][4];
     mm_tt<D>(Qt, Kt, ty, tx, s);
@@ -140,7 +146,7 @@ attn_bwd_dq_kernel(const AttnBwdParams p) {
       float mx = -INFINITY;
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
-        s[i][c] = (k0 + tx * 4 + c < p.T) ? s[i][c] * p.scale_log2 : -INFINITY;
+        s[i][c] = (k0 + tx * 4 + c < p.Tkv) ? s[i][c] * p.scale_log2 : -INFINITY;
         mx = fmaxf(mx, s[i][c]);
       }
       mx = group16_max(mx);
@@ -158,7 +164,7 @@ attn_bwd_dq_kernel(const AttnBwdParams p) {
   for (int i = 0; i < 4; ++i) {
     lse[i] = m[i] + log2f(l[i]);
     dl[i] = delta_s[ty * 4 + i];
-    if (tx == 0 && q0 + ty * 4 + i < p.T) p.lse[(int64_t)bh * p.T + q0 + ty * 4 + i] = lse[i];
+    if (tx == 0 && q0 + ty * 4 + i < p.Tq) p.lse[(int64_t)bh * p.Tq + q0 + ty * 4 + i] = lse[i];
   }
 
   // ---- pass 2: dQ = s^2 * sum_j dS_j K_j -------------------------------------------------------
@@ -170,8 +176,8 @@ attn_bwd_dq_kernel(const AttnBwdParams p) {
   for (int j = 0; j < n_tiles; ++j) {
     const int k0 = j * AB_T;
     __syncthreads();
-    load_tile<D>(qkv_b + koff, ld3, k0, p.T, Kt, Ks);
-    load_tile<D>(qkv_b + voff, ld3, k0, p.T, Vt, nullptr);
+    load_tile<D>(kv_b + koff, p.ldkv, k0, p.Tkv, Kt, Ks);
+    load_tile<D>(kv_b + voff, p.ldkv, k0, p.Tkv, Vt, nullptr);
     __syncthreads();
     float s[4][4], dp[4][4];
     mm_tt<D>(Qt, Kt, ty, tx, s);
@@ -181,7 +187,7 @@ attn_bwd_dq_kernel(const AttnBwdParams p) {
       float ds[4];
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
-        const float pr = (k0 + tx * 4 + c < p.T) ? exp2f(fmaf(s[i][c], p.scale_log2, -lse[i])) : 0.f;
+        const float pr = (k0 + tx * 4 + c < p.Tkv) ? exp2f(fmaf(s[i][c], p.scale_log2, -lse[i])) : 0.f;
         ds[c] = pr * (dp[i][c] - dl[i]);
       }
       *reinterpret_cast<float4*>(dSs + (ty * 4 + i) * AB_LD + tx * 4) = make_float4(ds[0], ds[1], ds[2], ds[3]);
@@ -203,8 +209,8 @@ attn_bwd_dq_kernel(const AttnBwdParams p) {
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int q = q0 + ty * 4 + i;
-    if (q >= p.T) continue;
-    float* dst = p.dqkv + ((int64_t)b * p.T + q) * ld3 + qoff + tx * DC;
+    if (q >= p.Tq) continue;
+    float* dst = p.dq + ((int64_t)b * p.Tq + q) * p.ldq + qoff + tx * DC;
 #pragma unroll
     for (int c = 0; c < DC; ++c) dst[c] = dq[i][c] * p.scale2;
   }
@@ -233,14 +239,14 @@ attn_bwd_dkv_kernel(const AttnBwdParams p) {
   const int bh = blockIdx.y, b = bh / p.heads, head = bh % p.heads;
   const int k0 = blockIdx.x * AB_T;
   int qoff, koff, voff;
-  head_offsets(p, head, D, qoff, koff, voff);
-  const int64_t ld3 = 3 * (int64_t)p.C;
-  const float* qkv_b = p.qkv + (int64_t)b * p.T * ld3;
-  const float* do_b = p.dout + (int64_t)b * p.T * p.C + head * D;
-  const int n_tiles = (p.T + AB_T - 1) / AB_T;
+  head_offsets(p, head, qoff, koff, voff);
+  const float* q_b = p.q + (int64_t)b * p.Tq * p.ldq;
+  const float* kv_b = p.kv + (int64_t)b * p.Tkv * p.ldkv;
+  const float* do_b = p.dout + (int64_t)b * p.Tq * p.C + head * D;
+  const int n_tiles = (p.Tq + AB_T - 1) / AB_T;
 
-  load_tile<D>(qkv_b + koff, ld3, k0, p.T, Kt, nullptr);
-  load_tile<D>(qkv_b + voff, ld3, k0, p.T, Vt, nullptr);
+  load_tile<D>(kv_b + koff, p.ldkv, k0, p.Tkv, Kt, nullptr);
+  load_tile<D>(kv_b + voff, p.ldkv, k0, p.Tkv, Vt, nullptr);
 
   float dk[4][DC], dv[4][DC];
 #pragma unroll
@@ -251,12 +257,12 @@ attn_bwd_dkv_kernel(const AttnBwdParams p) {
   for (int j = 0; j < n_tiles; ++j) {
     const int q0 = j * AB_T;
     __syncthreads();
-    load_tile<D>(qkv_b + qoff, ld3, q0, p.T, Qt, Qs);
-    load_tile<D>(do_b, p.C, q0, p.T, dOt, dOs);
+    load_tile<D>(q_b + qoff, p.ldq, q0, p.Tq, Qt, Qs);
+    load_tile<D>(do_b, p.C, q0, p.Tq, dOt, dOs);
     if (tid < AB_T) {
-      const bool ok = q0 + tid < p.T;
-      lse_s[tid] = ok ? p.lse[(int64_t)bh * p.T + q0 + tid] : 0.f;
-      delta_s[tid] = ok ? p.delta[(int64_t)bh * p.T + q0 + tid] : 0.f;
+      const bool ok = q0 + tid < p.Tq;
+      lse_s[tid] = ok ? p.lse[(int64_t)bh * p.Tq + q0 + tid] : 0.f;
+      delta_s[tid] = ok ? p.delta[(int64_t)bh * p.Tq + q0 + tid] : 0.f;
     }
     __syncthreads();
     float s[4][4], dp[4][4];
@@ -265,11 +271,11 @@ attn_bwd_dkv_kernel(const AttnBwdParams p) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const int r = ty * 4 + i;
-      const bool qok = q0 + r < p.T;
+      const bool qok = q0 + r < p.Tq;
       float pr[4], ds[4];
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
-        pr[c] = (qok && k0 + tx * 4 + c < p.T) ? exp2f(fmaf(s[i][c], p.scale_log2, -lse_s[r])) : 0.f;
+        pr[c] = (qok && k0 + tx * 4 + c < p.Tkv) ? exp2f(fmaf(s[i][c], p.scale_log2, -lse_s[r])) : 0.f;
         ds[c] = pr[c] * (dp[i][c] - delta_s[r]);
       }
       *reinterpret_cast<float4*>(Ps + r * AB_LD + tx * 4) = make_float4(pr[0], pr[1], pr[2], pr[3]);
@@ -297,8 +303,8 @@ attn_bwd_dkv_kernel(const AttnBwdParams p) {
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int k = k0 + ty * 4 + i;
-    if (k >= p.T) continue;
-    float* row = p.dqkv + ((int64_t)b * p.T + k) * ld3;
+    if (k >= p.Tkv) continue;
+    float* row = p.dkv + ((int64_t)b * p.Tkv + k) * p.ldkv;
 #pragma unroll
     for (int c = 0; c < DC; ++c) {
       row[koff + tx * DC + c] = dk[i][c] * p.scale2;
@@ -313,11 +319,31 @@ static int launch_bwd(const AttnBwdParams& p, int B, cudaStream_t s) {
   const size_t sm2 = (size_t)(6 * D * AB_T + 2 * AB_T * AB_LD + 2 * AB_T) * sizeof(float);
   BBDM_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dq_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1));
   BBDM_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dkv_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2));
-  const dim3 grid((p.T + AB_T - 1) / AB_T, B * p.heads);
-  attn_bwd_dq_kernel<D><<<grid, 256, sm1, s>>>(p);
+  attn_bwd_dq_kernel<D><<<dim3((p.Tq + AB_T - 1) / AB_T, B * p.heads), 256, sm1, s>>>(p);
   BBDM_LAUNCH_CHECK();
-  attn_bwd_dkv_kernel<D><<<grid, 256, sm2, s>>>(p);
+  attn_bwd_dkv_kernel<D><<<dim3((p.Tkv + AB_T - 1) / AB_T, B * p.heads), 256, sm2, s>>>(p);
   BBDM_LAUNCH_CHECK();
+  return BBDM_OK;
+}
+
+// shape checks, the D^-1/4 scales and the head_dim dispatch shared by both entry points
+static int attention_bwd_launch(const char* what, AttnBwdParams p, int B, void* stream) {
+  BBDM_REQUIRE(p.q && p.kv && p.o && p.dout && p.dq && p.dkv && p.lse && p.delta, "%s: null pointer", what);
+  BBDM_REQUIRE(B > 0 && p.Tq > 0 && p.Tkv > 0 && p.heads > 0 && p.C % p.heads == 0, "%s: bad shape", what);
+  BBDM_REQUIRE((int64_t)B * p.heads <= 65535, "%s: B*heads = %lld exceeds the grid limit", what, (long long)B * p.heads);
+  const int D = p.C / p.heads;
+  const double scale = 1.0 / sqrt(sqrt((double)D));
+  p.scale2 = (float)(scale * scale);
+  p.scale_log2 = (float)(scale * scale * 1.4426950408889634);
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (D) {
+    case 16: return launch_bwd<16>(p, B, s);
+    case 32: return launch_bwd<32>(p, B, s);
+    case 64: return launch_bwd<64>(p, B, s);
+    case 128: return launch_bwd<128>(p, B, s);     // kernel 2: 231,936 B of the 232,448 B opt-in shared memory
+    default:
+      BBDM_REQUIRE(false, "%s: head_dim %d not supported (16, 32, 64, 128)", what, D);
+  }
   return BBDM_OK;
 }
 
@@ -329,21 +355,29 @@ using namespace bbdm;
 // [B,T,C] (saved from the forward) and dout [B,T,C].  lse / delta: [B*heads*T] fp32 workspaces.
 extern "C" int bbdm_attention_bwd(const float* qkv, const float* out, const float* dout, int B, int T, int C, int heads,
                                   int order, float* dqkv, float* lse, float* delta, void* stream) {
-  BBDM_REQUIRE(qkv && out && dout && dqkv && lse && delta, "attention_bwd: null pointer");
-  BBDM_REQUIRE(B > 0 && T > 0 && heads > 0 && C % heads == 0 && (order == 0 || order == 1), "attention_bwd: bad shape");
-  BBDM_REQUIRE((int64_t)B * heads <= 65535, "attention_bwd: B*heads = %lld exceeds the grid limit", (long long)B * heads);
+  BBDM_REQUIRE(order == 0 || order == 1, "attention_bwd: bad shape");
+  BBDM_REQUIRE(heads > 0 && C % heads == 0, "attention_bwd: bad shape");
   const int D = C / heads;
-  const double scale = 1.0 / sqrt(sqrt((double)D));
-  AttnBwdParams p{qkv, out, dout, dqkv, lse, delta, T, C, heads, order, (float)(scale * scale),
-                  (float)(scale * scale * 1.4426950408889634)};
-  cudaStream_t s = (cudaStream_t)stream;
-  switch (D) {
-    case 16: return launch_bwd<16>(p, B, s);
-    case 32: return launch_bwd<32>(p, B, s);
-    case 64: return launch_bwd<64>(p, B, s);
-    case 128: return launch_bwd<128>(p, B, s);     // kernel 2: 231,936 B of the 232,448 B opt-in shared memory
-    default:
-      BBDM_REQUIRE(false, "attention_bwd: head_dim %d not supported (16, 32, 64, 128)", D);
-  }
-  return BBDM_OK;
+  AttnBwdParams p{};
+  p.q = p.kv = qkv; p.dq = p.dkv = dqkv;
+  p.o = out; p.dout = dout; p.lse = lse; p.delta = delta;
+  p.Tq = p.Tkv = T; p.C = C; p.heads = heads;
+  p.ldq = p.ldkv = 3 * (int64_t)C;
+  if (order == 0) { p.q_base = 0; p.k_base = D; p.v_base = 2 * D; p.q_hstride = p.kv_hstride = 3 * D; }
+  else { p.q_base = 0; p.k_base = C; p.v_base = 2 * C; p.q_hstride = p.kv_hstride = D; }
+  return attention_bwd_launch("attention_bwd", p, B, stream);
+}
+
+// Backward of bbdm_attention_cross: q [B,Tq,C], kv [B,Tkv,2C] (k = columns [0,C), v = [C,2C)) fp32, out [B,Tq,C] saved
+// from the forward, dout [B,Tq,C] -> dq [B,Tq,C], dkv [B,Tkv,2C].  lse / delta: [B*heads*Tq] fp32 workspaces.
+extern "C" int bbdm_attention_cross_bwd(const float* q, const float* kv, const float* out, const float* dout, int B,
+                                        int Tq, int Tkv, int C, int heads, float* dq, float* dkv, float* lse,
+                                        float* delta, void* stream) {
+  BBDM_REQUIRE(heads > 0 && C % heads == 0, "attention_cross_bwd: bad shape");
+  AttnBwdParams p{};
+  p.q = q; p.kv = kv; p.o = out; p.dout = dout; p.dq = dq; p.dkv = dkv; p.lse = lse; p.delta = delta;
+  p.Tq = Tq; p.Tkv = Tkv; p.C = C; p.heads = heads;
+  p.ldq = C; p.ldkv = 2 * (int64_t)C;
+  p.q_base = 0; p.k_base = 0; p.v_base = C; p.q_hstride = p.kv_hstride = C / heads;
+  return attention_bwd_launch("attention_cross_bwd", p, B, stream);
 }

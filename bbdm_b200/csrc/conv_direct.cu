@@ -212,8 +212,8 @@ extern "C" int bbdm_conv_direct_pad(const float* src, const float* w_packed, con
 // ---------------------------------------------------------------------------------------------
 // Weight gradient for the small-channel convolutions (UNet stem Cin = 3..32, head Cout = 3..16):
 //   dW[tap][co][ci] = sum_p dY[p][co] * X[p + tap][ci]          fp32 FMA, stride 1, pad k/2
-// One CTA per chunk of pixels; thread t owns the (co, ci) pairs t, t+256, ... for all taps
-// (<= 4 pairs x 9 taps accumulators); partials [chunk][tap][Cout][Cin] are reduced in a fixed order
+// One CTA per chunk of pixels and chunk of 1024 (co, ci) pairs (grid y); thread t owns the pairs t, t+256, ... of its
+// chunk for all taps (<= 4 pairs x 9 taps accumulators); partials [chunk][tap][Cout][Cin] are reduced in a fixed order
 // by bbdm's wgrad reduce kernel (deterministic).  The work is tiny (<= 2 GFLOP) -- this kernel only
 // has to not be slow; cuDNN's fp32 wgrad took 1.3 ms per call on these shapes.
 // ---------------------------------------------------------------------------------------------
@@ -239,7 +239,7 @@ conv_wgrad_direct_kernel(const float* __restrict__ dy, const float* __restrict__
   int co_[WD_MAX_PAIRS], ci_[WD_MAX_PAIRS];
 #pragma unroll
   for (int i = 0; i < WD_MAX_PAIRS; ++i) {
-    const int pr = threadIdx.x + i * 256;
+    const int pr = blockIdx.y * 256 * WD_MAX_PAIRS + threadIdx.x + i * 256;
     co_[i] = pr < pairs ? pr / Cin : -1;
     ci_[i] = pr < pairs ? pr % Cin : 0;
   }
@@ -274,7 +274,7 @@ conv_wgrad_direct_kernel(const float* __restrict__ dy, const float* __restrict__
   float* o = part + (int64_t)blockIdx.x * taps * pairs;
 #pragma unroll
   for (int i = 0; i < WD_MAX_PAIRS; ++i) {
-    const int pr = threadIdx.x + i * 256;
+    const int pr = blockIdx.y * 256 * WD_MAX_PAIRS + threadIdx.x + i * 256;
     if (pr >= pairs) continue;
 #pragma unroll
     for (int t = 0; t < 9; ++t)
@@ -307,8 +307,8 @@ extern "C" int bbdm_conv_wgrad_direct(const float* dy, const float* x, int B, in
                                       float* dw, float* workspace, int64_t workspace_floats, void* stream) {
   BBDM_REQUIRE(dy && x && dw && workspace, "conv_wgrad_direct: null pointer");
   BBDM_REQUIRE(B > 0 && H > 0 && W > 0 && (k == 1 || k == 3), "conv_wgrad_direct: bad shape");
-  BBDM_REQUIRE((int64_t)Cin * Cout <= 256 * bbdm::WD_MAX_PAIRS, "conv_wgrad_direct: Cin*Cout = %d too large (max %d)",
-               Cin * Cout, 256 * bbdm::WD_MAX_PAIRS);
+  BBDM_REQUIRE((int64_t)Cin * Cout <= (1 << 24), "conv_wgrad_direct: Cin*Cout = %lld too large",
+               (long long)Cin * Cout);
   const int64_t P = (int64_t)B * H * W;
   const int64_t n = (int64_t)k * k * Cin * Cout;
   int64_t nblk = workspace_floats / n;
@@ -318,8 +318,9 @@ extern "C" int bbdm_conv_wgrad_direct(const float* dy, const float* x, int B, in
   const int ppb = (int)((P + nblk - 1) / nblk);
   nblk = (P + ppb - 1) / ppb;
   cudaStream_t s = (cudaStream_t)stream;
-  if (k == 3) bbdm::conv_wgrad_direct_kernel<3><<<(unsigned)nblk, 256, 0, s>>>(dy, x, workspace, B, H, W, Cin, Cout, ppb);
-  else bbdm::conv_wgrad_direct_kernel<1><<<(unsigned)nblk, 256, 0, s>>>(dy, x, workspace, B, H, W, Cin, Cout, ppb);
+  const dim3 grid((unsigned)nblk, (unsigned)((Cin * Cout + 256 * bbdm::WD_MAX_PAIRS - 1) / (256 * bbdm::WD_MAX_PAIRS)));
+  if (k == 3) bbdm::conv_wgrad_direct_kernel<3><<<grid, 256, 0, s>>>(dy, x, workspace, B, H, W, Cin, Cout, ppb);
+  else bbdm::conv_wgrad_direct_kernel<1><<<grid, 256, 0, s>>>(dy, x, workspace, B, H, W, Cin, Cout, ppb);
   BBDM_LAUNCH_CHECK();
   bbdm::wgrad_direct_reduce_kernel<<<(unsigned)((n + 7) / 8), 256, 0, s>>>(workspace, (int)nblk, k * k, Cout, Cin, dw);
   BBDM_LAUNCH_CHECK();

@@ -195,9 +195,10 @@ class GNActConv2dFn(torch.autograd.Function):
     stats + prep + wgmma conv; the backward adds the two-pass GroupNorm/SiLU/FiLM gradient kernels."""
 
     @staticmethod
-    def forward(ctx, x, gamma, beta, scale, shift, weight, bias, resample=0, residual=None, act=True):
+    def forward(ctx, x, gamma, beta, scale, shift, weight, bias, resample=0, residual=None, act=True, eps=1e-5):
         """resample: 0 none, 1 nearest-2x up, 2 2x2 average pool -- applied between SiLU and the conv
-        (ResBlock(up/down), openaimodel.py:259-264)."""
+        (ResBlock(up/down), openaimodel.py:259-264).  eps: the GroupNorm's (1e-5 in GroupNorm32, 1e-6 in
+        SpatialTransformer.norm)."""
         be = backend()
         B, Cin, Hs, Ws = x.shape
         H, W = (Hs * 2, Ws * 2) if resample == 1 else ((Hs // 2, Ws // 2) if resample == 2 else (Hs, Ws))
@@ -207,7 +208,7 @@ class GNActConv2dFn(torch.autograd.Function):
         mean = torch.empty((B, 32), dtype=torch.float32, device=dev)
         rstd = torch.empty_like(mean)
         ws = torch.empty((B * 32 * cabi.GN_MAX_SLICES * 2,), dtype=torch.float64, device=dev)
-        be.gn_stats(xn, None, 32, 1e-5, mean, rstd, ws)
+        be.gn_stats(xn, None, 32, eps, mean, rstd, ws)
         fs = fh = None
         if scale is not None:
             fs, fh = scale.detach().contiguous().float(), shift.detach().contiguous().float()
@@ -271,7 +272,8 @@ class GNActConv2dFn(torch.autograd.Function):
         s2 = (gf * a2).view(B, 32, Cin // 32).sum(2).contiguous()
         dxn = torch.empty((B, H, W, Cin), dtype=torch.float32, device=dev)
         be.gn_bwd_apply(xn, da, 32, mean, rstd, g, b_, fs, fh, fstride, ctx.act, s1, s2, dxn)
-        return dxn.permute(0, 3, 1, 2), dgamma, dbeta, dscale, dshift, dw, dbias, None, (dy if ctx.has_res else None), None
+        return (dxn.permute(0, 3, 1, 2), dgamma, dbeta, dscale, dshift, dw, dbias, None, (dy if ctx.has_res else None),
+                None, None)
 
 
 def gn_act_conv2d(norm, conv, x, scale=None, shift=None, enabled=True, resample=0, residual=None, act=True):
@@ -284,7 +286,8 @@ def gn_act_conv2d(norm, conv, x, scale=None, shift=None, enabled=True, resample=
             (resample != 2 or (Hs % 2 == 0 and Ws % 2 == 0)):
         sc = None if scale is None else scale.reshape(scale.shape[0], -1)
         sh = None if shift is None else shift.reshape(shift.shape[0], -1)
-        return GNActConv2dFn.apply(x, norm.weight, norm.bias, sc, sh, conv.weight, conv.bias, resample, residual, act)
+        return GNActConv2dFn.apply(x, norm.weight, norm.bias, sc, sh, conv.weight, conv.bias, resample, residual, act,
+                                   norm.eps)
     if enabled:
         _library_path("GroupNorm+activation+conv", x)
     h = norm(x)
@@ -415,6 +418,125 @@ def attention_core(qkv4: torch.Tensor, heads: int, new_order: bool, enabled: boo
     return AttentionCoreFn.apply(qkv4, heads, 1 if new_order else 0)
 
 
+class LayerNormLinearFn(torch.autograd.Function):
+    """Linear(LayerNorm(x)) of a SpatialTransformer block (norm1/2/3 followed by to_q / q|k|v / ff.net.0.proj) over
+    the [B, C, H, W] token grid: LayerNorm writes the 1x1 conv's split operand planes directly (bbdm_layernorm_split);
+    the backward is the conv backward followed by bbdm_layernorm_bwd.  weight: [Cout, C, 1, 1]."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, weight, bias, eps):
+        be = backend()
+        B, Cin, H, W = x.shape
+        Cout = weight.shape[0]
+        dev = x.device
+        xn = _nhwc(x.detach()).contiguous()
+        a_hi = torch.empty((B, H, W, Cin), dtype=torch.bfloat16, device=dev)
+        a_lo = torch.empty_like(a_hi)
+        be.layernorm_split(xn, gamma.detach(), beta.detach(), eps, out_hi=a_hi, out_lo=a_lo)
+        w_hi, w_lo, wd_hi, wd_lo = _pack_weights(be, weight, True)
+        out = torch.empty((B, H, W, Cout), dtype=torch.float32, device=dev)
+        be.conv_umma(B=B, H=H, W=W, Cin=Cin, Cout=Cout, taps=1, a_hi=a_hi, a_lo=a_lo, w_hi=w_hi, w_lo=w_lo,
+                     bias=None if bias is None else bias.detach(), out=out, passes=3)
+        ctx.save_for_backward(xn, gamma, a_hi, a_lo, weight, wd_hi, wd_lo)
+        ctx.has_bias = bias is not None
+        ctx.shape = (B, H, W, Cin, Cout, 1)
+        ctx.eps = eps
+        return out.permute(0, 3, 1, 2)
+
+    @staticmethod
+    def backward(ctx, dy):
+        be = backend()
+        xn, gamma, a_hi, a_lo, weight, wd_hi, wd_lo = ctx.saved_tensors
+        da, dw, dbias = _conv_backward(be, ctx.shape, a_hi, a_lo, weight, dy, True, ctx.needs_input_grad[3],
+                                       ctx.has_bias and ctx.needs_input_grad[4], wd=(wd_hi, wd_lo))
+        Cin = xn.shape[3]
+        dev = dy.device
+        dxn = torch.empty_like(xn)
+        dgamma = torch.empty((Cin,), dtype=torch.float32, device=dev)
+        dbeta = torch.empty_like(dgamma)
+        ws = torch.empty((cabi.layernorm_bwd_workspace(xn.numel() // Cin, Cin),), dtype=torch.float32, device=dev)
+        be.layernorm_bwd(xn, da, gamma.detach(), ctx.eps, dxn, dgamma, dbeta, ws)
+        return dxn.permute(0, 3, 1, 2), dgamma, dbeta, dw, dbias, None
+
+
+class GEGLULinearFn(torch.autograd.Function):
+    """Linear(a * gelu(g)) for u = [a | g] (FeedForward(glu=True): GEGLU then ff.net.2) over the [B, 2N, H, W] token
+    grid: the gate writes the 1x1 conv's split operand planes directly (bbdm_geglu_split); the backward is the conv
+    backward followed by bbdm_geglu_bwd.  weight: [Cout, N, 1, 1]."""
+
+    @staticmethod
+    def forward(ctx, u, weight, bias):
+        be = backend()
+        B, N2, H, W = u.shape
+        Cout = weight.shape[0]
+        dev = u.device
+        un = _nhwc(u.detach()).contiguous()
+        g_hi = torch.empty((B, H, W, N2 // 2), dtype=torch.bfloat16, device=dev)
+        g_lo = torch.empty_like(g_hi)
+        be.geglu_split(un, out_hi=g_hi, out_lo=g_lo)
+        w_hi, w_lo, wd_hi, wd_lo = _pack_weights(be, weight, True)
+        out = torch.empty((B, H, W, Cout), dtype=torch.float32, device=dev)
+        be.conv_umma(B=B, H=H, W=W, Cin=N2 // 2, Cout=Cout, taps=1, a_hi=g_hi, a_lo=g_lo, w_hi=w_hi, w_lo=w_lo,
+                     bias=None if bias is None else bias.detach(), out=out, passes=3)
+        ctx.save_for_backward(un, g_hi, g_lo, weight, wd_hi, wd_lo)
+        ctx.has_bias = bias is not None
+        ctx.shape = (B, H, W, N2 // 2, Cout, 1)
+        return out.permute(0, 3, 1, 2)
+
+    @staticmethod
+    def backward(ctx, dy):
+        be = backend()
+        un, g_hi, g_lo, weight, wd_hi, wd_lo = ctx.saved_tensors
+        dg, dw, dbias = _conv_backward(be, ctx.shape, g_hi, g_lo, weight, dy, True, ctx.needs_input_grad[1],
+                                       ctx.has_bias and ctx.needs_input_grad[2], wd=(wd_hi, wd_lo))
+        du = torch.empty_like(un)
+        be.geglu_bwd(un, dg, du)
+        return du.permute(0, 3, 1, 2), dw, dbias
+
+
+class CrossAttentionCoreFn(torch.autograd.Function):
+    """softmax(q k^T D^-1/2) v per head (CrossAttention, attention.py:166-192) for queries q [B, C, H, W] and keys|values
+    kv [B, 2C, Hc, Wc] (k = channels [0, C), v = [C, 2C)) -> [B, C, H, W].  Forward: bbdm_attention_cross; backward:
+    bbdm_attention_cross_bwd (flash-style recompute, exact fp32): no Tq x Tkv tensor is stored, which also replaces
+    the reference's checkpoint() around the transformer block."""
+
+    @staticmethod
+    def forward(ctx, q, kv, heads):
+        be = backend()
+        B, Cc, H, W = q.shape
+        Tq, Tkv = H * W, kv.shape[2] * kv.shape[3]
+        dev = q.device
+        qn, kvn = _nhwc(q.detach()).contiguous(), _nhwc(kv.detach()).contiguous()
+        planes = []
+        for t in (qn, kvn):
+            hi = torch.empty(t.shape, dtype=torch.bfloat16, device=dev)
+            lo = torch.empty_like(hi)
+            be.prep(t, None, raw_hi=hi, raw_lo=lo)
+            planes += [hi, lo]
+        q_hi, q_lo, kv_hi, kv_lo = planes
+        out = torch.empty((B, Tq, Cc), dtype=torch.float32, device=dev)
+        be.attention_cross(q_hi.view(B, Tq, Cc), q_lo.view(B, Tq, Cc), kv_hi.view(B, Tkv, 2 * Cc),
+                           kv_lo.view(B, Tkv, 2 * Cc), heads, out_f32=out)
+        ctx.save_for_backward(qn, kvn, out)
+        ctx.heads = heads
+        return out.view(B, H, W, Cc).permute(0, 3, 1, 2)
+
+    @staticmethod
+    def backward(ctx, dout):
+        be = backend()
+        qn, kvn, out = ctx.saved_tensors
+        B, H, W, Cc = qn.shape
+        Tq, Tkv = H * W, kvn.shape[1] * kvn.shape[2]
+        dev = dout.device
+        don = _nhwc(dout).contiguous()
+        dq, dkv = torch.empty_like(qn), torch.empty_like(kvn)
+        lse = torch.empty((B * ctx.heads * Tq,), dtype=torch.float32, device=dev)
+        delta = torch.empty_like(lse)
+        be.attention_cross_bwd(qn.view(B, Tq, Cc), kvn.view(B, Tkv, 2 * Cc), out, don.view(B, Tq, Cc), ctx.heads,
+                               dq.view(B, Tq, Cc), dkv.view(B, Tkv, 2 * Cc), lse, delta)
+        return dq.permute(0, 3, 1, 2), dkv.permute(0, 3, 1, 2), None
+
+
 def gn_conv1x1(norm, conv1d: torch.nn.Conv1d, x4: torch.Tensor, enabled: bool = True):
     """conv1d_k1(GroupNorm32(x)) of AttentionBlock (openaimodel.py:307,321) fused like gn_act_conv2d, without
     the activation; None if the shape does not qualify."""
@@ -422,7 +544,7 @@ def gn_conv1x1(norm, conv1d: torch.nn.Conv1d, x4: torch.Tensor, enabled: bool = 
             and x4.shape[1] <= 4096):
         return None
     return GNActConv2dFn.apply(x4, norm.weight, norm.bias, None, None, conv1d.weight.unsqueeze(-1), conv1d.bias,
-                               0, None, False)
+                               0, None, False, norm.eps)
 
 
 def conv2d(conv: torch.nn.Conv2d, x: torch.Tensor, enabled: bool = True) -> torch.Tensor:

@@ -3,10 +3,14 @@
 Same parameter names and shapes as the reference modules
 (upstream model/BrownianBridge/base/modules/attention.py:36-264: GEGLU, FeedForward, CrossAttention,
 BasicTransformerBlock, SpatialTransformer), so checkpoints, EMA and ``weights_init`` (which keys on the class
-names ``Linear`` / ``Conv2d``) work unchanged.  The ``forward`` methods below are the training / autograd graph in
-stock PyTorch ops; no-grad CUDA calls are executed by ``bbdm_b200.engine.UNetEngine._spatial_transformer`` on the
-sm_90a kernels (GroupNorm + 1x1 projections and every Linear on the wgmma GEMM, LayerNorm / GEGLU as fused
-operand-producing passes, self- and cross-attention on the flash kernels).
+names ``Linear`` / ``Conv2d``) work unchanged.  No-grad CUDA calls are executed by
+``bbdm_b200.engine.UNetEngine._spatial_transformer`` on the sm_90a kernels (GroupNorm + 1x1 projections and every
+Linear on the wgmma GEMM, LayerNorm / GEGLU as fused operand-producing passes, self- and cross-attention on the flash
+kernels).  ``SpatialTransformer.forward`` is the training / autograd graph: on the device it runs the autograd
+Functions of ``bbdm_b200.train`` over the same kernels (each Linear a 1x1 ``Conv2dFn`` on the token grid,
+LayerNorm->Linear and GEGLU->Linear fused, the attention cores with flash-style backward kernels); on CPU tensors,
+shapes outside the kernels' envelope and with ``unet.NATIVE_TRAIN_CONV = False`` it runs the ``forward`` methods of
+the modules below, in stock PyTorch ops.
 
 Reference semantics kept: the UNet passes the SAME 4-D ``context`` tensor it concatenates to the input
 (openaimodel.py:741-748) to every transformer, where it is flattened to ``b (h w) c`` (attention.py:171-172), so
@@ -17,6 +21,8 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+
+from . import cabi, train
 
 
 def _zero(m):
@@ -92,6 +98,26 @@ class BasicTransformerBlock(nn.Module):
         x = self.attn2(self.norm2(x), context=context) + x
         return self.ff(self.norm3(x)) + x
 
+    def forward_native(self, h, context=None):
+        """forward() over the token grid h [B, C, H, W] (channels_last) on the autograd Functions of
+        bbdm_b200.train; context: the 4-D conditioning [B, context_dim, Hc, Wc] or None."""
+        a1, a2, ff = self.attn1, self.attn2, self.ff.net
+        ln_linear = lambda ln, x, w, b=None: train.LayerNormLinearFn.apply(x, ln.weight, ln.bias, w, b, ln.eps)
+        linear = lambda lin, x: train.Conv2dFn.apply(x, lin.weight[:, :, None, None], lin.bias)
+        # q|k|v as one GEMM over the concatenated weights (autograd splits the gradient back): q at channels h*D,
+        # k at C + h*D, v at 2C + h*D -- AttentionCoreFn's order 1; its (D^-1/4)^2 equals the D^-1/2 scale here
+        qkv_w = lambda a: torch.cat([a.to_q.weight, a.to_k.weight, a.to_v.weight])[:, :, None, None]
+        h = linear(a1.to_out[0], train.AttentionCoreFn.apply(ln_linear(self.norm1, h, qkv_w(a1)), a1.heads, 1)) + h
+        if context is None:               # attn2 attends to its own input: self-attention
+            o = train.AttentionCoreFn.apply(ln_linear(self.norm2, h, qkv_w(a2)), a2.heads, 1)
+        else:
+            # k|v of the few-channel context on the fp32 direct kernels (data gradient only if the context needs one)
+            kv = train.SmallConv2dFn.apply(context, torch.cat([a2.to_k.weight, a2.to_v.weight])[:, :, None, None], None)
+            o = train.CrossAttentionCoreFn.apply(ln_linear(self.norm2, h, a2.to_q.weight[:, :, None, None]), kv, a2.heads)
+        h = linear(a2.to_out[0], o) + h
+        u = ln_linear(self.norm3, h, ff[0].proj.weight[:, :, None, None], ff[0].proj.bias)
+        return train.GEGLULinearFn.apply(u, ff[2].weight[:, :, None, None], ff[2].bias) + h
+
 
 class SpatialTransformer(nn.Module):
     """GroupNorm(eps 1e-6) -> 1x1 proj_in -> depth x BasicTransformerBlock over 'b (h w) c' -> 1x1 proj_out -> + x
@@ -107,14 +133,28 @@ class SpatialTransformer(nn.Module):
             [BasicTransformerBlock(inner, n_heads, d_head, dropout=dropout, context_dim=context_dim) for _ in range(depth)])
         self.proj_out = _zero(nn.Conv2d(inner, in_channels, kernel_size=1))
 
-    _warned = False
+    def _native_ok(self, x, context):
+        """Shapes the training Functions' kernels take: tensor-core GEMM channel counts and token grid, GroupNorm
+        over 32 groups, LayerNorm width, attention head size, a few-channel fp32 context; no active dropout."""
+        inner = self.n_heads * self.d_head
+        ok = (train.native_ok(self.proj_in, x) and self.in_channels % 32 == 0 and self.in_channels <= 4096
+              and inner % 64 == 0 and inner <= cabi.LN_MAX_C and self.d_head in cabi.ATTN_HEAD_DIMS
+              and x.shape[0] * self.n_heads <= 65535
+              and not (self.training and any(m.p > 0 for m in self.modules() if isinstance(m, nn.Dropout))))
+        if context is not None:
+            ok = ok and (train._on_device(context) and context.dtype == torch.float32 and context.dim() == 4
+                         and context.shape[0] == x.shape[0] and context.shape[1] <= 32)
+        return ok
 
     def forward(self, x, context=None):
-        if x.is_cuda and not SpatialTransformer._warned:
-            SpatialTransformer._warned = True
-            import warnings
-            warnings.warn("bbdm_b200: SpatialTransformer blocks train on stock PyTorch kernels (their inference path is "
-                          "native: UNetEngine._spatial_transformer)", stacklevel=2)
+        from . import unet
+        if unet.NATIVE_TRAIN_CONV:
+            if self._native_ok(x, context):
+                h = train.gn_act_conv2d(self.norm, self.proj_in, x, act=False)
+                for blk in self.transformer_blocks:
+                    h = blk.forward_native(h, context)
+                return train.conv2d(self.proj_out, h) + x
+            train._library_path("SpatialTransformer", x)
         b, c, h, w = x.shape
         x_in = x
         x = self.proj_in(self.norm(x))

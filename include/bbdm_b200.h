@@ -374,7 +374,8 @@ int bbdm_conv_wgrad(const void* g_hi_t, const void* g_lo_t, const void* a_hi, co
                     int B, int H, int W, int Cin, int Cout, int taps, float* dw, float* workspace,
                     void* stream);
 
-/* Weight gradient of the small-channel fp32 convolutions (UNet stem / head; Cin*Cout <= 1024):
+/* Weight gradient of the small-channel fp32 convolutions (UNet stem / head, the SpatialTransformer's k|v
+ * projection of the few-channel context; Cin*Cout <= 2^24):
  * dy NHWC [B,H,W,Cout], x NHWC [B,H,W,Cin] fp32, stride 1, pad k/2 -> dw OIHW fp32 (overwritten).
  * workspace: any multiple of k*k*Cin*Cout floats (more = more CTAs, up to 4096); fixed-order reduce.
  * (The data gradient of these layers is bbdm_conv_direct with the flipped/transposed weights.) */
@@ -416,6 +417,19 @@ int bbdm_geglu_split(const float* u, int64_t rows, int N, float* out_f32, void* 
  * out[b,i,:] = softmax_j(q_i.k_j * D^-1/2) v_j per head, flash-style (no Tq x Tkv buffer).  D in {16,32,64,128}. */
 int bbdm_attention_cross(const void* q_hi, const void* q_lo, const void* kv_hi, const void* kv_lo, int B, int Tq,
                          int Tkv, int C, int heads, float* out_f32, void* out_hi, void* out_lo, void* stream);
+
+/* Training backward of the three ops above.
+ * bbdm_layernorm_bwd: x [rows][C] (the forward's input; mean / rstd are recomputed), dy [rows][C] -> dx [rows][C],
+ *   dgamma / dbeta [C] (fixed-order column sums, deterministic).  workspace: ceil(rows/64) * 2C floats.  C even, <= 2048.
+ * bbdm_geglu_bwd: u [rows][2N] (the forward's input), dy [rows][N] -> du [rows][2N] = [dy*gelu(g) | dy*a*gelu'(g)].
+ * bbdm_attention_cross_bwd: fp32 q [B,Tq,C], kv [B,Tkv,2C] and out [B,Tq,C] of bbdm_attention_cross, dout [B,Tq,C] ->
+ *   dq [B,Tq,C], dkv [B,Tkv,2C]; the probabilities are recomputed tile by tile (no Tq x Tkv buffer), exact fp32.
+ *   lse / delta: [B*heads*Tq] fp32 workspaces.  D in {16,32,64,128}; the same kernels as bbdm_attention_bwd. */
+int bbdm_layernorm_bwd(const float* x, const float* dy, int64_t rows, int C, const float* gamma, float eps, float* dx,
+                       float* dgamma, float* dbeta, float* workspace, void* stream);
+int bbdm_geglu_bwd(const float* u, const float* dy, int64_t rows, int N, float* du, void* stream);
+int bbdm_attention_cross_bwd(const float* q, const float* kv, const float* out, const float* dout, int B, int Tq, int Tkv,
+                             int C, int heads, float* dq, float* dkv, float* lse, float* delta, void* stream);
 
 /* SpatialRescaler, the latent model's cond-stage encoder (model/BrownianBridge/base/modules/encoders/modules.py:106-134:
  * n_stages x F.interpolate(scale_factor=0.5, mode='bilinear') then an optional 1x1 Conv2d channel_mapper), no-grad path,
