@@ -62,7 +62,8 @@ class _Pool:
 
 class KernelExecutor:
     """What every executor over the C-ABI kernels shares: the backend, the precision mode, the buffer
-    pools, GroupNorm statistics (fused partials or a stats pass) and the convolution dispatch."""
+    pools, GroupNorm statistics (fused partials or a stats pass), the convolution dispatch, and the
+    ResBlock flow, image head and resampling built on it."""
 
     gn_eps = GN_EPS
 
@@ -161,31 +162,75 @@ class KernelExecutor:
         self.be.conv_direct(a_f32, ent["f32"], bias, residual, out, cout, k, stride)
         return out, None, None
 
-    def _gn_act(self, pool, x, norm, umma, silu=True, want_raw_split=False, eps=None):
-        """GroupNorm (+ SiLU) of x as a conv operand: (a_f32, a_hi, a_lo, raw_hi, raw_lo)."""
+    def _gn_act(self, pool, x, norm, umma, silu=True, eps=None):
+        """GroupNorm (+ SiLU) of x as a conv operand: (a_f32, a_hi, a_lo)."""
         mean, rstd = self._stats(pool, x, None, eps=eps)
-        a_f32 = a_hi = a_lo = r_hi = r_lo = None
+        a_f32 = a_hi = a_lo = None
         if umma:
             a_hi, a_lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
         else:
             a_f32 = pool.get(x.shape)
-        if want_raw_split:
-            r_hi, r_lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
         self.be.prep(x, None, groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=norm.weight.detach(),
                      beta=norm.bias.detach(), silu=silu, resample=cabi.RESAMPLE_NONE, act_f32=a_f32, act_hi=a_hi,
-                     act_lo=a_lo, raw_hi=r_hi, raw_lo=r_lo)
+                     act_lo=a_lo)
         pool.put(mean, rstd)
-        return a_f32, a_hi, a_lo, r_hi, r_lo
+        return a_f32, a_hi, a_lo
 
-    def _padded_head(self, pool, h, norm, ent, out):
-        """GroupNorm -> SiLU -> 3x3 conv with Cout < 64 on the tensor-core path: the N tile is zero-padded to 64
-        couts and the epilogue stores the real ones into the NCHW tensor out."""
+    def _conv_plain(self, pool, ent, x, **kw):
+        """Conv of an fp32 NHWC tensor with no normalisation in front: on the tensor-core path from x's split planes,
+        else the fp32 direct conv.  kw: further _conv arguments."""
+        B, H, W, _ = x.shape
+        if "hi" in ent and W >= 4:
+            hi, lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
+            self.be.prep(x, None, raw_hi=hi, raw_lo=lo)
+            out, _, _ = self._conv(pool, ent, a_hi=hi, a_lo=lo, shape=(B, H, W), **kw)
+            pool.put(hi, lo)
+            return out
+        out, _, _ = self._conv(pool, ent, a_f32=x, shape=(B, H, W), **kw)
+        return out
+
+    def _head(self, pool, h, norm, ent, out=None):
+        """GroupNorm -> SiLU -> 3x3 conv of the last feature map h, which goes back to the pool here: the NHWC result,
+        or into the NCHW tensor out.  A head with Cout < 64 that has padded planes runs on the tensor-core path with
+        its N tile zero-padded to 64 couts, and the epilogue stores the real ones into out directly."""
         B, H, W, _ = h.shape
-        _, a_hi, a_lo, _, _ = self._gn_act(pool, h, norm, True)
-        self.be.conv_umma(B=B, H=H, W=W, Cin=ent["cin"], Cout=64, taps=9, a_hi=a_hi, a_lo=a_lo, w_hi=ent["hi_pad"],
-                          w_lo=ent["lo_pad"], bias=ent["bias_pad"], out=out, passes=self.passes,
-                          out_nchw_channels=out.shape[1])
-        pool.put(a_hi, a_lo)
+        if out is not None and "hi_pad" in ent and W >= 4:
+            _, a_hi, a_lo = self._gn_act(pool, h, norm, True)
+            self.be.conv_umma(B=B, H=H, W=W, Cin=ent["cin"], Cout=64, taps=9, a_hi=a_hi, a_lo=a_lo,
+                              w_hi=ent["hi_pad"], w_lo=ent["lo_pad"], bias=ent["bias_pad"], out=out,
+                              passes=self.passes, out_nchw_channels=out.shape[1])
+            pool.put(a_hi, a_lo, h)
+            return out
+        a_f32, a_hi, a_lo = self._gn_act(pool, h, norm, "hi" in ent and W >= 4)
+        pool.put(h)
+        y, _, _ = self._conv(pool, ent, a_f32=a_f32, a_hi=a_hi, a_lo=a_lo, shape=(B, H, W))
+        pool.put(a_f32, a_hi, a_lo)
+        if out is None:
+            return y
+        self.be.nhwc_to_nchw(y, out)
+        pool.put(y)
+        return out
+
+    def _upsample(self, pool, x, ent):
+        """Nearest-2x of x, then the 3x3 conv ent unless it is None: the fused 4-phase conv on x itself where the entry has
+        up-phase planes, else the direct conv of an upsampled fp32 copy."""
+        B, H, W, Cc = x.shape
+        if ent is not None and "up_hi" in ent and W >= 4:
+            return self._conv_plain(pool, ent, x, planes=(ent["up_hi"], ent["up_lo"]), taps=4, upsample2x=True,
+                                    stats=True)
+        up = pool.get((B, 2 * H, 2 * W, Cc))
+        self.be.prep(x, None, resample=cabi.RESAMPLE_UP2, raw_f32=up)
+        if ent is None:
+            return up
+        out, _, _ = self._conv(pool, ent, a_f32=up, shape=(B, 2 * H, 2 * W))
+        pool.put(up)
+        return out
+
+    def _avg_pool2(self, pool, x):
+        """2x2 average pool of x."""
+        B, H, W, Cc = x.shape
+        out = pool.get((B, H // 2, W // 2, Cc))
+        self.be.prep(x, None, resample=cabi.RESAMPLE_DOWN2, raw_f32=out)
         return out
 
     def _skip_residual(self, pool, es, src1, id_mode, r_f32, r_hi, r_lo, shape):
@@ -198,6 +243,104 @@ class KernelExecutor:
         if r_f32 is not None:
             return r_f32, cabi.RES_SAME, None
         return src1, id_mode, None
+
+    def _resblock_flow(self, pool, src1, src2, norm1, norm2, e1, e2, es, resample=cabi.RESAMPLE_NONE, film=None,
+                       bias1=None):
+        """ResBlock on cat(src1, src2): GN -> SiLU -> (up/down) -> conv1 (e1), GN (+FiLM) -> SiLU -> conv2 (e2), + the
+        skip conv es (None: identity skip).  Conditioning, if any: film = (scale, shift) views [B, Cout] of conv2's
+        FiLM rows, or bias1 = per-sample conv1 bias rows [B, Cout] that replace conv1's bias."""
+        be = self.be
+        B, Hs, Ws, c1 = src1.shape
+        c2 = 0 if src2 is None else src2.shape[3]
+        cin, cout = c1 + c2, e1["cout"]
+        H, W = {cabi.RESAMPLE_NONE: (Hs, Ws), cabi.RESAMPLE_UP2: (Hs * 2, Ws * 2),
+                cabi.RESAMPLE_DOWN2: (Hs // 2, Ws // 2)}[resample]
+        shape, shp = (B, H, W), (B, H, W, cin)
+        umma1 = self._umma_ok(cin, cout, W)
+        umma2 = self._umma_ok(cout, cout, W)
+        # a 1x1 skip conv rides as extra K-blocks of conv2 (or, before a Winograd conv2, as its own GEMM) on the raw
+        # input's split planes; any other skip that is not plain src1 needs the raw (resampled / concatenated) input
+        fuse_skip = es is not None and umma2 and es["k"] == 1 and cin % 64 == 0
+        need_raw_f32 = (es is not None and not fuse_skip) or \
+                       (es is None and (src2 is not None or (resample != cabi.RESAMPLE_NONE and not umma2)))
+        r_f32 = r_hi = r_lo = None
+
+        # ---- conv1: GN -> SiLU -> (up/down) -> conv3x3 ---------------------------------------------------------
+        mean, rstd = self._stats(pool, src1, src2)
+        gkw = dict(groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=norm1.weight.detach(), beta=norm1.bias.detach(),
+                   silu=True)
+        # the up-phase and Winograd convs add conv1's own bias: not taken with per-sample bias rows
+        if resample == cabi.RESAMPLE_UP2 and umma1 and "up_hi" in e1 and Ws >= 4 and bias1 is None \
+                and not need_raw_f32 and not fuse_skip:
+            # up-ResBlock on the tensor-core path: never materialise the upsampled activation -- the conv runs as
+            # 4 output phases x 2x2 taps on the low-res operand (2.25x fewer MACs)
+            a_hi, a_lo = pool.get((B, Hs, Ws, cin), torch.bfloat16), pool.get((B, Hs, Ws, cin), torch.bfloat16)
+            be.prep(src1, src2, **gkw, resample=cabi.RESAMPLE_NONE, act_hi=a_hi, act_lo=a_lo)
+            pool.put(mean, rstd)
+            h1, _, _ = self._conv(pool, e1, a_hi=a_hi, a_lo=a_lo, shape=(B, Hs, Ws), planes=(e1["up_hi"], e1["up_lo"]),
+                                  taps=4, upsample2x=True, stats=True)
+            pool.put(a_hi, a_lo)
+        elif umma1 and resample == cabi.RESAMPLE_NONE and not need_raw_f32 and bias1 is None \
+                and self._wino_ok(e1, B, H, W, c1):
+            # Winograd conv1; the raw split planes for a fused 1x1 skip come out of the same input pass
+            if fuse_skip:
+                r_hi, r_lo = pool.get(shp, torch.bfloat16), pool.get(shp, torch.bfloat16)
+            h1 = self._wino_conv(pool, e1, src1, src2, **gkw, raw_hi=r_hi, raw_lo=r_lo)
+            pool.put(mean, rstd)
+        else:
+            a_f32 = a_hi = a_lo = None
+            if umma1:
+                a_hi, a_lo = pool.get(shp, torch.bfloat16), pool.get(shp, torch.bfloat16)
+            else:
+                a_f32 = pool.get(shp)
+            if fuse_skip:
+                r_hi, r_lo = pool.get(shp, torch.bfloat16), pool.get(shp, torch.bfloat16)
+            if need_raw_f32:
+                r_f32 = pool.get(shp)
+            be.prep(src1, src2, **gkw, resample=resample, act_f32=a_f32, act_hi=a_hi, act_lo=a_lo,
+                    raw_f32=r_f32, raw_hi=r_hi, raw_lo=r_lo)
+            pool.put(mean, rstd)
+            if bias1 is None:
+                h1, _, _ = self._conv(pool, e1, a_f32=a_f32, a_hi=a_hi, a_lo=a_lo, shape=shape, stats=True)
+            else:
+                h1 = pool.get((B, H, W, cout))
+                for b in range(B):
+                    sl = lambda z: None if z is None else z[b:b + 1]
+                    self._conv(pool, e1, a_f32=sl(a_f32), a_hi=sl(a_hi), a_lo=sl(a_lo), shape=(1, H, W),
+                               bias=bias1[b], out=h1[b:b + 1])
+            pool.put(a_f32, a_hi, a_lo)
+
+        # ---- conv2: GN (+FiLM) -> SiLU -> conv3x3 (+skip) ------------------------------------------------------
+        mean, rstd = self._stats(pool, h1, None)
+        gkw = dict(groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=norm2.weight.detach(), beta=norm2.bias.detach(),
+                   silu=True)
+        if film is not None:
+            scale, shift = film
+            gkw.update(film_scale=scale, film_shift=shift, film_stride=scale.stride(0))
+        id_mode = resample_to_res(resample)
+        if umma2 and self._wino_ok(e2, B, H, W):
+            # Winograd conv2: the 1x1 skip (if any) runs as its own tensor-core GEMM and enters as the residual
+            residual, res_mode, skip_out = self._skip_residual(pool, es, src1, id_mode, r_f32, r_hi, r_lo, shape)
+            out = self._wino_conv(pool, e2, h1, None, **gkw, residual=residual, res_mode=res_mode)
+            pool.put(mean, rstd, h1)
+        else:
+            b_f32 = b_hi = b_lo = None
+            if umma2:
+                b_hi, b_lo = pool.get((B, H, W, cout), torch.bfloat16), pool.get((B, H, W, cout), torch.bfloat16)
+            else:
+                b_f32 = pool.get((B, H, W, cout))
+            be.prep(h1, None, **gkw, resample=cabi.RESAMPLE_NONE, act_f32=b_f32, act_hi=b_hi, act_lo=b_lo)
+            pool.put(mean, rstd, h1)
+            if fuse_skip:
+                second, residual, res_mode, skip_out = (es, r_hi, r_lo), None, cabi.RES_NONE, None
+            else:
+                second = None
+                residual, res_mode, skip_out = self._skip_residual(pool, es, src1, id_mode, r_f32, r_hi, r_lo, shape)
+            out, _, _ = self._conv(pool, e2, a_f32=b_f32, a_hi=b_hi, a_lo=b_lo, shape=shape, residual=residual,
+                                   res_mode=res_mode, second=second, stats=True)
+            pool.put(b_f32, b_hi, b_lo)
+        pool.put(r_f32, r_hi, r_lo, skip_out)
+        return out
 
     def _geom(self, H, W):
         key = (H, W)
@@ -369,103 +512,16 @@ class UNetEngine(KernelExecutor):
 
     # ------------------------------------------------------------------------------ blocks
     def _resblock(self, pool, name, m: ResBlock, src1, src2, film):
-        be, w = self.be, self._w
-        B, Hs, Ws, c1 = src1.shape
-        c2 = 0 if src2 is None else src2.shape[3]
-        cin, cout = c1 + c2, m.out_channels
-        assert cin == m.channels
+        w = self._w
+        assert src1.shape[3] + (0 if src2 is None else src2.shape[3]) == m.channels
         resample = cabi.RESAMPLE_UP2 if m.up else (cabi.RESAMPLE_DOWN2 if m.down else cabi.RESAMPLE_NONE)
-        H, W = (Hs * 2, Ws * 2) if m.up else ((Hs // 2, Ws // 2) if m.down else (Hs, Ws))
-        shape, shp = (B, H, W), (B, H, W, cin)
-        e1, e2 = w[name + ".in_layers.2"], w[name + ".out_layers.3"]
-        skip_conv = isinstance(m.skip_connection, nn.Conv2d)
-        es = w[name + ".skip_connection"] if skip_conv else None
-        umma1 = self._umma_ok(cin, cout, W)
-        umma2 = self._umma_ok(cout, cout, W)
-        # a 1x1 skip conv rides as extra K-blocks of conv2 (or, before a Winograd conv2, as its own GEMM) on the raw
-        # input's split planes; any other skip that is not plain src1 needs the raw (resampled / concatenated) input
-        fuse_skip = skip_conv and umma2 and es["k"] == 1 and cin % 64 == 0
-        need_raw_f32 = (skip_conv and not fuse_skip) or \
-                       (not skip_conv and (src2 is not None or (resample != cabi.RESAMPLE_NONE and not umma2)))
         foff, fn = w[name + "#film"]
-        r_f32 = r_hi = r_lo = None
-
-        # ---- conv1: GN -> SiLU -> (up/down) -> conv3x3 ---------------------------------------------------------
-        mean, rstd = self._stats(pool, src1, src2)
-        gn = m.in_layers[0]
-        gkw = dict(groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=gn.weight.detach(), beta=gn.bias.detach(), silu=True)
-        if m.up and umma1 and "up_hi" in e1 and Ws >= 4 and m.use_scale_shift_norm and not need_raw_f32 \
-                and not fuse_skip:
-            # up-ResBlock on the tensor-core path: never materialise the upsampled activation -- the conv runs as
-            # 4 output phases x 2x2 taps on the low-res operand (2.25x fewer MACs)
-            a_hi, a_lo = pool.get((B, Hs, Ws, cin), torch.bfloat16), pool.get((B, Hs, Ws, cin), torch.bfloat16)
-            be.prep(src1, src2, **gkw, resample=cabi.RESAMPLE_NONE, act_hi=a_hi, act_lo=a_lo)
-            pool.put(mean, rstd)
-            h1, _, _ = self._conv(pool, e1, a_hi=a_hi, a_lo=a_lo, shape=(B, Hs, Ws), planes=(e1["up_hi"], e1["up_lo"]),
-                                  taps=4, upsample2x=True, stats=True)
-            pool.put(a_hi, a_lo)
-        elif umma1 and resample == cabi.RESAMPLE_NONE and not need_raw_f32 and m.use_scale_shift_norm \
-                and self._wino_ok(e1, B, H, W, c1):
-            # Winograd conv1; the raw split planes for a fused 1x1 skip come out of the same input pass
-            if fuse_skip:
-                r_hi, r_lo = pool.get(shp, torch.bfloat16), pool.get(shp, torch.bfloat16)
-            h1 = self._wino_conv(pool, e1, src1, src2, **gkw, raw_hi=r_hi, raw_lo=r_lo)
-            pool.put(mean, rstd)
-        else:
-            a_f32 = a_hi = a_lo = None
-            if umma1:
-                a_hi, a_lo = pool.get(shp, torch.bfloat16), pool.get(shp, torch.bfloat16)
-            else:
-                a_f32 = pool.get(shp)
-            if fuse_skip:
-                r_hi, r_lo = pool.get(shp, torch.bfloat16), pool.get(shp, torch.bfloat16)
-            if need_raw_f32:
-                r_f32 = pool.get(shp)
-            be.prep(src1, src2, **gkw, resample=resample, act_f32=a_f32, act_hi=a_hi, act_lo=a_lo,
-                    raw_f32=r_f32, raw_hi=r_hi, raw_lo=r_lo)
-            pool.put(mean, rstd)
-            if m.use_scale_shift_norm:
-                h1, _, _ = self._conv(pool, e1, a_f32=a_f32, a_hi=a_hi, a_lo=a_lo, shape=shape, stats=True)
-            else:
-                # conv1 + (bias + emb_out[b]) per sample: per-sample bias rows live in `film`
-                h1 = pool.get((B, H, W, cout))
-                for b in range(B):
-                    sl = lambda z: None if z is None else z[b:b + 1]
-                    self._conv(pool, e1, a_f32=sl(a_f32), a_hi=sl(a_hi), a_lo=sl(a_lo), shape=(1, H, W),
-                               bias=film[b, foff:foff + fn], out=h1[b:b + 1])
-            pool.put(a_f32, a_hi, a_lo)
-
-        # ---- conv2: GN (+FiLM) -> SiLU -> conv3x3 (+skip) ------------------------------------------------------
-        mean, rstd = self._stats(pool, h1, None)
-        gn2 = m.out_layers[0]
-        gkw = dict(groups=GN_GROUPS, mean=mean, rstd=rstd, gamma=gn2.weight.detach(), beta=gn2.bias.detach(), silu=True)
-        if m.use_scale_shift_norm:
-            gkw.update(film_scale=film[:, foff:foff + cout], film_shift=film[:, foff + cout:foff + 2 * cout],
-                       film_stride=film.shape[1])
-        id_mode = resample_to_res(resample)
-        if umma2 and m.use_scale_shift_norm and self._wino_ok(e2, B, H, W):
-            # Winograd conv2: the 1x1 skip (if any) runs as its own tensor-core GEMM and enters as the residual
-            residual, res_mode, skip_out = self._skip_residual(pool, es, src1, id_mode, r_f32, r_hi, r_lo, shape)
-            out = self._wino_conv(pool, e2, h1, None, **gkw, residual=residual, res_mode=res_mode)
-            pool.put(mean, rstd, h1)
-        else:
-            b_f32 = b_hi = b_lo = None
-            if umma2:
-                b_hi, b_lo = pool.get((B, H, W, cout), torch.bfloat16), pool.get((B, H, W, cout), torch.bfloat16)
-            else:
-                b_f32 = pool.get((B, H, W, cout))
-            be.prep(h1, None, **gkw, resample=cabi.RESAMPLE_NONE, act_f32=b_f32, act_hi=b_hi, act_lo=b_lo)
-            pool.put(mean, rstd, h1)
-            if fuse_skip:
-                second, residual, res_mode, skip_out = (es, r_hi, r_lo), None, cabi.RES_NONE, None
-            else:
-                second = None
-                residual, res_mode, skip_out = self._skip_residual(pool, es, src1, id_mode, r_f32, r_hi, r_lo, shape)
-            out, _, _ = self._conv(pool, e2, a_f32=b_f32, a_hi=b_hi, a_lo=b_lo, shape=shape, residual=residual,
-                                   res_mode=res_mode, second=second, stats=True)
-            pool.put(b_f32, b_hi, b_lo)
-        pool.put(r_f32, r_hi, r_lo, skip_out)
-        return out
+        rows = film[:, foff:foff + fn]
+        # scale-shift: emb_out = [scale | shift] of out_layers' GroupNorm; else conv1's bias + emb_out per sample
+        cond = dict(film=rows.chunk(2, dim=1)) if m.use_scale_shift_norm else dict(bias1=rows)
+        es = w[name + ".skip_connection"] if isinstance(m.skip_connection, nn.Conv2d) else None
+        return self._resblock_flow(pool, src1, src2, m.in_layers[0], m.out_layers[0], w[name + ".in_layers.2"],
+                                   w[name + ".out_layers.3"], es, resample, **cond)
 
     def _attention(self, pool, name, m: AttentionBlock, x):
         be, w = self.be, self._w
@@ -477,7 +533,7 @@ class UNetEngine(KernelExecutor):
         if hd not in cabi.ATTN_HEAD_DIMS:
             raise NotImplementedError(f"attention head_dim {hd}: the sm_90a kernels support 16/32/64/128")
         umma = self._umma_ok(Cc, Cc, W)
-        a_f32, a_hi, a_lo, _, _ = self._gn_act(pool, x, m.norm, umma, silu=False)
+        a_f32, a_hi, a_lo = self._gn_act(pool, x, m.norm, umma, silu=False)
         # qkv 1x1: on the tensor-core path its epilogue writes the split planes the attention core reads
         qkv, q_hi, q_lo = self._conv(pool, eq, a_f32=a_f32, a_hi=a_hi, a_lo=a_lo, shape=(B, H, W),
                                      out_split=umma, want_f32=not umma)
@@ -529,7 +585,7 @@ class UNetEngine(KernelExecutor):
             raise NotImplementedError("SpatialTransformer: channel counts must be multiples of 64 (tensor-core GEMMs)")
         bf = torch.bfloat16
         tok = (B, H, W, inner)
-        _, a_hi, a_lo, _, _ = self._gn_act(pool, x, m.norm, True, silu=False, eps=m.norm.eps)
+        _, a_hi, a_lo = self._gn_act(pool, x, m.norm, True, silu=False, eps=m.norm.eps)
         h, _, _ = self._conv(pool, w[name + ".proj_in"], a_hi=a_hi, a_lo=a_lo, shape=(B, H, W))
         pool.put(a_hi, a_lo)
 
@@ -597,21 +653,11 @@ class UNetEngine(KernelExecutor):
         return out
 
     def _resample_layer(self, pool, name, m, x):
-        be, w = self.be, self._w
-        B, H, W, Cc = x.shape
-        if isinstance(m, Downsample):
-            if m.use_conv:
-                out, _, _ = self._conv(pool, w[name + ".op"], a_f32=x, shape=(B, H, W), stride=2)
-                return out
-            out = pool.get((B, H // 2, W // 2, Cc))
-            be.prep(x, None, resample=cabi.RESAMPLE_DOWN2, raw_f32=out)
-            return out
-        up = pool.get((B, H * 2, W * 2, Cc))
-        be.prep(x, None, resample=cabi.RESAMPLE_UP2, raw_f32=up)
+        if isinstance(m, Upsample):
+            return self._upsample(pool, x, self._w[name + ".conv"] if m.use_conv else None)
         if not m.use_conv:
-            return up
-        out, _, _ = self._conv(pool, w[name + ".conv"], a_f32=up, shape=(B, H * 2, W * 2))
-        pool.put(up)
+            return self._avg_pool2(pool, x)
+        out, _, _ = self._conv(pool, self._w[name + ".op"], a_f32=x, shape=x.shape[:3], stride=2)
         return out
 
     def _run_block(self, pool, prefix, block: TimestepEmbedSequential, h, skip, film, release_input):
@@ -690,17 +736,7 @@ class UNetEngine(KernelExecutor):
         # ---- head: GN -> SiLU -> conv3x3 -> NCHW ----------------------------------------------------
         if out is None:
             out = torch.empty((B, u.out_channels, H, W), dtype=torch.float32, device=dev)
-        eh, gn = w["out.2"], u.out[0]
-        if "hi_pad" in eh and W >= 4:
-            self._padded_head(pool, h, gn, eh, out)
-            pool.put(h)
-        else:
-            act, _, _, _, _ = self._gn_act(pool, h, gn, False)
-            pool.put(h)
-            y, _, _ = self._conv(pool, eh, a_f32=act, shape=(B, H, W))
-            pool.put(act)
-            be.nhwc_to_nchw(y, out)
-            pool.put(y)
+        self._head(pool, h, u.out[0], w["out.2"], out)
         pool.put(emb, film, self._ctx_nhwc)
         self._ctx_nhwc = None
         return out

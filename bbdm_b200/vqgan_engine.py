@@ -5,8 +5,9 @@ sample (LatentBrownianBridgeModel.py:57-100 of the reference).  This executor wa
 ``VQModel`` module tree (model/VQGAN/vqgan.py:30-88, model.py:342-537 -- the module stays the parameter
 container, exactly like the UNet) and issues the same kernels as the UNet executor:
 
-  ResnetBlock (model.py:76-138)   stats -> prep (GN eps 1e-6 + swish + split) -> wgmma conv, twice; the 1x1
-                                  nin_shortcut rides as extra K-blocks of conv2, the identity skip as its residual
+  ResnetBlock (model.py:76-138)   the UNet's ResBlock flow (KernelExecutor._resblock_flow) without conditioning,
+                                  GN eps 1e-6: the 1x1 nin_shortcut rides as extra K-blocks of conv2, the identity
+                                  skip as its residual
   AttnBlock   (model.py:140-192)  single head of width C: C <= 64 -> the flash kernels; C >= 128 -> per image two
                                   tensor-core GEMMs (S = Q K^T, O = P V) around bbdm_softmax_rows_split
   Downsample  (model.py:55-73)    zero-pad (0,1,0,1) + stride-2 conv = space-to-depth split + 2x2-tap wgmma conv
@@ -22,7 +23,7 @@ import torch
 import torch.nn as nn
 
 from . import cabi, convs
-from .engine import GN_GROUPS, KernelExecutor
+from .engine import KernelExecutor
 
 
 class VQGANEngine(KernelExecutor):
@@ -83,65 +84,11 @@ class VQGANEngine(KernelExecutor):
         self._w, self._wkey = w, key
 
     # ------------------------------------------------------------------------------ pieces
-    def _split(self, pool, x):
-        hi, lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
-        self.be.prep(x, None, raw_hi=hi, raw_lo=lo)
-        return hi, lo
-
-    def _conv_plain(self, pool, ent, x, **kw):
-        """conv on an fp32 NHWC tensor with no normalisation in front (conv_in, quant convs, shortcuts)."""
-        B, H, W, _ = x.shape
-        if "hi" in ent and W >= 4:
-            hi, lo = self._split(pool, x)
-            out, _, _ = self._conv(pool, ent, a_hi=hi, a_lo=lo, shape=(B, H, W), **kw)
-            pool.put(hi, lo)
-            return out
-        out, _, _ = self._conv(pool, ent, a_f32=x, shape=(B, H, W), **kw)
-        return out
-
     def _resnet(self, pool, name, m, x):
         w = self._w
-        B, H, W, cin = x.shape
-        e1, e2 = w[name + ".conv1"], w[name + ".conv2"]
         es = w.get(name + ".nin_shortcut", w.get(name + ".conv_shortcut"))
         assert (es is None) == (m.in_channels == m.out_channels)
-        umma1, umma2 = "hi" in e1 and W >= 4, "hi" in e2 and W >= 4
-        fuse_skip = es is not None and es["k"] == 1 and umma2 and "hi" in es
-        skip_umma = es is not None and not fuse_skip and "hi" in es and W >= 4
-        wino1, wino2 = umma1 and self._wino_ok(e1, B, H, W), umma2 and self._wino_ok(e2, B, H, W)
-        r_hi = r_lo = None
-        if wino1:
-            # Winograd conv1: the raw split planes a 1x1 shortcut needs come out of the same input pass
-            if fuse_skip or skip_umma:
-                r_hi, r_lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
-            mean, rstd = self._stats(pool, x, None)
-            h1 = self._wino_conv(pool, e1, x, None, groups=GN_GROUPS, mean=mean, rstd=rstd,
-                                 gamma=m.norm1.weight.detach(), beta=m.norm1.bias.detach(), raw_hi=r_hi, raw_lo=r_lo)
-            pool.put(mean, rstd)
-        else:
-            a_f32, a_hi, a_lo, r_hi, r_lo = self._gn_act(pool, x, m.norm1, umma1, want_raw_split=fuse_skip or skip_umma)
-            h1, _, _ = self._conv(pool, e1, a_f32=a_f32, a_hi=a_hi, a_lo=a_lo, shape=(B, H, W), stats=True)
-            pool.put(a_f32, a_hi, a_lo)
-        if wino2:
-            # Winograd conv2: the shortcut (1x1 GEMM or identity) enters as the output transform's residual
-            residual, res_mode, sk = self._skip_residual(pool, es, x, cabi.RES_SAME, x, r_hi, r_lo, (B, H, W))
-            mean, rstd = self._stats(pool, h1, None)
-            out = self._wino_conv(pool, e2, h1, None, groups=GN_GROUPS, mean=mean, rstd=rstd,
-                                  gamma=m.norm2.weight.detach(), beta=m.norm2.bias.detach(), residual=residual,
-                                  res_mode=res_mode)
-            pool.put(mean, rstd, h1, r_hi, r_lo, sk)
-            return out
-        b_f32, b_hi, b_lo, _, _ = self._gn_act(pool, h1, m.norm2, umma2)
-        pool.put(h1)
-        kw = dict(a_f32=b_f32, a_hi=b_hi, a_lo=b_lo, shape=(B, H, W), stats=True)
-        if fuse_skip:
-            sk = None
-            out, _, _ = self._conv(pool, e2, second=(es, r_hi, r_lo), **kw)
-        else:
-            residual, res_mode, sk = self._skip_residual(pool, es, x, cabi.RES_SAME, x, r_hi, r_lo, (B, H, W))
-            out, _, _ = self._conv(pool, e2, residual=residual, res_mode=res_mode, **kw)
-        pool.put(b_f32, b_hi, b_lo, r_hi, r_lo, sk)
-        return out
+        return self._resblock_flow(pool, x, None, m.norm1, m.norm2, w[name + ".conv1"], w[name + ".conv2"], es)
 
     def _attn(self, pool, name, m, x):
         be, w = self.be, self._w
@@ -149,7 +96,7 @@ class VQGANEngine(KernelExecutor):
         T = H * W
         ep = w[name + ".proj_out"]
         umma = self._umma_ok(Cc, Cc, W)
-        a_f32, a_hi, a_lo, _, _ = self._gn_act(pool, x, m.norm, umma, silu=False)
+        a_f32, a_hi, a_lo = self._gn_act(pool, x, m.norm, umma, silu=False)
         o_f32 = o_hi = o_lo = None
         if Cc in (16, 32, 64):
             # one head of width C: the flash kernel's scale D^-1/4 on q and on k is the reference's C^-1/2
@@ -193,41 +140,19 @@ class VQGANEngine(KernelExecutor):
 
     def _downsample(self, pool, name, m, x):
         B, H, W, Cc = x.shape
-        if m.with_conv:
-            ent = self._w[name + ".conv"]
-            if "ds_hi" in ent and H % 2 == 0 and W % 2 == 0 and W // 2 >= 4:
-                hi = pool.get((B, H // 2, W // 2, 4 * Cc), torch.bfloat16)
-                lo = pool.get((B, H // 2, W // 2, 4 * Cc), torch.bfloat16)
-                self.be.s2d_split(x, hi, lo)
-                out, _, _ = self._conv(pool, ent, a_hi=hi, a_lo=lo, shape=(B, H // 2, W // 2),
-                                       planes=(ent["ds_hi"], ent["ds_lo"]), taps=4, stats=True)
-                pool.put(hi, lo)
-                return out
-            out = pool.get((B, (H + 1 - 3) // 2 + 1, (W + 1 - 3) // 2 + 1, Cc))
-            self.be.conv_direct_pad(x, ent["f32"], ent["bias"], None, out, Cc, 3, 2, 0, 1)
-            return out
-        out = pool.get((B, H // 2, W // 2, Cc))
-        self.be.prep(x, None, resample=cabi.RESAMPLE_DOWN2, raw_f32=out)
-        return out
-
-    def _upsample(self, pool, name, m, x):
-        be = self.be
-        B, H, W, Cc = x.shape
         if not m.with_conv:
-            up = pool.get((B, 2 * H, 2 * W, Cc))
-            be.prep(x, None, resample=cabi.RESAMPLE_UP2, raw_f32=up)
-            return up
+            return self._avg_pool2(pool, x)
         ent = self._w[name + ".conv"]
-        if "up_hi" in ent and W >= 4:
-            hi, lo = self._split(pool, x)
-            out, _, _ = self._conv(pool, ent, a_hi=hi, a_lo=lo, shape=(B, H, W), planes=(ent["up_hi"], ent["up_lo"]),
-                                   taps=4, upsample2x=True, stats=True)
+        if "ds_hi" in ent and H % 2 == 0 and W % 2 == 0 and W // 2 >= 4:
+            hi = pool.get((B, H // 2, W // 2, 4 * Cc), torch.bfloat16)
+            lo = pool.get((B, H // 2, W // 2, 4 * Cc), torch.bfloat16)
+            self.be.s2d_split(x, hi, lo)
+            out, _, _ = self._conv(pool, ent, a_hi=hi, a_lo=lo, shape=(B, H // 2, W // 2),
+                                   planes=(ent["ds_hi"], ent["ds_lo"]), taps=4, stats=True)
             pool.put(hi, lo)
             return out
-        up = pool.get((B, 2 * H, 2 * W, Cc))
-        be.prep(x, None, resample=cabi.RESAMPLE_UP2, raw_f32=up)
-        out, _, _ = self._conv(pool, ent, a_f32=up, shape=(B, 2 * H, 2 * W))
-        pool.put(up)
+        out = pool.get((B, (H + 1 - 3) // 2 + 1, (W + 1 - 3) // 2 + 1, Cc))
+        self.be.conv_direct_pad(x, ent["f32"], ent["bias"], None, out, Cc, 3, 2, 0, 1)
         return out
 
     def _step(self, pool, h, fn, *args):
@@ -245,20 +170,6 @@ class VQGANEngine(KernelExecutor):
         xin = pool.get((B, H, W, Cx))
         self.be.nchw_to_nhwc_cat(x.contiguous().float(), None, xin)
         return xin
-
-    def _head(self, pool, h, norm, ent, out=None):
-        """norm_out -> swish -> conv_out: the NHWC result, or into the NCHW tensor out."""
-        B, H, W, _ = h.shape
-        if out is not None and "hi_pad" in ent and W >= 4:
-            return self._padded_head(pool, h, norm, ent, out)
-        a_f32, a_hi, a_lo, _, _ = self._gn_act(pool, h, norm, "hi" in ent and W >= 4)
-        y, _, _ = self._conv(pool, ent, a_f32=a_f32, a_hi=a_hi, a_lo=a_lo, shape=(B, H, W))
-        pool.put(a_f32, a_hi, a_lo)
-        if out is None:
-            return y
-        self.be.nhwc_to_nchw(y, out)
-        pool.put(y)
-        return out
 
     # ------------------------------------------------------------------------------ public
     # activation budget of one pass: 32 images of 256x256 (the cfg3 batch; ~25 GB of pooled NHWC tensors and operand
@@ -294,7 +205,6 @@ class VQGANEngine(KernelExecutor):
                 h = self._step(pool, h, self._downsample, f"encoder.down.{i}.downsample", lvl.downsample)
         h = self._mid(pool, "encoder.mid", enc.mid, h)
         y = self._head(pool, h, enc.norm_out, w["encoder.conv_out"])
-        pool.put(h)
         if quant_conv:
             y = self._step(pool, y, lambda p, t: self._conv_plain(p, w["quant_conv"], t))
         B, H, W, Cz = y.shape
@@ -344,10 +254,10 @@ class VQGANEngine(KernelExecutor):
                 if len(lvl.attn) > 0:
                     h = self._step(pool, h, self._attn, f"decoder.up.{i}.attn.{j}", lvl.attn[j])
             if i != 0:
-                h = self._step(pool, h, self._upsample, f"decoder.up.{i}.upsample", lvl.upsample)
+                ent = w[f"decoder.up.{i}.upsample.conv"] if lvl.upsample.with_conv else None
+                h = self._step(pool, h, lambda p, t: self._upsample(p, t, ent))
         ent = w["decoder.conv_out"]
         B, H, W, _ = h.shape
         out = torch.empty((B, ent["cout"], H, W), dtype=torch.float32, device=z.device)
         self._head(pool, h, dec.norm_out, ent, out)
-        pool.put(h)
         return (out, indices) if return_indices else out

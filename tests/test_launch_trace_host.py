@@ -7,8 +7,10 @@ keeps every logged tensor alive, so a freed address cannot come back as another 
 buffer pools' reuse pattern, which CUDA-graph replay depends on, and not only the launch sequence.
 
 tests/golden/launch_traces.json holds the sha256, the call count and the per-method counts of each scenario's trace,
-recorded from the executors before they were moved onto the shared code in bbdm_b200/convs.py.  A change to the host
-code that is meant to be a pure refactor must leave every trace unchanged.  On a mismatch the full trace is written to
+recorded from the executors before they were moved onto the shared code in bbdm_b200/convs.py; vqgan_vq_small and
+vqgan_vq_tc_winograd were re-recorded when the VQGAN's ResnetBlocks moved onto the UNet's ResBlock flow (a raw fp32
+input copy for an unfused 1x1 shortcut; the skip GEMM after conv2's GroupNorm statistics).  A change to the host code
+that is meant to be a pure refactor must leave every trace unchanged.  On a mismatch the full trace is written to
 the test's tmp_path, to be diffed against one dumped from the earlier code."""
 import collections
 import hashlib
