@@ -90,7 +90,7 @@ class WinoInputArgs(C.Structure):
 class WinoOutputArgs(C.Structure):
     _fields_ = [("m", C.c_void_p), ("inv_wscale", C.c_void_p), ("B", C.c_int), ("H", C.c_int), ("W", C.c_int), ("Cout", C.c_int),
                 ("bias", C.c_void_p), ("residual", C.c_void_p), ("res_mode", C.c_int),
-                ("out", C.c_void_p), ("stats_partial", C.c_void_p)]
+                ("out", C.c_void_p), ("stats_partial", C.c_void_p), ("up2_phases", C.c_int)]
 
 
 class BbdmError(RuntimeError):
@@ -400,11 +400,12 @@ class CudaBackend:
         LAUNCHES["n"] += 1
 
     def wino_output(self, m, *, B, H, W, Cout, bias=None, residual=None, res_mode=RES_NONE, out, stats_partial=None,
-                    inv_wscale=None, tile=4):
+                    inv_wscale=None, tile=4, up2_phases=False):
         """inv_wscale: the [1] fp32 device tensor wino_pack_weight wrote for the weight planes of this GEMM (None:
-        planes packed at the fixed 2^8)."""
+        planes packed at the fixed 2^8).  up2_phases (tile 6): m holds the 4*Cout phase-major channels of a nearest-2x
+        + 3x3 conv run on the HxW map; out is [B, 2H, 2W, Cout]."""
         a = WinoOutputArgs(ptr(_req(m)), None if inv_wscale is None else ptr(_req(inv_wscale)), B, H, W, Cout, ptr(bias), ptr(residual), res_mode, ptr(_req(out)),
-                           ptr(stats_partial))
+                           ptr(stats_partial), int(up2_phases))
         check(self._wino("output", tile)(C.byref(a), stream()))
         LAUNCHES["n"] += 1
 

@@ -68,19 +68,25 @@ class FreshBuffers:
 
 
 def wino_conv(be, pool, geometry, src1, src2, *, cout, planes=None, weight=None, dgrad=False, bias=None,
-              residual=None, res_mode=cabi.RES_NONE, stats=False, tile=4, **transform):
+              residual=None, res_mode=cabi.RES_NONE, stats=False, tile=4, up2_phases=False, **transform):
     """3x3 conv of cat(src1, src2) (NHWC fp32) on the Winograd path: input transform (``transform`` are the
     wino_input arguments: GroupNorm affine + FiLM + SiLU, or identity with silu=False; raw_* / act_* side outputs) ->
     (tile+2)^2 position GEMMs in one wgmma launch -> output transform (+ bias, + residual, + GroupNorm partial sums if
     stats).  tile: 4 (F(4x4,3x3)) or 6 (F(6x6,3x3)); geometry is the backend's wino_geometry for that tile.
 
     planes = (u_hi, u_lo, u_inv) packed beforehand (WeightPacker.winograd, same tile), or weight [Cout, Cin, 3, 3] to
-    pack here (dgrad: the flipped, channel-swapped kernel).  pool: the executors' _Pool or FreshBuffers."""
+    pack here (dgrad: the flipped, channel-swapped kernel).  pool: the executors' _Pool or FreshBuffers.
+
+    up2_phases (tile 6, planes of WeightPacker.up_phase_winograd): nearest-2x upsample of the activated input, then the
+    3x3 conv -- run on the input's own map as a 3x3 conv with 4*cout phase-major outputs, whose output transform
+    interleaves the phases into the [B, 2H, 2W, cout] result (bias [cout], no residual)."""
     B, H, W, c1 = src1.shape
     cin = c1 + (0 if src2 is None else src2.shape[3])
     th, _, mtot, _ = geometry
     npos = (tile + 2) ** 2
     tkw = {} if tile == 4 else dict(tile=tile)
+    assert not up2_phases or (tile == 6 and planes is not None and residual is None)
+    ncols = 4 * cout if up2_phases else cout            # output channels of the position GEMMs
     v_hi, v_lo = pool.get((npos, mtot, cin), torch.float16), pool.get((npos, mtot, cin), torch.float16)
     be.wino_input(src1, src2, v_hi=v_hi, v_lo=v_lo, **transform, **tkw)
     if planes is None:
@@ -92,17 +98,21 @@ def wino_conv(be, pool, geometry, src1, src2, *, cout, planes=None, weight=None,
     else:
         u_hi, u_lo, u_inv = planes
         assert u_hi.shape[0] == npos, (u_hi.shape, tile)
-    m = pool.get((npos, mtot, cout))
-    be.conv_umma(B=npos, H=mtot // 16, W=16, Cin=cin, Cout=cout, taps=1, a_hi=v_hi, a_lo=v_lo, w_hi=u_hi, w_lo=u_lo,
+    m = pool.get((npos, mtot, ncols))
+    be.conv_umma(B=npos, H=mtot // 16, W=16, Cin=cin, Cout=ncols, taps=1, a_hi=v_hi, a_lo=v_lo, w_hi=u_hi, w_lo=u_lo,
                  out=m, passes=3, weights_per_image=True, operand_f16=True)
     pool.put(v_hi, v_lo)
-    out = pool.get((B, H, W, cout))
-    part = pool.get((B * th, cout, 2)) if stats else None
+    f = 2 if up2_phases else 1
+    rows = 4 * th if up2_phases else th                 # GroupNorm partial-sum rows per image
+    out = pool.get((B, f * H, f * W, cout))
+    part = pool.get((B * rows, cout, 2)) if stats else None
+    if up2_phases:
+        tkw["up2_phases"] = True
     be.wino_output(m, B=B, H=H, W=W, Cout=cout, bias=bias, residual=residual, res_mode=res_mode, out=out,
                    stats_partial=part, **({} if u_inv is None else dict(inv_wscale=u_inv)), **tkw)
     pool.put(m)
     if part is not None:
-        out._gn = (part, th)
+        out._gn = (part, rows)
     return out
 
 
@@ -177,3 +187,18 @@ class WeightPacker:
         ent["up_hi"] = self._buf(name, "up_hi", (16, ent["cout"], ent["cin"]), torch.bfloat16)
         ent["up_lo"] = self._buf(name, "up_lo", (16, ent["cout"], ent["cin"]), torch.bfloat16)
         self.be.pack_weight_split_taps(upsample_phase_weights(weight.detach()), ent["up_hi"], ent["up_lo"])
+
+    def up_phase_winograd(self, name, weight):
+        """F(6x6,3x3) planes of nearest-2x + the packed 3x3 conv ``name`` as one 3x3 conv on the low-res map with
+        4*Cout outputs, phase-major (phase = 2a + b of output pixel (2y+a, 2x+b)): each phase's 2x2 taps sit in the
+        3x3 window at rows a..a+1, columns b..b+1.  A conv entry of its own, ``name + "#up6"`` (cout = 4*Cout),
+        that ent["up6"] refers to, for convs.wino_conv(up2_phases=True)."""
+        ent = self.w[name]
+        cout, cin = ent["cout"], ent["cin"]
+        pw = upsample_phase_weights(weight.detach()).view(cout, cin, 2, 2, 2, 2)      # [o, i, a, b, r, c]
+        w3 = torch.zeros(2, 2, cout, cin, 3, 3, dtype=pw.dtype, device=pw.device)
+        for a in range(2):
+            for b in range(2):
+                w3[a, b, :, :, a:a + 2, b:b + 2] = pw[:, :, a, b]
+        ent["up6"] = self.w[name + "#up6"] = {"cout": 4 * cout, "cin": cin, "k": 3}
+        self.winograd(name + "#up6", w3.view(4 * cout, cin, 3, 3), tile=6)

@@ -563,16 +563,25 @@ wino_output_kernel(const WinoOutParams p) {
   }
 }
 
+// F(6,3) output form of the phase-stacked nearest-2x conv (used as the RES template value, no residual): M holds 4*Cout
+// channels c' = phase * Cout + co on the LOW-RES tile grid of an H x W map, and pixel (i, j) of tile (ty, tx) in phase
+// (a, b) = (phase >> 1, phase & 1) is output pixel (2(6ty+i)+a, 2(6tx+j)+b), channel co, of the [B, 2H, 2W, Cout] result.
+constexpr int WINO6_UP_PHASES = 4;
+
 // F(6x6,3x3): one output tile (6x6 pixels) of ONE channel (64 M values instead of 2 x 36: one channel per thread keeps
 // the F(4,3) kernel's register budget).  Tiles run over ceil(H/6) x ceil(W/6): pixels, residual reads and partial sums
-// past H or W are masked.  __host__ __device__: tools/host_check_wino6_output.cu runs it on the CPU.
+// past H or W are masked.  c is the channel of M (WINO6_UP_PHASES: phase * Cout + co); bv the bias of its output
+// channel.  __host__ __device__: tools/host_check_wino6_output.cu and tools/host_check_wino6_up2_output.cu run it on
+// the CPU.
 template <int RES>
 __host__ __device__ __forceinline__ void wino6_output_tile(const WinoOutParams& p, int b, int ty, int tx, int c, float bv,
                                                            float inv, float& sum, float& sq) {
+  constexpr bool UP = RES == WINO6_UP_PHASES;
   const int64_t m = ((int64_t)b * p.th + ty) * p.tw + tx;
+  const int ldm = UP ? 4 * p.Cout : p.Cout;
   float mm[64];
 #pragma unroll
-  for (int q = 0; q < 64; ++q) mm[q] = p.m[((int64_t)q * p.Mtot + m) * p.Cout + c];
+  for (int q = 0; q < 64; ++q) mm[q] = p.m[((int64_t)q * p.Mtot + m) * ldm + c];
   // Y = A^T M A: columns (8 -> 6 rows), then rows (8 -> 6 columns)
   float t6[48], y[36];
 #pragma unroll
@@ -593,7 +602,16 @@ __host__ __device__ __forceinline__ void wino6_output_tile(const WinoOutParams& 
   }
   // three output rows at a time: their residual values (same / 2x2-average addressed) are fetched as one batch ahead
   // of their stores
-  const int64_t pix0 = ((int64_t)b * p.H + h0) * p.W + w0;          // first pixel of the tile
+  int co = c;
+  int64_t pix0 = ((int64_t)b * p.H + h0) * p.W + w0;                // first pixel of the tile
+  int64_t rstep = p.W, cstep = 1;                                   // output pixels per tile row / column
+  if constexpr (UP) {
+    const int ph = c / p.Cout;
+    co = c - ph * p.Cout;
+    pix0 = ((int64_t)b * 2 * p.H + 2 * h0 + (ph >> 1)) * (2 * p.W) + 2 * w0 + (ph & 1);
+    rstep = 4 * (int64_t)p.W;
+    cstep = 2;
+  }
 #pragma unroll
   for (int i0 = 0; i0 < 6; i0 += 3) {
     float rs[18];
@@ -619,7 +637,7 @@ __host__ __device__ __forceinline__ void wino6_output_tile(const WinoOutParams& 
         float r = fmaf(y[(i0 + i) * 6 + j], inv, bv);
         if constexpr (RES == BBDM_RES_SAME || RES == BBDM_RES_DOWN2) r += rs[i * 6 + j];
         else if constexpr (RES == BBDM_RES_UP2) r += rup[((i0 + i) >> 1) * 3 + (j >> 1)];
-        p.out[(pix0 + (int64_t)(i0 + i) * p.W + j) * p.Cout + c] = r;
+        p.out[(pix0 + (i0 + i) * rstep + j * cstep) * p.Cout + co] = r;
         sum += r;
         sq = fmaf(r, r, sq);
       }
@@ -627,7 +645,8 @@ __host__ __device__ __forceinline__ void wino6_output_tile(const WinoOutParams& 
 }
 
 // One CTA per (64-channel group, tile row ty, sample b): 64 channels x 4 tile-column lanes (a warp reads 128
-// contiguous bytes of M per position).
+// contiguous bytes of M per position).  WINO6_UP_PHASES: 4*Cout/64 channel groups of M, each inside one phase, and one
+// partial-sum row per (tile row, phase).
 // The same-addressed and 2x2-averaged residual modes need more than 128 registers (ptxas: spills at 2 CTAs per SM).
 template <int RES>
 __global__ void __launch_bounds__(256, RES == BBDM_RES_SAME || RES == BBDM_RES_DOWN2 ? 1 : 2)
@@ -636,7 +655,9 @@ wino6_output_kernel(const WinoOutParams p) {
   const int cg = blockIdx.x, ty = blockIdx.y, b = blockIdx.z;
   const int cl = threadIdx.x & 63, tl = threadIdx.x >> 6;
   const int c = cg * 64 + cl;
-  const float bv = p.bias ? p.bias[c] : 0.f;
+  const int ph = RES == WINO6_UP_PHASES ? cg * 64 / p.Cout : 0;
+  const int co0 = cg * 64 - ph * p.Cout;                            // first output channel of the group
+  const float bv = p.bias ? p.bias[co0 + cl] : 0.f;
   const float inv = p.inv_wscale ? __ldg(p.inv_wscale) : 1.0f / WINO_WSCALE_FIXED;
   float sum = 0.f, sq = 0.f;
   for (int tx = tl; tx < p.tw; tx += 4) wino6_output_tile<RES>(p, b, ty, tx, c, bv, inv, sum, sq);
@@ -648,8 +669,8 @@ wino6_output_kernel(const WinoOutParams p) {
       float a = 0.f, q = 0.f;
 #pragma unroll
       for (int k = 0; k < 4; ++k) { a += red[k][threadIdx.x][0]; q += red[k][threadIdx.x][1]; }
-      const int64_t prow = (int64_t)b * p.th + ty;
-      *reinterpret_cast<float2*>(p.stats + (prow * p.Cout + cg * 64 + threadIdx.x) * 2) = make_float2(a, q);
+      const int64_t prow = RES == WINO6_UP_PHASES ? ((int64_t)b * p.th + ty) * 4 + ph : (int64_t)b * p.th + ty;
+      *reinterpret_cast<float2*>(p.stats + (prow * p.Cout + co0 + threadIdx.x) * 2) = make_float2(a, q);
     }
   }
 }
@@ -846,13 +867,17 @@ int wino_output_t(const BbdmWinoOutputArgs* a, void* stream) {
   BBDM_REQUIRE(p.Cout > 0 && p.Cout % 64 == 0, "wino_output: Cout %% 64 != 0");
   BBDM_REQUIRE(a->res_mode >= 0 && a->res_mode <= 3 && (a->res_mode == 0 || a->residual), "wino_output: bad residual");
   if (a->res_mode == BBDM_RES_UP2) BBDM_REQUIRE(p.H % 2 == 0 && p.W % 2 == 0, "wino_output: RES_UP2 needs even H, W");
+  BBDM_REQUIRE(!a->up2_phases || (T == 6 && a->res_mode == BBDM_RES_NONE),
+               "wino_output: up2_phases is an F(6,3) form without a residual");
   wino_geometry_t<T>(p.B, p.H, p.W, &p.th, &p.tw, &p.Mtot, nullptr);
   BBDM_REQUIRE(p.th <= 65535, "wino_output: too many tile rows");
   p.bias = a->bias; p.residual = a->residual; p.res_mode = a->res_mode;
   p.out = a->out; p.stats = a->stats_partial;
-  dim3 grid(p.Cout / 64, p.th, p.B);
+  dim3 grid(p.Cout / 64 * (a->up2_phases ? 4 : 1), p.th, p.B);
   cudaStream_t st = (cudaStream_t)stream;
-  if constexpr (T == 4) {
+  if (a->up2_phases) {
+    wino6_output_kernel<WINO6_UP_PHASES><<<grid, 256, 0, st>>>(p);
+  } else if constexpr (T == 4) {
     switch (p.res_mode) {
       case BBDM_RES_SAME: wino_output_kernel<BBDM_RES_SAME><<<grid, 256, 0, st>>>(p); break;
       case BBDM_RES_UP2: wino_output_kernel<BBDM_RES_UP2><<<grid, 256, 0, st>>>(p); break;

@@ -292,6 +292,7 @@ typedef struct {
   const float* residual; int res_mode;
   float* out;
   float* stats_partial;
+  int up2_phases;            /* F(6,3) only, res_mode 0: see bbdm_wino6_output below */
 } BbdmWinoOutputArgs;
 int bbdm_wino_output(const BbdmWinoOutputArgs* a, void* stream);
 
@@ -317,6 +318,10 @@ int bbdm_wino_pack_weight(const float* w, int Cout, int Cin, int dgrad, void* u_
  *                that is not a finite fp16 number sets the device fault word to 0xC0000000 | C
  *                (bbdm_check_device_fault reports it).
  *   output       m [64][tiles_total][Cout]; stats_partial [B * tiles_h][Cout][2].
+ *                up2_phases != 0: the output of a nearest-2x upsample followed by a 3x3 conv, run as one 3x3 conv on
+ *                the H x W (low-res) map with 4*Cout outputs, phase-major: channel phase*Cout + co of m is output
+ *                channel co at the pixels (2y+a, 2x+b) of out [B, 2H, 2W, Cout], phase = 2a + b.  bias [Cout];
+ *                no residual; stats_partial [B * tiles_h * 4][Cout][2] (rows_per_image = 4 * tiles_h).
  *   pack_weight  u_hi, u_lo [64][Cout][Cin] (dgrad: [64][Cin][Cout]); the same scale s (|s U| <= 1.55 * 2^14). */
 int bbdm_wino6_geometry(int B, int H, int W, int* tiles_h, int* tiles_w, int64_t* tiles_total, int* eligible);
 int bbdm_wino6_input(const BbdmWinoInputArgs* a, void* stream);

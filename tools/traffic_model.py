@@ -52,15 +52,32 @@ class Rec:
     def pack_weight_split_taps(self, *a): pass
     def pack_weight_f32(self, *a): pass
     def conv_umma(self, **kw):
+        # FLOPs: 2x the MACs the kernel issues (split3 runs each product three times on the tensor pipe)
         B, H, W, Cin, Cout, taps = (kw[k] for k in ("B", "H", "W", "Cin", "Cout", "taps"))
         up = kw.get("upsample2x")
-        npx = B * H * W * (4 if up else 1)
-        fl = 2.0 * npx * Cout * (9 * Cin if up else taps * Cin + kw.get("Cin2", 0))
+        fl = 2.0 * B * H * W * (4 if up else 1) * Cout * (taps * Cin + kw.get("Cin2", 0))
         by = nbytes(kw["a_hi"], kw["a_lo"], kw["w_hi"], kw["w_lo"], kw.get("a2_hi"), kw.get("a2_lo"), kw.get("out"),
                     kw.get("out_hi"), kw.get("out_lo"), kw.get("stats_partial"))
         if kw.get("res_mode"):
             by += nbytes(kw["residual"])
-        self._add("conv_umma", by, fl)
+        fam = "wino_gemm" if kw.get("weights_per_image") else ("conv_umma_up2" if up else f"conv_umma_{taps}tap")
+        self._add(fam, by, fl)
+    # Winograd transforms (F(4x4,3x3) and F(6x6,3x3)) and their tile grids, as bbdm_wino*_geometry computes them
+    wino_tiles = (4, 6)
+    wino_tensor_scale = True
+    def wino_geometry(self, B, H, W, tile=4):
+        th, tw = -(-H // tile), -(-W // tile)
+        tot = B * th * tw
+        if tile == 6:
+            return th, tw, max(128, -(-tot // 16) * 16), True
+        return th, tw, tot, H % 4 == 0 and W % 4 == 0 and tot % 16 == 0 and tot >= 128
+    def wino_pack_weight(self, *a, **kw): pass
+    def wino_input(self, s1, s2, **kw):
+        outs = [kw.get(k) for k in ("v_hi", "v_lo", "raw_hi", "raw_lo", "act_hi", "act_lo")]
+        self._add("wino_input", nbytes(s1, s2, *outs))
+    def wino_output(self, m, **kw):
+        res = kw.get("residual") if kw.get("res_mode") else None
+        self._add("wino_output", nbytes(m, res, kw["out"], kw.get("stats_partial")))
     def conv_direct(self, src, w, bias, res, out, Cout, k, stride=1):
         self._add("conv_direct", nbytes(src, w, res, out), 2.0 * out.numel() * src.shape[3] * k * k)
     def attention(self, qkv, heads, order, out_f32=None, out_hi=None, out_lo=None):
