@@ -7,6 +7,7 @@ eager/PyTorch fallback for the kernels.  ``python -m bbdm_b200.build`` (or
 from __future__ import annotations
 
 import ctypes as C
+import gc
 import os
 
 import torch
@@ -15,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BBDM_LIB selects another in-tree build of the same sources (A/B experiments, tools/); the product default is fixed
 LIB_PATH = os.environ.get("BBDM_LIB") or os.path.join(_HERE, "libbbdm_b200.so")
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 OBJ = {"grad": 0, "noise": 1, "ysubx": 2}
 RESAMPLE_NONE, RESAMPLE_UP2, RESAMPLE_DOWN2 = 0, 1, 2
 RES_NONE, RES_SAME, RES_UP2, RES_DOWN2 = 0, 1, 2, 3
@@ -84,7 +85,7 @@ class WinoInputArgs(C.Structure):
                 ("film_scale", C.c_void_p), ("film_shift", C.c_void_p), ("film_stride", C.c_int64),
                 ("silu", C.c_int),
                 ("v_hi", C.c_void_p), ("v_lo", C.c_void_p), ("raw_hi", C.c_void_p), ("raw_lo", C.c_void_p),
-                ("act_hi", C.c_void_p), ("act_lo", C.c_void_p)]
+                ("act_hi", C.c_void_p), ("act_lo", C.c_void_p), ("down2", C.c_int)]
 
 
 class WinoOutputArgs(C.Structure):
@@ -254,7 +255,13 @@ class CudaBackend:
 
     # -- memory ------------------------------------------------------------------------------
     def empty(self, shape, dtype, device):
-        return torch.empty(shape, dtype=dtype, device=device)
+        try:
+            return torch.empty(shape, dtype=dtype, device=device)
+        except torch.OutOfMemoryError:
+            # a model and its executor refer to each other, so the buffer pools of a dropped model go back to the
+            # allocator only when the cycle collector runs: run it, then try once more
+            gc.collect()
+            return torch.empty(shape, dtype=dtype, device=device)
 
     # -- bridge --------------------------------------------------------------------------------
     def q_sample(self, x0, y, noise, t, m_t, var_t, objective, xt_out, obj_out):
@@ -390,12 +397,14 @@ class CudaBackend:
 
     def wino_input(self, src1, src2, *, groups=32, mean=None, rstd=None, gamma=None, beta=None, film_scale=None,
                    film_shift=None, film_stride=0, silu=True, v_hi, v_lo, raw_hi=None, raw_lo=None, act_hi=None,
-                   act_lo=None, tile=4):
+                   act_lo=None, tile=4, down2=False):
+        """down2 (tile 6): transform the 2x2 average pool of the activated input (the conv runs on the H/2 x W/2
+        map)."""
         B, H, W, c1 = src1.shape
         a = WinoInputArgs(ptr(_req(src1)), c1, ptr(src2), 0 if src2 is None else src2.shape[3], B, H, W, groups,
                           ptr(mean), ptr(rstd), ptr(gamma), ptr(beta), ptr(film_scale), ptr(film_shift), film_stride,
                           int(silu), ptr(_req(v_hi, torch.float16)), ptr(_req(v_lo, torch.float16)),
-                          ptr(raw_hi), ptr(raw_lo), ptr(act_hi), ptr(act_lo))
+                          ptr(raw_hi), ptr(raw_lo), ptr(act_hi), ptr(act_lo), int(down2))
         check(self._wino("input", tile)(C.byref(a), stream()))
         LAUNCHES["n"] += 1
 

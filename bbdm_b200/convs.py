@@ -27,9 +27,21 @@ WINO_MIN_C = int(os.environ.get("BBDM_WINO_MIN_C", "256"))
 WINO_MIN_TILES = int(os.environ.get("BBDM_WINO_MIN_TILES", "512"))
 
 
-def wino_channels_ok(cin, cout, min_c):
-    """The channel half of the Winograd rule (the executors apply it when they pack the weight planes)."""
-    return cin % 64 == 0 and cout % 64 == 0 and min(cin, cout) >= min_c
+def wino_channels_ok(cin, cout, min_c, tile=4):
+    """The channel half of the Winograd rule (the executors apply it when they pack the weight planes).
+
+    F(6x6,3x3) (the UNet sampling executor on its large maps) also takes a conv with cin >= 256 and cout >= 128: it
+    issues about 0.2x the direct kernel's MACs and pays for them with the V / M round trip through HBM, which the
+    wide-input convs win.  Measured in isolation at the cfg2 shapes (B=16, tools/time_wino.py --f63-conv1, H100 80GB
+    HBM3 at 700 W; GroupNorm-SiLU operand pass + direct conv against the F(6,3) chain): 640 -> 128 at 256x256
+    10.8 -> 6.9 ms, 256 -> 128 at 256x256 3.8 -> 3.4 ms (both with the raw planes of the fused 1x1 skip).  128 -> 512 at
+    128x128 (1.6 -> 1.9 ms: the M round trip of 512 outputs outweighs the MACs 128 inputs save) and 128 -> 128 lose and
+    stay direct."""
+    if cin % 64 or cout % 64:
+        return False
+    if min(cin, cout) >= min_c:
+        return True
+    return tile == 6 and cin >= 256 and cout >= 128
 
 
 def wino_tile(H, W):
@@ -50,7 +62,8 @@ def winograd_ok(geometry, cin, cout, min_c, min_tiles, tile=4):
     only when the whole batch has min_tiles F(4,3) tiles' worth."""
     th, tw, tiles, ok = geometry
     px = tile * tile
-    return bool(ok and wino_channels_ok(cin, cout, min_c) and (th * tw * px >= 128 * 16 or tiles * px >= min_tiles * 16))
+    return bool(ok and wino_channels_ok(cin, cout, min_c, tile) and
+                (th * tw * px >= 128 * 16 or tiles * px >= min_tiles * 16))
 
 
 class FreshBuffers:
@@ -68,7 +81,7 @@ class FreshBuffers:
 
 
 def wino_conv(be, pool, geometry, src1, src2, *, cout, planes=None, weight=None, dgrad=False, bias=None,
-              residual=None, res_mode=cabi.RES_NONE, stats=False, tile=4, up2_phases=False, **transform):
+              residual=None, res_mode=cabi.RES_NONE, stats=False, tile=4, up2_phases=False, down2=False, **transform):
     """3x3 conv of cat(src1, src2) (NHWC fp32) on the Winograd path: input transform (``transform`` are the
     wino_input arguments: GroupNorm affine + FiLM + SiLU, or identity with silu=False; raw_* / act_* side outputs) ->
     (tile+2)^2 position GEMMs in one wgmma launch -> output transform (+ bias, + residual, + GroupNorm partial sums if
@@ -79,13 +92,20 @@ def wino_conv(be, pool, geometry, src1, src2, *, cout, planes=None, weight=None,
 
     up2_phases (tile 6, planes of WeightPacker.up_phase_winograd): nearest-2x upsample of the activated input, then the
     3x3 conv -- run on the input's own map as a 3x3 conv with 4*cout phase-major outputs, whose output transform
-    interleaves the phases into the [B, 2H, 2W, cout] result (bias [cout], no residual)."""
+    interleaves the phases into the [B, 2H, 2W, cout] result (bias [cout], no residual).
+
+    down2 (tile 6): the conv's input is the 2x2 average pool of the activated input; it runs on the H/2 x W/2 map, which
+    geometry describes."""
     B, H, W, c1 = src1.shape
     cin = c1 + (0 if src2 is None else src2.shape[3])
     th, _, mtot, _ = geometry
     npos = (tile + 2) ** 2
     tkw = {} if tile == 4 else dict(tile=tile)
     assert not up2_phases or (tile == 6 and planes is not None and residual is None)
+    assert not down2 or (tile == 6 and not up2_phases)
+    if down2:
+        H, W = H // 2, W // 2
+        transform["down2"] = True
     ncols = 4 * cout if up2_phases else cout            # output channels of the position GEMMs
     v_hi, v_lo = pool.get((npos, mtot, cin), torch.float16), pool.get((npos, mtot, cin), torch.float16)
     be.wino_input(src1, src2, v_hi=v_hi, v_lo=v_lo, **transform, **tkw)

@@ -118,7 +118,8 @@ __device__ __forceinline__ void split2_f16(float a, float b, uint32_t& hi, uint3
 struct WinoInParams {
   const float* src1; int c1;
   const float* src2; int c2;
-  int B, H, W, C, groups, cpg, th, tw;
+  int B, H, W, C, groups, cpg, th, tw;   // H x W: the conv's map
+  int sH, sW;                // the sources' map: H x W, or 2H(+1) x 2W(+1) for the 2x2-pooled form (down2)
   int64_t Mtot;              // rows of the V planes: B*th*tw tiles (F(6,3): padded to a multiple of 16, zero rows)
   const float* mean; const float* rstd; const float* gamma; const float* beta;
   const float* fscale; const float* fshift; int64_t fstride;
@@ -260,6 +261,10 @@ wino_input_kernel(const WinoInParams p) {
 // transforms, splits to fp16 hi/lo and stores (128 contiguous bytes per warp, position and plane).  F(6,3): thread
 // (tile, channel) does the same for its 8x8 tile (64 floats of state, not 128: the kernel stays spill-free at 2 CTAs
 // per SM), 64 contiguous bytes per warp, position and plane.
+// POOL (F(6,3), the down-ResBlock's conv1): the conv's input is the 2x2 average of the ACTIVATED 2H x 2W sources
+// (GroupNorm + SiLU, then the pool: the reference order).  Phase 2 reads the four source pixels of each patch pixel
+// itself, activates each and stores their average; nothing is staged by cp.async (a full-resolution patch would not
+// fit twice per CTA at 2 CTAs per SM).
 template <int T>
 struct WinoIn {
   static constexpr int N = T + 2;                    // input tile side
@@ -275,9 +280,10 @@ __device__ __forceinline__ void cp_async16(uint32_t saddr, const void* g) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(saddr), "l"(g) : "memory");
 }
 
-template <int T>
+template <int T, bool POOL>
 __global__ void __launch_bounds__(256, 2)
 wino_input_smem_kernel(const WinoInParams p) {
+  static_assert(!POOL || T == 6, "the pooled input form is F(6,3) only");
   using K = WinoIn<T>;
   constexpr int N = K::N, CC = K::CC, TX = K::TX, COLS = K::COLS;
   extern __shared__ __align__(16) float patch[];          // [2][N][COLS][CC]
@@ -326,16 +332,27 @@ wino_input_smem_kernel(const WinoInParams p) {
   const uint32_t patch_s = (uint32_t)__cvta_generic_to_shared(patch);
 
   auto stage = [&](int seg, int buf) {
-    const int x0 = T * TX * seg - 1;
-    int i = 0, j = pix0;                                  // pix0 < 16 <= COLS: row 0
-    for (int px = pix0; px < NPIX; px += 16, j += 16) {
-      if (j >= COLS) { j -= COLS; ++i; }
-      const int iy = y0 + i, ix = x0 + j;
-      if (iy >= 0 && iy < p.H && ix >= 0 && ix < p.W)
-        cp_async16(patch_s + (uint32_t)(((buf * NPIX + px) * CC + ch4 * 4) * 4),
-                   base + (((int64_t)b * p.H + iy) * p.W + ix) * cs + cc0 + ch4 * 4);
+    if constexpr (!POOL) {
+      const int x0 = T * TX * seg - 1;
+      int i = 0, j = pix0;                                // pix0 < 16 <= COLS: row 0
+      for (int px = pix0; px < NPIX; px += 16, j += 16) {
+        if (j >= COLS) { j -= COLS; ++i; }
+        const int iy = y0 + i, ix = x0 + j;
+        if (iy >= 0 && iy < p.H && ix >= 0 && ix < p.W)
+          cp_async16(patch_s + (uint32_t)(((buf * NPIX + px) * CC + ch4 * 4) * 4),
+                     base + (((int64_t)b * p.H + iy) * p.W + ix) * cs + cc0 + ch4 * 4);
+      }
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+  auto activate = [&](const float4 x) {
+    float4 a = make_float4(fmaf(x.x, sc[0], sh[0]), fmaf(x.y, sc[1], sh[1]), fmaf(x.z, sc[2], sh[2]),
+                           fmaf(x.w, sc[3], sh[3]));
+    if (p.silu) {
+      a.x = __fdividef(a.x, 1.0f + __expf(-a.x)); a.y = __fdividef(a.y, 1.0f + __expf(-a.y));
+      a.z = __fdividef(a.z, 1.0f + __expf(-a.z)); a.w = __fdividef(a.w, 1.0f + __expf(-a.w));
+    }
+    return a;
   };
 
   stage(0, 0);
@@ -357,7 +374,16 @@ wino_input_smem_kernel(const WinoInParams p) {
       const int iy = y0 + i, ix = x0 + j;
       float4* q = reinterpret_cast<float4*>(pb + px * CC + ch4 * 4);
       float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (iy >= 0 && iy < p.H && ix >= 0 && ix < p.W) {
+      if (POOL && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W) {
+        const float* s = base + (((int64_t)b * p.sH + 2 * iy) * p.sW + 2 * ix) * cs + cc0 + ch4 * 4;
+        const int64_t rs = (int64_t)p.sW * cs;
+        const float4 a0 = activate(__ldg(reinterpret_cast<const float4*>(s)));
+        const float4 a1 = activate(__ldg(reinterpret_cast<const float4*>(s + cs)));
+        const float4 a2 = activate(__ldg(reinterpret_cast<const float4*>(s + rs)));
+        const float4 a3 = activate(__ldg(reinterpret_cast<const float4*>(s + rs + cs)));
+        a = make_float4(0.25f * (((a0.x + a1.x) + a2.x) + a3.x), 0.25f * (((a0.y + a1.y) + a2.y) + a3.y),
+                        0.25f * (((a0.z + a1.z) + a2.z) + a3.z), 0.25f * (((a0.w + a1.w) + a2.w) + a3.w));
+      } else if (!POOL && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W) {
         const float4 x = *q;
         if (p.raw_hi && i >= 1 && i <= T && j >= 1 && j <= T * TX) {
           // pixels this segment owns: raw split-bf16 planes for the 1x1 skip conv
@@ -367,12 +393,7 @@ wino_input_smem_kernel(const WinoInParams p) {
           *reinterpret_cast<uint2*>(p.raw_hi + off) = h;
           *reinterpret_cast<uint2*>(p.raw_lo + off) = l;
         }
-        a.x = fmaf(x.x, sc[0], sh[0]); a.y = fmaf(x.y, sc[1], sh[1]);
-        a.z = fmaf(x.z, sc[2], sh[2]); a.w = fmaf(x.w, sc[3], sh[3]);
-        if (p.silu) {
-          a.x = __fdividef(a.x, 1.0f + __expf(-a.x)); a.y = __fdividef(a.y, 1.0f + __expf(-a.y));
-          a.z = __fdividef(a.z, 1.0f + __expf(-a.z)); a.w = __fdividef(a.w, 1.0f + __expf(-a.w));
-        }
+        a = activate(x);
         if (p.act_hi && i >= 1 && i <= T && j >= 1 && j <= T * TX) {
           // training: the activated tensor's split-bf16 planes are the weight-gradient GEMM's operand
           uint2 h, l;
@@ -784,6 +805,19 @@ int wino_geometry_t(int B, int H, int W, int* tiles_h, int* tiles_w, int64_t* ti
   return BBDM_OK;
 }
 
+template <int T, bool POOL>
+int launch_wino_input_smem(const WinoInParams& p, dim3 grid, void* stream) {
+  static DeviceOnce configured;
+  if (configured.need()) {
+    BBDM_CUDA_CHECK(cudaFuncSetAttribute(wino_input_smem_kernel<T, POOL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)WinoIn<T>::SMEM));
+    configured.mark();
+  }
+  wino_input_smem_kernel<T, POOL><<<grid, 256, WinoIn<T>::SMEM, (cudaStream_t)stream>>>(p);
+  BBDM_LAUNCH_CHECK();
+  return BBDM_OK;
+}
+
 template <int T>
 int wino_input_t(const BbdmWinoInputArgs* a, void* stream) {
   BBDM_REQUIRE(a && a->src1 && a->v_hi && a->v_lo, "wino_input: null args");
@@ -808,6 +842,12 @@ int wino_input_t(const BbdmWinoInputArgs* a, void* stream) {
   BBDM_REQUIRE((a->film_scale == nullptr) == (a->film_shift == nullptr), "wino_input: film scale/shift mismatch");
   BBDM_REQUIRE((a->raw_hi == nullptr) == (a->raw_lo == nullptr), "wino_input: raw hi/lo must come in pairs");
   p.cpg = p.C / p.groups;
+  p.sH = p.H; p.sW = p.W;
+  if (a->down2) {
+    BBDM_REQUIRE(T == 6 && !a->raw_hi && !a->act_hi && p.H >= 2 && p.W >= 2,
+                 "wino_input: down2 is an F(6,3) form without raw / act planes (H, W >= 2)");
+    p.H /= 2; p.W /= 2;
+  }
   wino_geometry_t<T>(p.B, p.H, p.W, &p.th, &p.tw, &p.Mtot, nullptr);
   p.mean = a->mean; p.rstd = a->rstd; p.gamma = a->gamma; p.beta = a->beta;
   p.fscale = a->film_scale; p.fshift = a->film_shift; p.fstride = a->film_stride;
@@ -830,14 +870,11 @@ int wino_input_t(const BbdmWinoInputArgs* a, void* stream) {
   static int vec = -1;
   if (vec < 0) { const char* e = getenv("BBDM_WINO_IN_VEC"); vec = e ? (atoi(e) == 2 ? 2 : 1) : 0; }
   if ((T == 6 || vec == 0) && p.c1 % CC == 0 && p.c2 % CC == 0) {
-    static DeviceOnce configured;
-    if (configured.need()) {
-      BBDM_CUDA_CHECK(cudaFuncSetAttribute(wino_input_smem_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)WinoIn<T>::SMEM));
-      configured.mark();
+    const dim3 grid((unsigned)ctas, p.C / CC);
+    if constexpr (T == 6) {
+      if (a->down2) return launch_wino_input_smem<T, true>(p, grid, stream);
     }
-    dim3 grid((unsigned)ctas, p.C / CC);
-    wino_input_smem_kernel<T><<<grid, 256, WinoIn<T>::SMEM, (cudaStream_t)stream>>>(p);
+    return launch_wino_input_smem<T, false>(p, grid, stream);
   } else if (T == 6) {
     BBDM_REQUIRE(false, "wino6_input: channel counts must be multiples of 64");
   } else if (smem_only) {

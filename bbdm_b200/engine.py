@@ -289,12 +289,15 @@ class KernelExecutor:
             h1, _, _ = self._conv(pool, e1, a_hi=a_hi, a_lo=a_lo, shape=(B, Hs, Ws), planes=(e1["up_hi"], e1["up_lo"]),
                                   taps=4, upsample2x=True, stats=True)
             pool.put(a_hi, a_lo)
-        elif umma1 and resample == cabi.RESAMPLE_NONE and not need_raw_f32 and bias1 is None \
-                and self._wino_ok(e1, B, H, W, c1):
-            # Winograd conv1; the raw split planes for a fused 1x1 skip come out of the same input pass
+        elif umma1 and not need_raw_f32 and bias1 is None and (
+                resample == cabi.RESAMPLE_NONE or (resample == cabi.RESAMPLE_DOWN2 and e1.get("u_tile") == 6
+                                                   and not fuse_skip)) and self._wino_ok(e1, B, H, W, c1):
+            # Winograd conv1; the raw split planes for a fused 1x1 skip come out of the same input pass.  A
+            # down-ResBlock's conv1 (F(6,3) only) takes the 2x2 pool of the activated input inside the input transform
             if fuse_skip:
                 r_hi, r_lo = pool.get(shp, torch.bfloat16), pool.get(shp, torch.bfloat16)
-            h1 = self._wino_conv(pool, e1, src1, src2, **gkw, raw_hi=r_hi, raw_lo=r_lo)
+            h1 = self._wino_conv(pool, e1, src1, src2, **gkw, raw_hi=r_hi, raw_lo=r_lo,
+                                 down2=resample == cabi.RESAMPLE_DOWN2)
             pool.put(mean, rstd)
         else:
             a_f32 = a_hi = a_lo = None
@@ -378,19 +381,21 @@ class KernelExecutor:
         return convs.winograd_ok(self._wino_geometry(B, H, W, tile), ent["cin"], ent["cout"], self.wino_min_c,
                                  self.wino_min_tiles, tile)
 
-    def _wino_ready(self, ent):
-        """Whether refresh_weights gives the packed conv ent Winograd planes."""
+    def _wino_ready(self, ent, tile=4):
+        """Whether refresh_weights gives the packed conv ent Winograd planes of that tile size."""
         return self.wino and "hi" in ent and ent["k"] == 3 and convs.wino_channels_ok(ent["cin"], ent["cout"],
-                                                                                     self.wino_min_c)
+                                                                                     self.wino_min_c, tile)
 
-    def _wino_conv(self, pool, ent, src1, src2, *, residual=None, res_mode=cabi.RES_NONE, **transform):
-        """GroupNorm-affine(+FiLM)+SiLU -> 3x3 conv (+bias, +residual, GN partial sums) of cat(src1, src2) on the
-        Winograd path with the entry's planes; transform: the wino_input arguments (groups, mean, rstd, ...)."""
+    def _wino_conv(self, pool, ent, src1, src2, *, residual=None, res_mode=cabi.RES_NONE, down2=False, **transform):
+        """GroupNorm-affine(+FiLM)+SiLU (-> 2x2 average pool if down2) -> 3x3 conv (+bias, +residual, GN partial sums)
+        of cat(src1, src2) on the Winograd path with the entry's planes; transform: the wino_input arguments (groups,
+        mean, rstd, ...)."""
         B, H, W, _ = src1.shape
+        f = 2 if down2 else 1
         tile = ent["u_tile"]
-        return convs.wino_conv(self.be, pool, self._wino_geometry(B, H, W, tile), src1, src2, cout=ent["cout"],
-                               planes=(ent["u_hi"], ent["u_lo"], ent.get("u_inv")), bias=ent["bias"],
-                               residual=residual, res_mode=res_mode, stats=True, tile=tile, **transform)
+        return convs.wino_conv(self.be, pool, self._wino_geometry(B, H // f, W // f, tile), src1, src2,
+                               cout=ent["cout"], planes=(ent["u_hi"], ent["u_lo"], ent.get("u_inv")), bias=ent["bias"],
+                               residual=residual, res_mode=res_mode, stats=True, tile=tile, down2=down2, **transform)
 
 
 class UNetEngine(KernelExecutor):
@@ -466,13 +471,14 @@ class UNetEngine(KernelExecutor):
         for name, m in u.named_modules():
             # Winograd planes for the stride-1 3x3 convs of the scale-shift ResBlocks: F(6x6,3x3) for the convs that
             # run on a large map at the UNet's image_size (convs.wino_tile), else F(4x4,3x3); a forward at another
-            # size runs the form that is packed
+            # size runs the form that is packed.  A down-ResBlock's conv1 only on F(6,3), whose input transform pools
+            # its input; an up-ResBlock's conv1 gets the phase planes below instead
             if isinstance(m, ResBlock) and m.use_scale_shift_norm:
                 hw = sizes[name]
                 tile = convs.wino_tile(hw, hw) if 6 in getattr(be, "wino_tiles", (4,)) else 4
-                for cname, conv, resampled in ((name + ".in_layers.2", m.in_layers[2], m.up or m.down),
-                                               (name + ".out_layers.3", m.out_layers[3], False)):
-                    if not resampled and self._wino_ready(w[cname]):
+                for cname, conv, direct in ((name + ".in_layers.2", m.in_layers[2], m.up or (m.down and tile != 6)),
+                                            (name + ".out_layers.3", m.out_layers[3], False)):
+                    if not direct and self._wino_ready(w[cname], tile):
                         packer.winograd(cname, conv.weight, tile)
         for name, m in u.named_modules():
             if isinstance(m, ResBlock) and m.up and m.channels % 64 == 0 and m.out_channels % 64 == 0:

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define BBDM_ABI_VERSION 3
+#define BBDM_ABI_VERSION 4
 
 enum {
   BBDM_OK = 0,
@@ -277,6 +277,7 @@ typedef struct {
   void* raw_hi; void* raw_lo;
   void* act_hi; void* act_lo;   /* optional: split-bf16 NHWC planes of the ACTIVATED tensor (training: operand of the
                                    weight-gradient GEMM, bbdm_conv_wgrad) */
+  int down2;                    /* F(6,3) only: see bbdm_wino6_input below */
 } BbdmWinoInputArgs;
 int bbdm_wino_input(const BbdmWinoInputArgs* a, void* stream);
 
@@ -317,7 +318,10 @@ int bbdm_wino_pack_weight(const float* w, int Cout, int Cin, int dgrad, void* u_
  *                tile by at most 225 (F(4,3): 100), so max|act| <= 291 is finite for every input; a V value
  *                that is not a finite fp16 number sets the device fault word to 0xC0000000 | C
  *                (bbdm_check_device_fault reports it).
- *   output       m [64][tiles_total][Cout]; stats_partial [B * tiles_h][Cout][2].
+ *                down2 != 0: the conv's input is the 2x2 average pool of the activated [B,H,W,C] sources (the
+ *                down-ResBlock's in_layers -> h_upd order: activate every pixel, then average), so the transform
+ *                and the geometry are those of the H/2 x W/2 map; no raw or act planes.
+ *   output      m [64][tiles_total][Cout]; stats_partial [B * tiles_h][Cout][2].
  *                up2_phases != 0: the output of a nearest-2x upsample followed by a 3x3 conv, run as one 3x3 conv on
  *                the H x W (low-res) map with 4*Cout outputs, phase-major: channel phase*Cout + co of m is output
  *                channel co at the pixels (2y+a, 2x+b) of out [B, 2H, 2W, Cout], phase = 2a + b.  bias [Cout];
