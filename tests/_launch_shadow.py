@@ -1,0 +1,802 @@
+"""TEST-ONLY: a shadow backend that checks every kernel launch of the UNet executor against an fp64 recomputation of
+that launch, from copies of the tensors the launch read.
+
+``Shadow`` wraps a backend (cabi.CudaBackend, or the CPU emulation to test the checker itself) the way the Recorder of
+tests/test_launch_trace_host.py wraps the emulation: every launching method is bound to its signature, the tensors it
+reads are cloned, the real launch runs, the device is synchronized and its fault word read, and then
+
+- every input that is not also an output must be bit-unchanged (an out-of-bounds write into a neighbouring pool buffer
+  that the launch reads shows here);
+- every output is compared with a float64 recomputation from the clones, on the tensors' own device.  The deviation is
+  taken per image: the max over images of max|got - want| / max|want| within the image, so one wrong image of a batch
+  cannot hide behind the others.
+
+The Winograd chains are paired by buffer identity (wino_input's V planes -> the position GEMMs' A operand, the GEMMs'
+output -> wino_output's M) and checked stage by stage and as a whole, against the fp64 conv of the fp64 activation with
+the module's fp32 weight; ``register_engine`` maps each cache entry's U planes to its module weight.
+
+Bounds are those of the single-kernel GPU tests, measured on an H100 with synthetic operands; each names its source.
+A launch whose output goes beyond its bound is a finding, not a bound to raise.
+"""
+import collections
+import inspect
+import math
+
+import torch
+import torch.nn.functional as F
+
+from oracle import bbdm_oracle as O
+from test_launch_trace_host import NOT_LAUNCHES
+
+F64 = torch.float64
+
+# what each launching method writes; a method not listed is an error (a new launch kind must get a reference)
+OUTPUTS = {
+    "nchw_to_nhwc_cat": ("out",), "nhwc_to_nchw": ("out",), "gather_rows": ("out",), "linear": ("out",),
+    "gn_stats": ("mean", "rstd", "workspace"), "gn_finalize_partials": ("mean", "rstd"),
+    "prep": ("act_f32", "act_hi", "act_lo", "raw_f32", "raw_hi", "raw_lo"),
+    "pack_weight_split": ("hi", "lo"), "pack_weight_split_taps": ("hi", "lo"), "pack_weight_f32": ("out",),
+    "wino_pack_weight": ("u_hi", "u_lo", "inv_wscale"),
+    "conv_umma": ("out", "out_hi", "out_lo", "stats_partial"), "conv_direct": ("out",),
+    "conv_stem": ("out", "stats_partial"),
+    "wino_input": ("v_hi", "v_lo", "raw_hi", "raw_lo", "act_hi", "act_lo"), "wino_output": ("out", "stats_partial"),
+    "attention": ("out_f32", "out_hi", "out_lo"), "attention_split": ("out_f32", "out_hi", "out_lo"),
+    "attention_tc": ("out_f32", "out_hi", "out_lo"),
+}
+
+# a split-bf16 pair carries 16 bits: 2^-17 = 7.6e-6 of the element (test_gpu_winograd.py::test_wino_input_production_layouts)
+PAIR = 8e-6
+BOUNDS = {
+    "exact": 0.0,
+    "linear": 2e-6,             # test_gpu_kernels.py::test_gather_and_linear
+    "gn_stats": 2e-6,           # test_gpu_kernels.py::test_gn_stats
+    "gn_finalize": 3e-6,        # test_gpu_kernels.py::test_conv_umma_fused_groupnorm_statistics
+    "prep_act": 5e-6,           # test_gpu_kernels.py::test_prep_operand (act_f32)
+    "prep_act_planes": 5e-6 + PAIR,
+    "prep_raw": 1e-6,           # test_gpu_kernels.py::test_prep_operand (raw_f32)
+    "prep_raw_planes": 1e-6 + PAIR,
+    "conv_direct": 3e-6,        # test_gpu_kernels.py::test_conv_direct
+    "conv_stem": 2e-6,          # test_gpu_kernels.py::test_conv_stem_equals_conv_direct_and_fuses_gn_partials
+    "conv_umma": 6e-6,          # test_gpu_kernels.py::test_conv_umma (fp64 evaluation of the same split products)
+    "conv_umma_planes": 6e-6 + PAIR,
+    "stats": 1e-5,              # test_gpu_winograd6.py::test_wino6_chain_vs_fp64_conv (GroupNorm partial sums)
+    "attention": 2e-5,          # test_gpu_kernels.py::test_attention_tc / test_attention_split / test_attention
+    "attention_planes": 2e-5 + PAIR,
+    "wino_v6": 1e-6,            # test_gpu_winograd6.py::test_wino6_input_transform_exact_positions
+    "wino_v4": 2e-6,            # test_gpu_winograd.py::test_wino_input_production_layouts
+    "wino_act_planes": PAIR,    # test_gpu_winograd.py::test_wino_input_production_layouts (act planes)
+    "wino_m": 3e-6,             # test_gpu_winograd.py::test_wino_conv_chain_vs_fp64_conv (position GEMMs)
+    # tools/host_check_wino6_output.cu (run by test_wino6_output_host.py) holds the output transform to 2e-6 of max|Y|
+    # with random M.  In the model M is far larger than Y (the transform cancels), and the fp32 evaluation's error
+    # scales with |A^T| |M| |A|: measured up to 3.7e-6 on an H100 80GB HBM3 (cfg2 at B = 16 and cfg4 at B = 64, the
+    # 64x64 F(6,3) wide-input conv1s), while the same launches stay within the chain bound against the independent
+    # fp64 conv (1.84e-5 and 1.34e-5).
+    "wino_y": 5e-6,
+    "chain6": 2e-5,             # test_gpu_winograd6.py CHAIN_BOUND
+    "chain4": 1.6e-5,           # test_gpu_winograd.py CHAIN_BOUND_BIASED
+    "pack_wino6": 1e-6,         # test_gpu_winograd6.py::test_wino6_pack_weight
+    "pack_wino4": 2e-7,         # test_gpu_winograd.py::test_wino_pack_weight
+    "up_phase": 2.0 ** -16,     # test_gpu_kernels.py::test_conv_umma_fused_upsample: the taps are summed in fp32, then split
+}
+
+# Winograd matrices, interpolation points 0, +-1, +-2 (F(4,3)) and 0, +-1, +-2, +-1/2 (F(6,3))
+BT = {4: [[4, 0, -5, 0, 1, 0], [0, -4, -4, 1, 1, 0], [0, 4, -4, -1, 1, 0], [0, -2, -1, 2, 1, 0], [0, 2, -1, -2, 1, 0],
+          [0, 4, 0, -5, 0, 1]],
+      6: [[1, 0, -21 / 4, 0, 21 / 4, 0, -1, 0], [0, 1, 1, -17 / 4, -17 / 4, 1, 1, 0], [0, -1, 1, 17 / 4, -17 / 4, -1, 1, 0],
+          [0, 1 / 2, 1 / 4, -5 / 2, -5 / 4, 2, 1, 0], [0, -1 / 2, 1 / 4, 5 / 2, -5 / 4, -2, 1, 0],
+          [0, 2, 4, -5 / 2, -5, 1 / 2, 1, 0], [0, -2, 4, 5 / 2, -5, -1 / 2, 1, 0], [0, -1, 0, 21 / 4, 0, -21 / 4, 0, 1]]}
+G = {4: [[1 / 4, 0, 0], [-1 / 6, -1 / 6, -1 / 6], [-1 / 6, 1 / 6, -1 / 6], [1 / 24, 1 / 12, 1 / 6],
+         [1 / 24, -1 / 12, 1 / 6], [0, 0, 1]],
+     6: [[1, 0, 0], [-2 / 9, -2 / 9, -2 / 9], [-2 / 9, 2 / 9, -2 / 9], [1 / 90, 1 / 45, 2 / 45], [1 / 90, -1 / 45, 2 / 45],
+         [32 / 45, 16 / 45, 8 / 45], [32 / 45, -16 / 45, 8 / 45], [0, 0, 1]]}
+AT = {4: [[1, 1, 1, 1, 1, 0], [0, 1, -1, 2, -2, 0], [0, 1, 1, 4, 4, 0], [0, 1, -1, 8, -8, 1]],
+      6: [[1, 1, 1, 1, 1, 1, 1, 0], [0, 1, -1, 2, -2, 1 / 2, -1 / 2, 0], [0, 1, 1, 4, 4, 1 / 4, 1 / 4, 0],
+          [0, 1, -1, 8, -8, 1 / 8, -1 / 8, 0], [0, 1, 1, 16, 16, 1 / 16, 1 / 16, 0],
+          [0, 1, -1, 32, -32, 1 / 32, -1 / 32, 1]]}
+
+
+def _mat(table, tile, dev):
+    return torch.tensor(table[tile], dtype=F64, device=dev)
+
+
+# ------------------------------------------------------------------------------------------------ metrics
+def image_devs(got, want):
+    """Per image (dim 0): max|got - want| / max|want|; NaN counts as infinitely wrong."""
+    n = got.shape[0]
+    g, w = got.reshape(n, -1).to(F64), want.reshape(n, -1).to(F64)
+    d = (g - w).abs().amax(1) / w.abs().amax(1).clamp_min(1e-30)
+    return torch.nan_to_num(d, nan=math.inf)
+
+
+def image_equal(got, want):
+    """Per image: 0 where got is bit-identical to want, else inf."""
+    n = got.shape[0]
+    same = (got.reshape(n, -1) == want.reshape(n, -1)).all(1)
+    return torch.where(same, 0.0, math.inf).to(F64)
+
+
+def _words(t):
+    b = t.contiguous().view(-1).view(torch.uint8)
+    return b.view(torch.int32) if b.numel() % 4 == 0 else b
+
+
+def bits_equal(a, b):
+    if a.shape != b.shape:
+        return False
+    wa, wb = _words(a), _words(b)
+    step = 1 << 26                     # no full-size temporaries next to the executor's multi-GB buffers
+    return all(torch.equal(wa[i:i + step], wb[i:i + step]) for i in range(0, wa.numel(), step))
+
+
+# inputs of at least this size (the F(6,3) V planes and wide concat inputs at 256x256, batch 16) are not copied: two
+# checksums of their bytes, taken before and after the launch, stand in for the copy, and the references read them in
+# place
+BIG = 1 << 30
+
+
+def fingerprint(t):
+    """(sum of the 32-bit words, position-weighted sum) of t's bytes, chunked."""
+    w = _words(t)
+    s1 = s2 = 0
+    step = 1 << 26
+    for i in range(0, w.numel(), step):
+        x = w[i:i + step].to(torch.int64)
+        s1 += int(x.sum())
+        s2 += int((x * (torch.arange(x.numel(), device=x.device) % 65521 + i % 65521 + 1)).sum())
+    return s1, s2
+
+
+def split_bf16(x):
+    """x (fp32) -> (hi, lo) bf16 with hi = bf16(x), lo = bf16(x - hi)."""
+    h = x.to(torch.bfloat16)
+    return h, (x - h.float()).to(torch.bfloat16)
+
+
+def pair_well_formed(hi, lo):
+    """Per image: 0 where hi is bf16(hi + lo) (a split pair, not two arbitrary halves), else inf."""
+    v = hi.float() + lo.float()
+    r = v.to(torch.bfloat16).float()
+    ok = (r == hi.float()) | ((r - hi.float()).abs() == 2 * lo.float().abs())
+    n = hi.shape[0]
+    return torch.where(ok.reshape(n, -1).all(1), 0.0, math.inf).to(F64)
+
+
+def planes(hi, lo):
+    return hi.to(F64) + lo.to(F64)
+
+
+def chunks(n, per_item_bytes, dev):
+    """Slices of range(n) whose fp64 working set stays under a few GB (references must not exhaust the device)."""
+    limit = (2 << 30) if torch.device(dev).type == "cuda" else (1 << 30)
+    step = max(1, int(limit // max(1, per_item_bytes)))
+    for b0 in range(0, n, step):
+        yield slice(b0, min(n, b0 + step))
+
+
+# ------------------------------------------------------------------------------------------------ fp64 operations
+def tap_conv(ap, taps, H, W):
+    """sum over (dy, dx, w [Cout, C]) of ap[:, dy:dy+H, dx:dx+W] @ w^T; ap [n, Hp, Wp, C] fp64 -> [n, H, W, Cout]."""
+    n, C = ap.shape[0], ap.shape[3]
+    out = None
+    for dy, dx, w in taps:
+        t = ap[:, dy:dy + H, dx:dx + W].reshape(n * H * W, C) @ w.t()
+        out = t if out is None else out.add_(t)
+    return out.view(n, H, W, -1)
+
+
+def conv3x3(a, w):
+    """'same' 3x3 conv of NHWC a (fp64) with OIHW w (fp64)."""
+    n, H, W, _ = a.shape
+    ap = F.pad(a, (0, 0, 1, 1, 1, 1))
+    return tap_conv(ap, [(ky, kx, w[:, :, ky, kx]) for ky in range(3) for kx in range(3)], H, W)
+
+
+def up2(a):
+    return a.repeat_interleave(2, 1).repeat_interleave(2, 2)
+
+
+def pool2(a):
+    n, H, W, C = a.shape
+    return a[:, :H // 2 * 2, :W // 2 * 2].reshape(n, H // 2, 2, W // 2, 2, C).mean((2, 4))
+
+
+def add_residual(o, res, mode):
+    """o [n, Ho, Wo, C] fp64 + the residual of the C ABI's res_mode (1 same, 2 nearest-up of half size, 3 2x2 average
+    of double size)."""
+    if mode == 0 or res is None:
+        return o
+    r = res.to(F64)
+    return o + {1: lambda: r, 2: lambda: up2(r), 3: lambda: pool2(r)}[mode]()
+
+
+def gn_act(x, a, sl):
+    """The prep / wino_input activation of images sl in fp64: GroupNorm affine (+FiLM) (+SiLU), or x itself without
+    statistics.  a: the launch's cloned arguments."""
+    xb = x[sl].to(F64)
+    if a.get("mean") is None:
+        return xb
+    f = lambda t: None if t is None else t[sl].to(F64)
+    return O.op_gn_act(xb, f(a["mean"]), f(a["rstd"]), a["gamma"].to(F64), a["beta"].to(F64), f(a.get("film_scale")),
+                       f(a.get("film_shift")), bool(a.get("silu", True)), 0)
+
+
+def cat(a, b):
+    return a if b is None else torch.cat([a, b], 3)
+
+
+def up_phase_reference(w):
+    """fp64 phase taps [16, Cout, Cin] of nearest-2x + the 3x3 conv w, from the definition: output pixel 2y+a reads
+    upsampled row 2y+a+ky-1, i.e. source row y + (a+ky-1)//2, which is tap r = (a+ky-1)//2 + 1 - a of phase a."""
+    w = w.to(F64)
+    out = torch.zeros(16, w.shape[0], w.shape[1], dtype=F64, device=w.device)
+    for a in range(2):
+        for b in range(2):
+            for ky in range(3):
+                for kx in range(3):
+                    r, c = (a + ky - 1) // 2 + 1 - a, (b + kx - 1) // 2 + 1 - b
+                    out[(2 * a + b) * 4 + 2 * r + c] += w[:, :, ky, kx]
+    return out
+
+
+def attention_ref(qkv, heads, order, sl_img):
+    """fp64 softmax attention of images sl_img of qkv [B, T, 3C] (fp64), head by head -> [n, T, C]."""
+    B, T, C3 = qkv.shape
+    C = C3 // 3
+    d = C // heads
+    out = torch.empty(qkv[sl_img].shape[0], T, C, dtype=F64, device=qkv.device)
+    for i, b in enumerate(range(*sl_img.indices(B))):
+        for h in range(heads):
+            if order:      # new order: q | k | v, each heads x d
+                q, k, v = (qkv[b, :, j * C + h * d:j * C + (h + 1) * d] for j in range(3))
+            else:          # legacy order: per head q, k, v of d channels each
+                q, k, v = (qkv[b, :, h * 3 * d + j * d:h * 3 * d + (j + 1) * d] for j in range(3))
+            s = torch.softmax((q @ k.t()) / math.sqrt(d), dim=-1)
+            out[i, :, h * d:(h + 1) * d] = s @ v
+    return out
+
+
+# ------------------------------------------------------------------------------------------------ the shadow
+Check = collections.namedtuple("Check", "launch method form what dev bound shapes")
+
+
+class Shadow:
+    def __init__(self, be, bounds=None):
+        """bounds: entries of BOUNDS to replace (the CPU emulation's chain)."""
+        self.be = be
+        self.bounds = dict(BOUNDS, **(bounds or {}))
+        self.checks, self.launches = [], []
+        self.mutate = {}                  # launch index -> fn(bound arguments): perturbs an output after the launch
+        self._wino_in, self._wino_m = {}, {}
+        self._weights = {}                # U planes' data_ptr -> (module weight [Cout, Cin, 3, 3], up2_phases, name)
+
+    # -- bookkeeping -------------------------------------------------------------------------------------------
+    def register_engine(self, eng):
+        """Map every Winograd cache entry's U planes to the module weight they were packed from (plain convs, tile 4 and
+        6, and the phase-stacked '#up6' entries of the up-ResBlock conv1s), and check the up-phase tap stacks against the
+        module weights."""
+        for name, ent in eng._w.items():
+            if not isinstance(ent, dict):
+                continue
+            mod = name[:-len("#up6")] if name.endswith("#up6") else name
+            if "u_hi" in ent:
+                w = eng.unet.get_submodule(mod).weight.detach()
+                self._weights[ent["u_hi"].data_ptr()] = (w, name.endswith("#up6"), name)
+            if "up_hi" in ent:
+                w = eng.unet.get_submodule(mod).weight.detach()
+                d = image_devs(planes(ent["up_hi"], ent["up_lo"])[None], up_phase_reference(w)[None])
+                self._record(-1, "pack_weight_split_taps", "up-phase stack", "phase taps vs module weight", d,
+                             self.bounds["up_phase"], [tuple(ent["up_hi"].shape)])
+
+    def _record(self, idx, method, form, what, devs, bound, shapes):
+        dev = float(devs.max()) if isinstance(devs, torch.Tensor) and devs.numel() else float(devs)
+        self.checks.append(Check(idx, method, form, what, dev, bound, shapes))
+
+    def failures(self):
+        return [c for c in self.checks if not c.dev <= c.bound]
+
+    def flagged_launches(self):
+        return sorted({c.launch for c in self.failures()})
+
+    def families(self):
+        """{(method, what): (checks, worst deviation, bound)}"""
+        fam = {}
+        for c in self.checks:
+            k = (c.method, c.what)
+            n, worst, _ = fam.get(k, (0, 0.0, c.bound))
+            fam[k] = (n + 1, max(worst, c.dev), c.bound)
+        return fam
+
+    def table(self, title):
+        lines = [f"{title}: {len(self.launches)} launches, {len(self.checks)} checks",
+                 "  launches per method: " + ", ".join(f"{m} {n}" for m, n in
+                                                       sorted(collections.Counter(m for m, _ in self.launches).items()))]
+        for (m, what), (n, worst, bound) in sorted(self.families().items()):
+            lines.append(f"  {m:22s} {what:34s} {n:5d}  worst {worst:.2e}  bound {bound:.1e}")
+        return "\n".join(lines)
+
+    def forms(self):
+        return collections.Counter(self.launches)
+
+    # -- the wrapper -------------------------------------------------------------------------------------------
+    def __getattr__(self, name):
+        attr = getattr(self.be, name)
+        if name in NOT_LAUNCHES or name == "check_fault" or not callable(attr):
+            return attr
+        if name not in OUTPUTS:
+            raise NotImplementedError(f"no fp64 reference for launch {name}")
+        sig = inspect.signature(attr)
+
+        def launch(*args, **kwargs):
+            bound = sig.bind(*args, **kwargs)
+            bound.apply_defaults()
+            a = dict(bound.arguments)
+            outs = {k for k in OUTPUTS[name] if isinstance(a.get(k), torch.Tensor)}
+            out_ptrs = {a[k].untyped_storage().data_ptr() for k in outs}
+            ins = {k: v for k, v in a.items() if isinstance(v, torch.Tensor) and k not in outs}
+            big = {k for k, v in ins.items() if v.numel() * v.element_size() >= BIG}
+            clones = {k: v.clone() for k, v in ins.items() if k not in big}
+            prints = {k: fingerprint(ins[k]) for k in big}
+            pre = {k: a[k].clone() for k in outs} if name == "pack_weight_split" else {}
+            r = attr(*args, **kwargs)
+            dev = next(iter(ins.values())).device
+            if dev.type == "cuda":
+                torch.cuda.synchronize(dev)
+            self.be.check_fault()
+            idx = len(self.launches)
+            if idx in self.mutate:
+                self.mutate[idx](a)
+            form = self._form(name, a)
+            self.launches.append((name, form))
+            shapes = [tuple(v.shape) for v in a.values() if isinstance(v, torch.Tensor)]
+            for k, v in ins.items():
+                if v.untyped_storage().data_ptr() not in out_ptrs:
+                    same = fingerprint(v) == prints[k] if k in big else bits_equal(v, clones[k])
+                    self._record(idx, name, form, "inputs unchanged", 0.0 if same else math.inf, 0.0,
+                                 [(k, tuple(v.shape))])
+            c = dict(a, **clones)            # the launch's arguments, inputs replaced by their clones
+            c["_prints"] = prints
+            getattr(self, "_ref_" + name)(idx, form, shapes, c, a, pre)
+            del c, clones
+            if dev.type == "cuda":
+                torch.cuda.empty_cache()     # the references' multi-GB temporaries must not fragment the executor's pool
+            return r
+        return launch
+
+    @staticmethod
+    def _form(name, a):
+        f = []
+        if name == "conv_umma":
+            if a["weights_per_image"]:
+                return "position GEMMs"
+            f.append(f"taps {a['taps']}")
+            f += [t for t, on in (("upsample2x", a["upsample2x"]), ("fused 1x1", a["Cin2"]),
+                                  ("NCHW head", a["out_nchw_channels"]), ("split out", a["out_hi"] is not None),
+                                  ("stats", a["stats_partial"] is not None)) if on]
+            if a["res_mode"]:
+                f.append(f"res {a['res_mode']}")
+        elif name in ("wino_input", "wino_output", "wino_pack_weight"):
+            f.append(f"F({a.get('tile', 4)},3)")
+            if name == "wino_input":
+                f += [t for t, on in (("two-source", a["src2"] is not None), ("raw planes", a["raw_hi"] is not None),
+                                      ("act planes", a["act_hi"] is not None), ("down2", a.get("down2")),
+                                      ("identity", a["mean"] is None)) if on]
+            elif name == "wino_output":
+                if a.get("up2_phases"):
+                    f.append("up2_phases")
+                if a["res_mode"]:
+                    f.append(f"res {a['res_mode']}")
+        elif name == "prep":
+            f.append("gn" if a["mean"] is not None else "raw")
+            f += [t for t, on in (("two-source", a["src2"] is not None), ("film", a["film_scale"] is not None),
+                                  (f"resample {a['resample']}", a["resample"])) if on]
+        return " ".join(f)
+
+    # -- references: layout / dense ----------------------------------------------------------------------------
+    def _ref_nchw_to_nhwc_cat(self, idx, form, shapes, c, a, pre):
+        want = torch.cat([c["x"], c["ctx"]], 1) if c["ctx"] is not None else c["x"]
+        self._record(idx, "nchw_to_nhwc_cat", form, "copy", image_equal(a["out"], want.permute(0, 2, 3, 1)),
+                     0.0, shapes)
+
+    def _ref_nhwc_to_nchw(self, idx, form, shapes, c, a, pre):
+        self._record(idx, "nhwc_to_nchw", form, "copy", image_equal(a["out"], c["src"].permute(0, 3, 1, 2)), 0.0,
+                     shapes)
+
+    def _ref_gather_rows(self, idx, form, shapes, c, a, pre):
+        self._record(idx, "gather_rows", form, "copy", image_equal(a["out"], c["table"][c["idx"]]), 0.0, shapes)
+
+    def _ref_linear(self, idx, form, shapes, c, a, pre):
+        z = c["x"].to(F64)
+        z = F.silu(z) if c["act_in"] else z
+        z = z @ c["w"].to(F64).t() + (0 if c["bias"] is None else c["bias"].to(F64))
+        z = F.silu(z) if c["act_out"] else z
+        self._record(idx, "linear", form, "out", image_devs(a["out"], z), self.bounds["linear"], shapes)
+
+    # -- group norm / prep -------------------------------------------------------------------------------------
+    def _check_stats(self, idx, method, form, shapes, mean, rstd, m_want, r_want, bound):
+        """mean in units of the group's standard deviation (what (x - mean) * rstd sees), rstd relative; per image."""
+        dm = ((mean.to(F64) - m_want).abs() * r_want).amax(1)
+        self._record(idx, method, form, "mean", torch.nan_to_num(dm, nan=math.inf), bound, shapes)
+        self._record(idx, method, form, "rstd", image_devs(rstd, r_want), bound, shapes)
+
+    @staticmethod
+    def _moments(s, sq, n, eps):
+        m = s / n
+        return m, 1.0 / torch.sqrt((sq / n - m * m).clamp_min(0) + eps)
+
+    def _ref_gn_stats(self, idx, form, shapes, c, a, pre):
+        x = cat(c["src1"], c["src2"])
+        B, H, W, C = x.shape
+        g = c["groups"]
+        ms, rs = [], []
+        for sl in chunks(B, H * W * C * 8, x.device):
+            xg = x[sl].to(F64).reshape(-1, H * W, g, C // g)
+            ms.append(xg.mean((1, 3)))
+            rs.append(1.0 / torch.sqrt(xg.var((1, 3), unbiased=False) + c["eps"]))
+        self._check_stats(idx, "gn_stats", form, shapes, a["mean"], a["rstd"], torch.cat(ms), torch.cat(rs),
+                          self.bounds["gn_stats"])
+
+    def _ref_gn_finalize_partials(self, idx, form, shapes, c, a, pre):
+        B, g = c["B"], c["groups"]
+        s = [c["part1"].to(F64).view(B, c["rows1"], -1, 2).sum(1)]
+        if c["part2"] is not None:
+            s.append(c["part2"].to(F64).view(B, c["rows2"], -1, 2).sum(1))
+        s = torch.cat(s, 1)
+        C = s.shape[1]
+        sg = s.view(B, g, C // g, 2).sum(2)
+        m, r = self._moments(sg[..., 0], sg[..., 1], c["hw"] * (C // g), c["eps"])
+        self._check_stats(idx, "gn_finalize_partials", form, shapes, a["mean"], a["rstd"], m, r,
+                          self.bounds["gn_finalize"])
+
+    def _ref_prep(self, idx, form, shapes, c, a, pre):
+        x = cat(c["src1"], c["src2"])
+        B, H, W, C = x.shape
+        res = c["resample"]
+        dv = collections.defaultdict(list)
+        for sl in chunks(B, H * W * C * 8 * 8, x.device):
+            if c["mean"] is not None:
+                act = O.op_resample(gn_act(x, c, sl), res)
+                if a["act_f32"] is not None:
+                    dv["act_f32"].append(image_devs(a["act_f32"][sl], act))
+                if a["act_hi"] is not None:
+                    dv["act planes"].append(image_devs(planes(a["act_hi"][sl], a["act_lo"][sl]), act))
+                    dv["act planes split"].append(self._split_of(a["act_hi"][sl], a["act_lo"][sl], a["act_f32"], sl))
+            if a["raw_f32"] is not None or a["raw_hi"] is not None:
+                raw = O.op_resample(x[sl].to(F64), res)
+                if a["raw_f32"] is not None:
+                    dv["raw_f32"].append(image_devs(a["raw_f32"][sl], raw))
+                if a["raw_hi"] is not None:
+                    dv["raw planes"].append(image_devs(planes(a["raw_hi"][sl], a["raw_lo"][sl]), raw))
+                    dv["raw planes split"].append(self._split_of(a["raw_hi"][sl], a["raw_lo"][sl], a["raw_f32"], sl))
+        bound = {"act_f32": self.bounds["prep_act"], "act planes": self.bounds["prep_act_planes"], "raw_f32": self.bounds["prep_raw"],
+                 "raw planes": self.bounds["prep_raw_planes"]}
+        for what, devs in dv.items():
+            self._record(idx, "prep", form, what, torch.cat(devs), bound.get(what, 0.0), shapes)
+
+    @staticmethod
+    def _split_of(hi, lo, f32, sl):
+        """The planes are bf16(v), bf16(v - hi) of the launch's own fp32 output v where it writes one, else a well-formed
+        pair."""
+        if f32 is None:
+            return pair_well_formed(hi, lo)
+        h, l = split_bf16(f32[sl])
+        return torch.maximum(image_equal(hi, h), image_equal(lo, l))
+
+    # -- weight packing ----------------------------------------------------------------------------------------
+    def _ref_pack_weight_split(self, idx, form, shapes, c, a, pre):
+        w = c["w"]
+        while w.dim() < 4:
+            w = w.unsqueeze(-1)
+        cout, cin, k = w.shape[0], w.shape[1], w.shape[2]
+        h, l = split_bf16(w.permute(2, 3, 0, 1).reshape(k * k, cout, cin).contiguous())
+        want_hi, want_lo = pre["hi"].clone(), pre["lo"].clone()       # padding rows beyond Cout: left as they were
+        want_hi[:, :cout], want_lo[:, :cout] = h, l
+        ok = bits_equal(a["hi"], want_hi) and bits_equal(a["lo"], want_lo)
+        self._record(idx, "pack_weight_split", form, "split planes", 0.0 if ok else math.inf, 0.0, shapes)
+
+    def _ref_pack_weight_split_taps(self, idx, form, shapes, c, a, pre):
+        h, l = split_bf16(c["w"].permute(2, 0, 1).contiguous())
+        ok = bits_equal(a["hi"], h) and bits_equal(a["lo"], l)
+        self._record(idx, "pack_weight_split_taps", form, "split planes", 0.0 if ok else math.inf, 0.0, shapes)
+
+    def _ref_pack_weight_f32(self, idx, form, shapes, c, a, pre):
+        w = c["w"]
+        while w.dim() < 4:
+            w = w.unsqueeze(-1)
+        k = w.shape[2]
+        ok = bits_equal(a["out"], w.permute(2, 3, 1, 0).reshape(k * k, w.shape[1], w.shape[0]).contiguous())
+        self._record(idx, "pack_weight_f32", form, "fp32 planes", 0.0 if ok else math.inf, 0.0, shapes)
+
+    def _ref_wino_pack_weight(self, idx, form, shapes, c, a, pre):
+        t = c.get("tile", 4)
+        w = c["w"].to(F64)
+        if c["dgrad"]:
+            w = w.flip(2, 3).transpose(0, 1)
+        s = 256.0
+        if a["inv_wscale"] is not None:
+            inv = float(a["inv_wscale"].item())
+            pow2 = inv > 0 and math.frexp(inv)[0] == 0.5
+            self._record(idx, "wino_pack_weight", form, "scale is a power of two", 0.0 if pow2 else math.inf, 0.0,
+                         shapes)
+            s = 1.0 / inv
+        g = _mat(G, t, w.device)
+        U = torch.einsum("ij,kcjl,ml->imkc", g, w, g).reshape(a["u_hi"].shape) * s
+        self._record(idx, "wino_pack_weight", form, f"U planes F({t},3)", image_devs(planes(a["u_hi"], a["u_lo"])[None],
+                                                                                   U[None]),
+                     self.bounds[f"pack_wino{t}"], shapes)
+
+    # -- convolutions ------------------------------------------------------------------------------------------
+    def _stats_check(self, idx, method, form, shapes, out, part, B):
+        """GroupNorm partial sums: the rows of each image summed against the fp64 sums of the launch's own output (the
+        consumer, gn_finalize_partials, reads only these per-image sums)."""
+        rows = part.shape[0] // B
+        got = part.to(F64).view(B, rows, -1, 2).sum(1)
+        devs = []
+        for sl in chunks(B, out[0].numel() * 8 * 2, out.device):
+            o = out[sl].to(F64).reshape(out[sl].shape[0], -1, out.shape[-1])
+            want = torch.stack([o.sum(1), (o * o).sum(1)], -1)
+            g = got[sl]
+            devs.append(torch.maximum(image_devs(g[..., 0], want[..., 0]), image_devs(g[..., 1], want[..., 1])))
+        self._record(idx, method, form, "GroupNorm partial sums", torch.cat(devs), self.bounds["stats"], shapes)
+
+    def _ref_conv_umma(self, idx, form, shapes, c, a, pre):
+        if c["weights_per_image"]:
+            return self._ref_position_gemms(idx, form, shapes, c, a)
+        B, H, W, Cin, Cout, taps = c["B"], c["H"], c["W"], c["Cin"], c["Cout"], c["taps"]
+        f = 2 if c["upsample2x"] else 1
+        Ho, Wo = f * H, f * W
+        wh, wl = c["w_hi"].to(F64), c["w_lo"].to(F64)
+        if c["upsample2x"]:
+            # 4 output phases x 2x2 taps on the low-res operand: phase (pa, pb), tap (r, s) reads source row y + r - 1 + pa
+            assert taps == 4
+            tap_of = lambda w: [[(r + pa, s + pb, w[(2 * pa + pb) * 4 + 2 * r + s]) for r in range(2) for s in range(2)]
+                                for pa in range(2) for pb in range(2)]
+        elif taps == 9:
+            tap_of = lambda w: [[(ky, kx, w[3 * ky + kx]) for ky in range(3) for kx in range(3)]]
+        elif taps == 4:     # 2x2 window at rows / columns 0..1, zero padding bottom / right
+            tap_of = lambda w: [[(1 + r, 1 + s, w[2 * r + s]) for r in range(2) for s in range(2)]]
+        else:
+            assert taps == 1
+            tap_of = lambda w: [[(1, 1, w[0])]]
+        passes = c["passes"]
+        res = c["residual"]
+        if res is not None:
+            rs = {1: (Ho, Wo), 2: (Ho // 2, Wo // 2), 3: (2 * Ho, 2 * Wo)}[c["res_mode"]]
+            res = res.reshape(B, rs[0], rs[1], Cout)
+        a_hi, a_lo = c["a_hi"].reshape(B, H, W, Cin), c["a_lo"].reshape(B, H, W, Cin)
+        dv = collections.defaultdict(list)
+        nchw = c["out_nchw_channels"]
+        for sl in chunks(B, (H + 2) * (W + 2) * Cin * 8 * 4 + Ho * Wo * Cout * 8 * 2, a_hi.device):
+            ah = F.pad(a_hi[sl].to(F64), (0, 0, 1, 1, 1, 1))
+            av = ah + F.pad(a_lo[sl].to(F64), (0, 0, 1, 1, 1, 1))
+            # split products A_hi W_hi + A_lo W_hi + A_hi W_lo (passes 3), or A_hi W_hi (passes 1), in fp64
+            phases = []
+            for tl_h, tl_l in zip(tap_of(wh), tap_of(wl)):
+                o = tap_conv(av if passes == 3 else ah, tl_h, H, W)
+                if passes == 3:
+                    o = o.add_(tap_conv(ah, tl_l, H, W))
+                phases.append(o)
+            if c["upsample2x"]:
+                o = torch.empty(phases[0].shape[0], Ho, Wo, Cout, dtype=F64, device=ah.device)
+                for ph, p in enumerate(phases):
+                    o[:, ph >> 1::2, ph & 1::2] = p
+            else:
+                o = phases[0]
+            if c["Cin2"]:
+                a2h = c["a2_hi"].reshape(B, H, W, -1)[sl].to(F64)
+                a2v = a2h + c["a2_lo"].reshape(B, H, W, -1)[sl].to(F64)
+                w2h, w2l = c["w2_hi"][0].to(F64), c["w2_lo"][0].to(F64)
+                n = a2h.shape[0]
+                o2 = (a2v if passes == 3 else a2h).reshape(-1, c["Cin2"]) @ w2h.t()
+                if passes == 3:
+                    o2 += a2h.reshape(-1, c["Cin2"]) @ w2l.t()
+                o = o + o2.view(n, H, W, Cout)
+                if c["bias2"] is not None:
+                    o = o + c["bias2"].to(F64)
+            if c["bias"] is not None:
+                o = o + c["bias"].to(F64)
+            o = add_residual(o, None if res is None else res[sl], c["res_mode"])
+            if nchw:
+                dv["out"].append(image_devs(a["out"][sl], o[..., :nchw].permute(0, 3, 1, 2)))
+            elif a["out"] is not None:
+                dv["out"].append(image_devs(a["out"][sl].reshape(o.shape), o))
+            if a["out_hi"] is not None:
+                hi, lo = a["out_hi"][sl].reshape(o.shape), a["out_lo"][sl].reshape(o.shape)
+                if a["out"] is None:
+                    dv["out planes"].append(image_devs(planes(hi, lo), o))
+                dv["out planes split"].append(self._split_of(hi, lo, None if a["out"] is None else
+                                                             a["out"].reshape(B, Ho, Wo, Cout), sl))
+        bound = {"out": self.bounds["conv_umma"], "out planes": self.bounds["conv_umma_planes"]}
+        for what, devs in dv.items():
+            self._record(idx, "conv_umma", form, what, torch.cat(devs), bound.get(what, 0.0), shapes)
+        if a["stats_partial"] is not None:
+            self._stats_check(idx, "conv_umma", form, shapes, a["out"].reshape(B, Ho, Wo, Cout), a["stats_partial"], B)
+
+    def _ref_position_gemms(self, idx, form, shapes, c, a):
+        P, Cout = c["B"], c["Cout"]
+        V = c["a_hi"].reshape(P, -1, c["Cin"])
+        Vl = c["a_lo"].reshape(P, -1, c["Cin"])
+        m = a["out"].reshape(P, -1, Cout)
+        devs = []
+        for sl in chunks(P, V.shape[1] * (c["Cin"] + Cout) * 8 * 2, V.device):
+            want = torch.bmm(planes(V[sl], Vl[sl]), planes(c["w_hi"][sl], c["w_lo"][sl]).transpose(1, 2))
+            devs.append(image_devs(m[sl], want))
+        self._record(idx, "conv_umma", form, "Winograd M (per position)", torch.cat(devs), self.bounds["wino_m"], shapes)
+        src = self._wino_in.pop(a["a_hi"].data_ptr(), None)
+        self._wino_m[a["out"].data_ptr()] = dict(launch=idx, input=src, u=a["w_hi"].data_ptr())
+
+    def _ref_conv_direct(self, idx, form, shapes, c, a, pre):
+        src, k, cout, stride = c["src"], c["k"], c["Cout"], c["stride"]
+        w = c["w_packed"].reshape(k, k, src.shape[3], cout).permute(3, 2, 0, 1).to(F64)
+        devs = []
+        for sl in chunks(src.shape[0], src[0].numel() * 8 * 4, src.device):
+            o = F.conv2d(src[sl].to(F64).permute(0, 3, 1, 2), w, None if c["bias"] is None else c["bias"].to(F64),
+                         stride=stride, padding=k // 2).permute(0, 2, 3, 1)
+            if c["residual"] is not None:
+                o = o + c["residual"][sl].to(F64)
+            devs.append(image_devs(a["out"][sl], o))
+        self._record(idx, "conv_direct", form, "out", torch.cat(devs), self.bounds["conv_direct"], shapes)
+
+    def _ref_conv_stem(self, idx, form, shapes, c, a, pre):
+        src, cout = c["src"], c["Cout"]
+        B, H, W, cin = src.shape
+        w = c["w_packed"].reshape(3, 3, cin, cout).permute(3, 2, 0, 1).to(F64)
+        devs = []
+        for sl in chunks(B, H * W * (cin + cout) * 8 * 2, src.device):
+            o = F.conv2d(src[sl].to(F64).permute(0, 3, 1, 2), w, None if c["bias"] is None else c["bias"].to(F64),
+                         padding=1).permute(0, 2, 3, 1)
+            devs.append(image_devs(a["out"][sl], o))
+        self._record(idx, "conv_stem", form, "out", torch.cat(devs), self.bounds["conv_stem"], shapes)
+        if a["stats_partial"] is not None:
+            self._stats_check(idx, "conv_stem", form, shapes, a["out"], a["stats_partial"], B)
+
+    # -- Winograd ----------------------------------------------------------------------------------------------
+    def _wino_act(self, rec, sl):
+        """fp64 input of the 3x3 conv of a wino_input launch (activation, 2x2-pooled for down2), images sl."""
+        c = rec["args"]
+        act = gn_act(cat(c["src1"], c["src2"]), c, sl)
+        return pool2(act) if c.get("down2") else act
+
+    @staticmethod
+    def _inputs_intact(rec):
+        """Whether the inputs of a wino_input launch that the shadow did not copy still hold what that launch read (the
+        whole-chain check reads them at the output transform)."""
+        return all(fingerprint(rec["args"][k]) == p for k, p in rec["args"]["_prints"].items())
+
+    def _ref_wino_input(self, idx, form, shapes, c, a, pre):
+        t = c.get("tile", 4)
+        x = cat(c["src1"], c["src2"])
+        B, Hs, Ws, C = x.shape
+        rec = dict(launch=idx, args=c, tile=t)
+        H, W = (Hs // 2, Ws // 2) if c.get("down2") else (Hs, Ws)
+        th, tw = -(-H // t), -(-W // t)
+        npos = (t + 2) ** 2
+        bt = _mat(BT, t, x.device)
+        vh, vl = a["v_hi"], a["v_lo"]
+        dv = collections.defaultdict(list)
+        for sl in chunks(B, Hs * Ws * C * 8 * 3 + npos * th * tw * C * 8 * 3, x.device):
+            act = self._wino_act(rec, sl)
+            n = act.shape[0]
+            pad = (0, 0, 1, t * tw + 1 - W, 1, t * th + 1 - H)
+            tiles = F.pad(act, pad).unfold(1, t + 2, t).unfold(2, t + 2, t)          # [n, th, tw, C, t+2, t+2]
+            V = torch.einsum("ij,nxycjk,lk->nilxyc", bt, tiles, bt).reshape(n, npos, th * tw, C)
+            rows = slice(sl.start * th * tw, sl.stop * th * tw)
+            got = planes(vh[:, rows], vl[:, rows]).reshape(npos, n, th * tw, C).transpose(0, 1)
+            dv[f"V F({t},3)"].append(image_devs(got, V))
+            if c["raw_hi"] is not None:
+                h, l = split_bf16(x[sl].float())
+                dv["raw planes (bit-exact split)"].append(torch.maximum(image_equal(a["raw_hi"][sl], h),
+                                                                        image_equal(a["raw_lo"][sl], l)))
+            if c["act_hi"] is not None:
+                dv["act planes"].append(image_devs(planes(a["act_hi"][sl], a["act_lo"][sl]), gn_act(x, c, sl)))
+                dv["act planes split"].append(pair_well_formed(a["act_hi"][sl], a["act_lo"][sl]))
+        bound = {f"V F({t},3)": self.bounds[f"wino_v{t}"], "act planes": self.bounds["wino_act_planes"]}
+        for what, devs in dv.items():
+            self._record(idx, "wino_input", form, what, torch.cat(devs), bound.get(what, 0.0), shapes)
+        zero = bool((vh[:, B * th * tw:] == 0).all()) and bool((vl[:, B * th * tw:] == 0).all())
+        self._record(idx, "wino_input", form, "GEMM padding rows zero", 0.0 if zero else math.inf, 0.0, shapes)
+        self._wino_in[vh.data_ptr()] = rec
+
+    def _ref_wino_output(self, idx, form, shapes, c, a, pre):
+        t, B, H, W, Cout = c.get("tile", 4), c["B"], c["H"], c["W"], c["Cout"]
+        up = c.get("up2_phases", False)
+        th, tw = -(-H // t), -(-W // t)
+        ncols = 4 * Cout if up else Cout
+        inv = 1.0 / 256.0 if c["inv_wscale"] is None else float(c["inv_wscale"].item())
+        at = _mat(AT, t, c["m"].device)
+        f = 2 if up else 1
+        Ho, Wo = f * H, f * W
+        res = c["residual"]
+        if res is not None:
+            rs = {1: (Ho, Wo), 2: (Ho // 2, Wo // 2), 3: (2 * Ho, 2 * Wo)}[c["res_mode"]]
+            res = res.reshape(B, rs[0], rs[1], Cout)
+        bias = 0.0 if c["bias"] is None else c["bias"].to(F64)
+        chain = self._wino_m.pop(a["m"].data_ptr(), None)
+        src = None if chain is None else chain["input"]
+        wt = None if chain is None else self._weights.get(chain["u"])
+        out = a["out"]
+        dv = collections.defaultdict(list)
+        M = c["m"].reshape((t + 2) ** 2, -1, ncols)
+        for sl in chunks(B, th * tw * (t + 2) ** 2 * ncols * 8 * 3 + Ho * Wo * Cout * 8 * 4, out.device):
+            n = out[sl].shape[0]
+            Mb = M[:, sl.start * th * tw:sl.stop * th * tw].to(F64).reshape(t + 2, t + 2, n, th, tw, ncols)
+            Y = torch.einsum("ij,jlnxyc,ml->nxiymc", at, Mb, at) * inv
+            y = Y.reshape(n, t * th, t * tw, ncols)[:, :H, :W]
+            if up:     # phase-major channels -> output pixel (2y + ph // 2, 2x + ph % 2)
+                yy = torch.empty(n, Ho, Wo, Cout, dtype=F64, device=y.device)
+                for ph in range(4):
+                    yy[:, ph >> 1::2, ph & 1::2] = y[..., ph * Cout:(ph + 1) * Cout]
+                y = yy
+            r = None if res is None else res[sl]
+            dv["Y = A^T M A / s"].append(image_devs(out[sl], add_residual(y + bias, r, c["res_mode"])))
+            if src is not None and wt is not None and self._inputs_intact(src):
+                act = self._wino_act(src, sl)
+                w, w_up, _ = wt
+                want = conv3x3(up2(act) if w_up else act, w.to(act.device, F64)) + bias
+                dv[f"chain F({t},3) vs fp64 conv"].append(image_devs(out[sl], add_residual(want, r, c["res_mode"])))
+        if chain is None or src is None or wt is None or not self._inputs_intact(src):
+            # an output transform whose GEMM, input transform or weight the shadow did not see cannot be checked whole
+            dv[f"chain F({t},3) vs fp64 conv"].append(torch.tensor([math.inf], dtype=F64))
+        bound = {"Y = A^T M A / s": self.bounds["wino_y"], f"chain F({t},3) vs fp64 conv": self.bounds[f"chain{t}"]}
+        for what, devs in dv.items():
+            self._record(idx, "wino_output", form, what, torch.cat([d.cpu() for d in devs]), bound[what], shapes)
+        if a["stats_partial"] is not None:
+            self._stats_check(idx, "wino_output", form, shapes, out, a["stats_partial"], B)
+
+    # -- attention ---------------------------------------------------------------------------------------------
+    def _attention(self, idx, name, form, shapes, qkv, c, a):
+        B, T, C3 = qkv.shape
+        dv = collections.defaultdict(list)
+        for sl in chunks(B, T * T * 8 * 2 + T * C3 * 8, qkv.device):
+            o = attention_ref(qkv[sl].to(F64) if qkv.dtype != F64 else qkv[sl], c["heads"], c["order"],
+                              slice(0, qkv[sl].shape[0]))
+            if a["out_f32"] is not None:
+                dv["out"].append(image_devs(a["out_f32"][sl], o))
+            if a["out_hi"] is not None:
+                if a["out_f32"] is None:
+                    dv["out planes"].append(image_devs(planes(a["out_hi"][sl], a["out_lo"][sl]), o))
+                dv["out planes split"].append(self._split_of(a["out_hi"][sl], a["out_lo"][sl], a["out_f32"], sl))
+        bound = {"out": self.bounds["attention"], "out planes": self.bounds["attention_planes"]}
+        for what, devs in dv.items():
+            self._record(idx, name, form, what, torch.cat(devs), bound.get(what, 0.0), shapes)
+
+    def _ref_attention(self, idx, form, shapes, c, a, pre):
+        self._attention(idx, "attention", form, shapes, c["qkv"], c, a)
+
+    def _ref_attention_split(self, idx, form, shapes, c, a, pre):
+        self._attention(idx, "attention_split", form, shapes, planes(c["qkv_hi"], c["qkv_lo"]), c, a)
+
+    def _ref_attention_tc(self, idx, form, shapes, c, a, pre):
+        self._attention(idx, "attention_tc", form, shapes, planes(c["qkv_hi"], c["qkv_lo"]), c, a)
+
+
+# ------------------------------------------------------------------------------------------------ coverage
+# (method, features that one launch's form must all have, features it must not have).  What the cfg2 routing issues: the
+# F(6,3) forms -- plain, two-source with the raw planes of a fused 1x1 skip, the down-ResBlock's pooled conv1, the
+# up-ResBlock's phase-stacked conv1, each residual mode -- and the direct tensor-core forms.  Its up-ResBlocks all take
+# the phase-stacked F(6,3) conv, so the fused nearest-2x direct conv (UPSAMPLE_FORMS) is required of cfg1 and cfg3-5.
+CFG2_FORMS = [
+    ("wino_input", ("F(6,3)",), ("two-source", "down2", "raw planes")),
+    ("wino_input", ("F(6,3)", "two-source", "raw planes"), ()),
+    ("wino_input", ("F(6,3)", "down2"), ()),
+    ("wino_output", ("F(6,3)", "up2_phases"), ()),
+    ("wino_output", ("F(6,3)",), ("res", "up2_phases")),
+    ("wino_output", ("F(6,3)", "res 1"), ()),
+    ("wino_output", ("F(6,3)", "res 2"), ()),
+    ("wino_output", ("F(6,3)", "res 3"), ()),
+    ("conv_umma", ("position GEMMs",), ()),
+    ("conv_umma", ("fused 1x1",), ()),
+    ("conv_umma", ("NCHW head",), ()),
+    ("conv_umma", ("split out",), ()),
+    ("conv_umma", ("taps 9", "res 1"), ()),
+    ("conv_umma", ("taps 9", "res 3"), ()),
+    ("attention_tc", (), ()),
+    ("conv_stem", (), ()),
+]
+UPSAMPLE_FORMS = [("conv_umma", ("upsample2x",), ())]
+F43_FORMS = [("wino_input", ("F(4,3)",), ()), ("wino_output", ("F(4,3)",), ())]
+
+
+def missing_forms(shadow, required):
+    """The entries of required that no launch of the shadow matched."""
+    return [r for r in required if not any(m == r[0] and all(f in form for f in r[1]) and
+                                           not any(f in form for f in r[2]) for m, form in shadow.launches)]
