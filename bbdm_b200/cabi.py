@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BBDM_LIB selects another in-tree build of the same sources (A/B experiments, tools/); the product default is fixed
 LIB_PATH = os.environ.get("BBDM_LIB") or os.path.join(_HERE, "libbbdm_b200.so")
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 OBJ = {"grad": 0, "noise": 1, "ysubx": 2}
 RESAMPLE_NONE, RESAMPLE_UP2, RESAMPLE_DOWN2 = 0, 1, 2
 RES_NONE, RES_SAME, RES_UP2, RES_DOWN2 = 0, 1, 2, 3
@@ -167,7 +167,8 @@ def load():
     lib.bbdm_geglu_bwd.argtypes = [vp, vp, i64, i, vp, vp]
     lib.bbdm_attention_cross_bwd.argtypes = [vp, vp, vp, vp, i, i, i, i, i, vp, vp, vp, vp, vp]
     lib.bbdm_optim_chunk_elems.argtypes = []
-    lib.bbdm_adam_multi.argtypes = [vp, vp, vp, vp, vp, vp, i, vp, vp, f, f, f, f, f, i64, vp, C.c_double, vp]
+    lib.bbdm_adam_multi.argtypes = [vp, vp, vp, vp, vp, vp, i, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double,
+                                     C.c_double, i64, vp, C.c_double, vp]
     lib.bbdm_ema_multi.argtypes = [vp, vp, vp, vp, vp, i, vp, C.c_double, i, vp]
     for s in SYMBOLS:
         fn = getattr(lib, s)

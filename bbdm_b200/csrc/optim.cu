@@ -80,19 +80,21 @@ int bbdm_optim_chunk_elems(void) { return OPT_CHUNK; }
 
 int bbdm_adam_multi(void* const* params, const void* const* grads, const int64_t* numel, const int64_t* state_off,
                     const int32_t* chunk_tensor, const int32_t* chunk_index, int n_chunks, float* exp_avg,
-                    float* exp_avg_sq, float lr, float beta1, float beta2, float eps, float weight_decay, int64_t step,
+                    float* exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay, int64_t step,
                     float* ema_shadow, double ema_decay, void* stream) {
   BBDM_REQUIRE(params && grads && numel && state_off && chunk_tensor && chunk_index && exp_avg && exp_avg_sq,
                "adam_multi: null pointer");
   BBDM_REQUIRE(n_chunks > 0 && step >= 1, "adam_multi: need n_chunks > 0 and step >= 1");
-  // scalar preparation exactly as torch.optim.adam._single_tensor_adam does it (python floats = fp64)
-  const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
+  // scalar preparation exactly as torch.optim.adam._single_tensor_adam does it (python floats = fp64), each scalar
+  // rounded to fp32 once at the end.  The hyper-parameters must arrive as doubles: 1 - beta2 of an fp32-rounded beta2
+  // 0.999 is 1.3e-5 off, and with it exp_avg_sq and the bias correction.
+  const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
   AdamScalars a;
-  a.lr_over_bc1 = (float)((double)lr / bc1);
-  a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = weight_decay;
+  a.lr_over_bc1 = (float)(lr / bc1);
+  a.beta1 = (float)beta1; a.beta2 = (float)beta2; a.eps = (float)eps; a.weight_decay = (float)weight_decay;
   a.inv_bc2_sqrt = (float)(1.0 / sqrt(bc2));
-  a.one_minus_beta1 = (float)(1.0 - (double)beta1);
-  a.one_minus_beta2 = (float)(1.0 - (double)beta2);
+  a.one_minus_beta1 = (float)(1.0 - beta1);
+  a.one_minus_beta2 = (float)(1.0 - beta2);
   a.ema_decay = ema_shadow ? (float)ema_decay : -1.0f;
   a.ema_one_minus = (float)(1.0 - ema_decay);
   adam_multi_kernel<<<n_chunks, 256, 0, (cudaStream_t)stream>>>((float* const*)params, (const float* const*)grads, numel,

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define BBDM_ABI_VERSION 4
+#define BBDM_ABI_VERSION 5
 
 enum {
   BBDM_OK = 0,
@@ -469,12 +469,13 @@ int bbdm_denorm_to_uint8(const float* images, int B, int C, int H, int W, int to
 int bbdm_optim_chunk_elems(void);
 
 /* torch.optim.Adam's update (the optimizer runners/utils.py:48-57 builds, stepped at runners/BaseRunner.py:413),
- * non-amsgrad, L2 weight decay, `step` = the 1-based step count of this update (bias corrections computed in fp64 as
- * torch does).  ema_shadow != NULL additionally applies shadow = (1-ema_decay)*p_new + ema_decay*shadow in the same
+ * non-amsgrad, L2 weight decay, `step` = the 1-based step count of this update.  The hyper-parameters are doubles like
+ * the python floats torch.optim.Adam holds: 1 - beta1, 1 - beta2 and the bias corrections are computed from them in
+ * fp64, as torch does, before each is rounded to fp32 once.  ema_shadow != NULL additionally applies shadow = (1-ema_decay)*p_new + ema_decay*shadow in the same
  * pass (runners/base/EMA.py:21-29 with with_decay=True). */
 int bbdm_adam_multi(void* const* params, const void* const* grads, const int64_t* numel, const int64_t* state_off,
                     const int32_t* chunk_tensor, const int32_t* chunk_index, int n_chunks, float* exp_avg,
-                    float* exp_avg_sq, float lr, float beta1, float beta2, float eps, float weight_decay, int64_t step,
+                    float* exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay, int64_t step,
                     float* ema_shadow, double ema_decay, void* stream);
 
 /* EMA.update (runners/base/EMA.py:21-29): shadow = (1-decay)*param + decay*shadow (the reference's operation

@@ -15,6 +15,14 @@ The Winograd chains are paired by buffer identity (wino_input's V planes -> the 
 output -> wino_output's M) and checked stage by stage and as a whole, against the fp64 conv of the fp64 activation with
 the module's fp32 weight; ``register_engine`` maps each cache entry's U planes to its module weight.
 
+The training Functions of bbdm_b200/train.py and FusedAdam are checked the same way: the backward kernels against fp64
+autograd of the operation they implement, from the launch's own inputs (GroupNorm statistics, split planes, the forward
+output attention_bwd reads); the weight packers bit for bit; adam_multi per parameter tensor against an fp64
+torch.optim.Adam step from the pre-launch parameters, gradients and moments, which it reads through the TensorTable's
+pointer arrays rather than tensor arguments.  Training packs its Winograd weight planes on the fly, so
+wino_pack_weight itself maps the U planes to the weight they hold (for the data gradient the flipped, channel-swapped
+kernel), and the output transform that consumes them takes the entry out again.
+
 Bounds are those of the single-kernel GPU tests, measured on an H100 with synthetic operands; each names its source.
 A launch whose output goes beyond its bound is a finding, not a bound to raise.
 """
@@ -42,7 +50,20 @@ OUTPUTS = {
     "wino_input": ("v_hi", "v_lo", "raw_hi", "raw_lo", "act_hi", "act_lo"), "wino_output": ("out", "stats_partial"),
     "attention": ("out_f32", "out_hi", "out_lo"), "attention_split": ("out_f32", "out_hi", "out_lo"),
     "attention_tc": ("out_f32", "out_hi", "out_lo"),
+    # training: bridge, gradient operands, backward kernels, optimizer
+    "q_sample": ("xt_out", "obj_out"),
+    "split_grad": ("hi", "lo", "hi_t", "lo_t", "colsum", "workspace"),
+    "pack_weight_split_both": ("f_hi", "f_lo", "d_hi", "d_lo"), "pack_weight_split_dgrad": ("hi", "lo"),
+    "conv_wgrad": ("dw", "workspace"), "conv_wgrad_direct": ("dw", "workspace"),
+    "gn_bwd_reduce": ("a12", "ws"), "gn_bwd_apply": ("dx",),
+    "attention_bwd": ("dqkv", "lse", "delta"),
+    "attention_cross": ("out_f32", "out_hi", "out_lo"), "attention_cross_bwd": ("dq", "dkv", "lse", "delta"),
+    "layernorm_split": ("out_f32", "out_hi", "out_lo"), "layernorm_bwd": ("dx", "dgamma", "dbeta", "workspace"),
+    "geglu_split": ("out_f32", "out_hi", "out_lo"), "geglu_bwd": ("du",),
+    "adam_multi": ("exp_avg", "exp_avg_sq", "ema_shadow"), "ema_multi": ("shadow",),
 }
+# launches that read (and adam_multi writes) the parameters of a TensorTable instead of tensor arguments
+TABLE_LAUNCHES = ("adam_multi", "ema_multi")
 
 # a split-bf16 pair carries 16 bits: 2^-17 = 7.6e-6 of the element (test_gpu_winograd.py::test_wino_input_production_layouts)
 PAIR = 8e-6
@@ -74,9 +95,37 @@ BOUNDS = {
     "wino_y": 5e-6,
     "chain6": 2e-5,             # test_gpu_winograd6.py CHAIN_BOUND
     "chain4": 1.6e-5,           # test_gpu_winograd.py CHAIN_BOUND_BIASED
+    # The training data gradient's F(4,3) chain (identity input transform of the power-of-two normalised dY, flipped
+    # weight planes), per image.  CHAIN_BOUND_BIASED was measured on forward chains, whole tensor.  The dgrad chains of
+    # the cfg3 training step at B = 32 reach 1.63e-5 on an H100 80GB HBM3 (700 W; the 32x32 512-channel convs) with
+    # every stage within its own bound (V 3.6e-7, position GEMMs 1.5e-6, output transform 2.4e-6), and the CPU
+    # emulation, whose transforms are exact fp64, reaches 1.65e-5 on the same kind of operands
+    # (test_train_shadow_host.py): the F(4,3) deviation of 22-bit fp16-pair planes on data-gradient operands.
+    "chain4_dgrad": 2e-5,
     "pack_wino6": 1e-6,         # test_gpu_winograd6.py::test_wino6_pack_weight
     "pack_wino4": 2e-7,         # test_gpu_winograd.py::test_wino_pack_weight
     "up_phase": 2.0 ** -16,     # test_gpu_kernels.py::test_conv_umma_fused_upsample: the taps are summed in fp32, then split
+    # training
+    "colsum": 1e-6,             # test_gpu_training.py::test_split_grad
+    "conv_wgrad": 2e-5,         # test_gpu_training.py::test_conv_wgrad (whole tensor)
+    "conv_wgrad_direct": 2e-6,  # test_gpu_training.py::test_small_conv_function_gradients
+    "gn_bwd": 2e-6,             # test_gpu_training.py::test_gn_bwd_kernels
+    "attention_bwd": 2e-5,      # test_gpu_training.py::test_attention_bwd_kernel
+    "attention_cross": 2e-5,    # test_gpu_kernels.py::test_attention_cross
+    "attention_cross_bwd": 2e-5,  # test_gpu_transformer_training.py::test_attention_cross_bwd_kernel
+    "layernorm": 2e-6,          # test_gpu_kernels.py::test_layernorm_split
+    "layernorm_planes": 2e-6 + PAIR,
+    "layernorm_bwd": 2e-6,      # test_gpu_transformer_training.py::test_layernorm_bwd_kernel
+    "geglu": 2e-6,              # test_gpu_kernels.py::test_geglu_split
+    "geglu_planes": 2e-6 + PAIR,
+    "geglu_bwd": 2e-6,          # test_gpu_transformer_training.py::test_geglu_bwd_kernel
+    # adam_multi / ema_multi, per parameter tensor.  No single-kernel test bounds these at this granularity
+    # (test_optim_host.py compares parameters after several steps).  The moments and the EMA shadow are one fp32
+    # multiply-add of the previous value: a few 2^-24 of the tensor's largest element.  The update dp is counted
+    # beyond the half-ulp of the fp32 parameter that has to hold it (see _ref_adam_multi).
+    "adam_dp": 1e-5,
+    "adam_moments": 1e-6,
+    "ema": 1e-6,
 }
 
 # Winograd matrices, interpolation points 0, +-1, +-2 (F(4,3)) and 0, +-1, +-2, +-1/2 (F(6,3))
@@ -268,6 +317,8 @@ class Shadow:
         self.mutate = {}                  # launch index -> fn(bound arguments): perturbs an output after the launch
         self._wino_in, self._wino_m = {}, {}
         self._weights = {}                # U planes' data_ptr -> (module weight [Cout, Cin, 3, 3], up2_phases, name)
+        self._packed = {}                 # U planes' data_ptr -> (weight clone, dgrad) of an on-the-fly pack
+        self._dgrad_w = set()             # data_ptrs of data-gradient split planes not yet read by a conv
 
     # -- bookkeeping -------------------------------------------------------------------------------------------
     def register_engine(self, eng):
@@ -281,6 +332,7 @@ class Shadow:
             if "u_hi" in ent:
                 w = eng.unet.get_submodule(mod).weight.detach()
                 self._weights[ent["u_hi"].data_ptr()] = (w, name.endswith("#up6"), name)
+                self._packed.pop(ent["u_hi"].data_ptr(), None)
             if "up_hi" in ent:
                 w = eng.unet.get_submodule(mod).weight.detach()
                 d = image_devs(planes(ent["up_hi"], ent["up_lo"])[None], up_phase_reference(w)[None])
@@ -336,9 +388,13 @@ class Shadow:
             big = {k for k, v in ins.items() if v.numel() * v.element_size() >= BIG}
             clones = {k: v.clone() for k, v in ins.items() if k not in big}
             prints = {k: fingerprint(ins[k]) for k in big}
-            pre = {k: a[k].clone() for k in outs} if name == "pack_weight_split" else {}
+            pre = {k: a[k].clone() for k in outs} if name in ("pack_weight_split",) + TABLE_LAUNCHES else {}
+            tab = a.get("tab") if name in TABLE_LAUNCHES else None
+            if tab is not None:         # what the launch reads through the table's pointer arrays
+                pre["params"] = [p.detach().clone() for p in tab.tensors]
+                pre["grads"] = [None if p.grad is None else p.grad.clone() for p in tab.tensors]
             r = attr(*args, **kwargs)
-            dev = next(iter(ins.values())).device
+            dev = next((v.device for v in a.values() if isinstance(v, torch.Tensor)), None) or tab.device
             if dev.type == "cuda":
                 torch.cuda.synchronize(dev)
             self.be.check_fault()
@@ -353,6 +409,12 @@ class Shadow:
                     same = fingerprint(v) == prints[k] if k in big else bits_equal(v, clones[k])
                     self._record(idx, name, form, "inputs unchanged", 0.0 if same else math.inf, 0.0,
                                  [(k, tuple(v.shape))])
+            if tab is not None:         # adam_multi reads the gradients, ema_multi the parameters
+                read = [p.grad for p in tab.tensors] if name == "adam_multi" else [p.detach() for p in tab.tensors]
+                want = pre["grads"] if name == "adam_multi" else pre["params"]
+                same = all((g is None) == (w is None) and (g is None or bits_equal(g, w)) for g, w in zip(read, want))
+                self._record(idx, name, form, "inputs unchanged", 0.0 if same else math.inf, 0.0,
+                             [("tab", len(tab.tensors))])
             c = dict(a, **clones)            # the launch's arguments, inputs replaced by their clones
             c["_prints"] = prints
             getattr(self, "_ref_" + name)(idx, form, shapes, c, a, pre)
@@ -362,13 +424,15 @@ class Shadow:
             return r
         return launch
 
-    @staticmethod
-    def _form(name, a):
+    def _form(self, name, a):
         f = []
         if name == "conv_umma":
             if a["weights_per_image"]:
                 return "position GEMMs"
             f.append(f"taps {a['taps']}")
+            if a["w_hi"].data_ptr() in self._dgrad_w:        # a training data gradient (each plane set is read once)
+                self._dgrad_w.discard(a["w_hi"].data_ptr())
+                f.append("dgrad")
             f += [t for t, on in (("upsample2x", a["upsample2x"]), ("fused 1x1", a["Cin2"]),
                                   ("NCHW head", a["out_nchw_channels"]), ("split out", a["out_hi"] is not None),
                                   ("stats", a["stats_partial"] is not None)) if on]
@@ -376,6 +440,8 @@ class Shadow:
                 f.append(f"res {a['res_mode']}")
         elif name in ("wino_input", "wino_output", "wino_pack_weight"):
             f.append(f"F({a.get('tile', 4)},3)")
+            if name == "wino_pack_weight" and a["dgrad"]:
+                f.append("dgrad")
             if name == "wino_input":
                 f += [t for t, on in (("two-source", a["src2"] is not None), ("raw planes", a["raw_hi"] is not None),
                                       ("act planes", a["act_hi"] is not None), ("down2", a.get("down2")),
@@ -389,6 +455,22 @@ class Shadow:
             f.append("gn" if a["mean"] is not None else "raw")
             f += [t for t, on in (("two-source", a["src2"] is not None), ("film", a["film_scale"] is not None),
                                   (f"resample {a['resample']}", a["resample"])) if on]
+        elif name == "split_grad":
+            f += [t for t, on in (("planes", a["hi"] is not None), ("colsum", a["colsum"] is not None)) if on]
+        elif name == "conv_wgrad":
+            f.append(f"taps {a['taps']}")
+        elif name == "conv_wgrad_direct":
+            f.append(f"taps {a['k'] ** 2}")
+            if a["x"].shape[3] * a["dy"].shape[3] > 1024:
+                f.append("beyond 1024 channel pairs")
+        elif name in ("gn_bwd_reduce", "gn_bwd_apply"):
+            f += [t for t, on in (("film", a["fscale"] is not None), ("no act", not a["silu"])) if on]
+        elif name == "attention_bwd":
+            f.append(f"order {a['order']}")
+        elif name == "adam_multi":
+            f.append(f"step {a['step']}")
+            if a["ema_shadow"] is not None:
+                f.append("ema")
         return " ".join(f)
 
     # -- references: layout / dense ----------------------------------------------------------------------------
@@ -523,6 +605,8 @@ class Shadow:
         self._record(idx, "wino_pack_weight", form, f"U planes F({t},3)", image_devs(planes(a["u_hi"], a["u_lo"])[None],
                                                                                    U[None]),
                      self.bounds[f"pack_wino{t}"], shapes)
+        # the weight the chain through these planes computes with (register_engine's entries take precedence)
+        self._packed[a["u_hi"].data_ptr()] = (c["w"], bool(c["dgrad"]))
 
     # -- convolutions ------------------------------------------------------------------------------------------
     def _stats_check(self, idx, method, form, shapes, out, part, B):
@@ -713,6 +797,12 @@ class Shadow:
         chain = self._wino_m.pop(a["m"].data_ptr(), None)
         src = None if chain is None else chain["input"]
         wt = None if chain is None else self._weights.get(chain["u"])
+        packed = None if chain is None else self._packed.pop(chain["u"], None)     # a freed address must not pair again
+        dgrad = False
+        if wt is None and packed is not None:
+            w, dgrad = packed
+            wt = (w.to(F64).flip(2, 3).transpose(0, 1) if dgrad else w, False, "packed with the launch")
+        whole = f"chain F({t},3){' dgrad' if dgrad else ''} vs fp64 conv"
         out = a["out"]
         dv = collections.defaultdict(list)
         M = c["m"].reshape((t + 2) ** 2, -1, ncols)
@@ -732,11 +822,11 @@ class Shadow:
                 act = self._wino_act(src, sl)
                 w, w_up, _ = wt
                 want = conv3x3(up2(act) if w_up else act, w.to(act.device, F64)) + bias
-                dv[f"chain F({t},3) vs fp64 conv"].append(image_devs(out[sl], add_residual(want, r, c["res_mode"])))
+                dv[whole].append(image_devs(out[sl], add_residual(want, r, c["res_mode"])))
         if chain is None or src is None or wt is None or not self._inputs_intact(src):
             # an output transform whose GEMM, input transform or weight the shadow did not see cannot be checked whole
-            dv[f"chain F({t},3) vs fp64 conv"].append(torch.tensor([math.inf], dtype=F64))
-        bound = {"Y = A^T M A / s": self.bounds["wino_y"], f"chain F({t},3) vs fp64 conv": self.bounds[f"chain{t}"]}
+            dv[whole].append(torch.tensor([math.inf], dtype=F64))
+        bound = {"Y = A^T M A / s": self.bounds["wino_y"], whole: self.bounds[f"chain{t}{'_dgrad' if dgrad else ''}"]}
         for what, devs in dv.items():
             self._record(idx, "wino_output", form, what, torch.cat([d.cpu() for d in devs]), bound[what], shapes)
         if a["stats_partial"] is not None:
@@ -768,6 +858,314 @@ class Shadow:
     def _ref_attention_tc(self, idx, form, shapes, c, a, pre):
         self._attention(idx, "attention_tc", form, shapes, planes(c["qkv_hi"], c["qkv_lo"]), c, a)
 
+    # -- training: bridge, gradient operands, weight packing -----------------------------------------------------
+    def _ref_q_sample(self, idx, form, shapes, c, a, pre):
+        """The oracle's expression on the CPU, as test_gpu_kernels.py::test_q_sample_bit_exact holds the kernel to."""
+        cpu = lambda k: c[k].cpu()
+        xt, obj = O.q_sample({"m_t": cpu("m_t"), "variance_t": cpu("var_t")}, cpu("x0"), cpu("y"), cpu("t"),
+                             cpu("noise"), c["objective"])
+        for what, got, want in (("x_t", a["xt_out"], xt), ("objective", a["obj_out"], obj)):
+            self._record(idx, "q_sample", form, what, image_equal(got.cpu(), want), 0.0, shapes)
+
+    def _ref_split_grad(self, idx, form, shapes, c, a, pre):
+        src = c["src"]
+        h, l = split_bf16(src.reshape(-1, src.shape[-1]))
+        if a["hi"] is not None:
+            self._record(idx, "split_grad", form, "planes (bit-exact split)",
+                         torch.maximum(image_equal(a["hi"], h.reshape(a["hi"].shape)),
+                                       image_equal(a["lo"], l.reshape(a["lo"].shape))), 0.0, shapes)
+        if a["hi_t"] is not None:
+            ok = bits_equal(a["hi_t"], h.t().contiguous()) and bits_equal(a["lo_t"], l.t().contiguous())
+            self._record(idx, "split_grad", form, "transposed planes (bit-exact)", 0.0 if ok else math.inf, 0.0, shapes)
+        if a["colsum"] is not None:
+            want = src.reshape(-1, src.shape[-1]).to(F64).sum(0)
+            self._record(idx, "split_grad", form, "column sums", image_devs(a["colsum"][None], want[None]),
+                         self.bounds["colsum"], shapes)
+
+    @staticmethod
+    def _dgrad_layout(w):
+        """[Cout, Cin, k, k] -> [k*k, Cin, Cout]: the kernel flipped, the channels swapped."""
+        k = w.shape[2]
+        return w.flip(2, 3).permute(2, 3, 1, 0).reshape(k * k, w.shape[1], w.shape[0]).contiguous()
+
+    def _ref_pack_weight_split_both(self, idx, form, shapes, c, a, pre):
+        w = c["w"]
+        k = w.shape[2]
+        ok = True
+        if a["f_hi"] is not None:
+            h, l = split_bf16(w.permute(2, 3, 0, 1).reshape(k * k, w.shape[0], w.shape[1]).contiguous())
+            ok = bits_equal(a["f_hi"], h) and bits_equal(a["f_lo"], l)
+        if a["d_hi"] is not None:
+            h, l = split_bf16(self._dgrad_layout(w))
+            ok = ok and bits_equal(a["d_hi"], h) and bits_equal(a["d_lo"], l)
+            self._dgrad_w.add(a["d_hi"].data_ptr())
+        self._record(idx, "pack_weight_split_both", form, "split planes", 0.0 if ok else math.inf, 0.0, shapes)
+
+    def _ref_pack_weight_split_dgrad(self, idx, form, shapes, c, a, pre):
+        h, l = split_bf16(self._dgrad_layout(c["w"]))
+        ok = bits_equal(a["hi"], h) and bits_equal(a["lo"], l)
+        self._dgrad_w.add(a["hi"].data_ptr())
+        self._record(idx, "pack_weight_split_dgrad", form, "split planes", 0.0 if ok else math.inf, 0.0, shapes)
+
+    # -- training: weight gradients ------------------------------------------------------------------------------
+    @staticmethod
+    def _wgrad64(act, grad_rows, k):
+        """fp64 weight gradient [Cout, Cin, k, k] of a stride-1 'same' conv: act [B, H, W, Cin] (any dtype), grad_rows
+        fn(slice of images) -> [Cout, n*H*W] fp64, summed over image chunks."""
+        B, H, W, Cin = act.shape
+        p = k // 2
+        dw = None
+        for sl in chunks(B, (H + 2 * p) * (W + 2 * p) * Cin * 8 * 2, act.device):
+            ap = F.pad(act[sl].to(F64), (0, 0, p, p, p, p))
+            g = grad_rows(sl)
+            if dw is None:
+                dw = torch.zeros(g.shape[0], Cin, k, k, dtype=F64, device=act.device)
+            for ky in range(k):
+                for kx in range(k):
+                    dw[:, :, ky, kx] += g @ ap[:, ky:ky + H, kx:kx + W].reshape(-1, Cin)
+        return dw
+
+    def _ref_conv_wgrad(self, idx, form, shapes, c, a, pre):
+        B, H, W, Cin, Cout, taps = c["B"], c["H"], c["W"], c["Cin"], c["Cout"], c["taps"]
+        act = planes(c["a_hi"], c["a_lo"]).reshape(B, H, W, Cin)
+        gh, gl = c["g_hi_t"].reshape(Cout, -1), c["g_lo_t"].reshape(Cout, -1)
+        rows = lambda sl: planes(gh[:, sl.start * H * W:sl.stop * H * W], gl[:, sl.start * H * W:sl.stop * H * W])
+        want = self._wgrad64(act, rows, 3 if taps == 9 else 1)
+        self._record(idx, "conv_wgrad", form, "dW", image_devs(a["dw"][None], want[None]), self.bounds["conv_wgrad"],
+                     shapes)
+
+    def _ref_conv_wgrad_direct(self, idx, form, shapes, c, a, pre):
+        dy = c["dy"]
+        B, H, W, Cout = dy.shape
+        rows = lambda sl: dy[sl].to(F64).reshape(-1, Cout).t()
+        want = self._wgrad64(c["x"], rows, c["k"])
+        self._record(idx, "conv_wgrad_direct", form, "dW", image_devs(a["dw"][None], want[None]),
+                     self.bounds["conv_wgrad_direct"], shapes)
+
+    # -- training: GroupNorm (+FiLM) (+SiLU) backward ------------------------------------------------------------
+    @staticmethod
+    def _gn_bwd_terms(c, sl):
+        """fp64 (x_hat, dz, rstd, 1 + scale) of images sl, from the fp32 statistics the launch got."""
+        x = c["x"][sl].to(F64)
+        C, G = x.shape[3], c["groups"]
+        e = lambda t: t[sl].to(F64).repeat_interleave(C // G, 1)[:, None, None, :]
+        r = e(c["rstd"])
+        xh = (x - e(c["mean"])) * r
+        f1 = f0 = None
+        if c["fscale"] is not None:
+            f1 = 1.0 + c["fscale"][sl, :C].to(F64)[:, None, None, :]
+            f0 = c["fshift"][sl, :C].to(F64)[:, None, None, :]
+        z = c["gamma"].to(F64) * xh + c["beta"].to(F64)
+        if f1 is not None:
+            z = z * f1 + f0
+        da = c["da"][sl].to(F64)
+        if c["silu"]:
+            sg = torch.sigmoid(z)
+            da = da * sg * (1 + z * (1 - sg))
+        return xh, da, r, (1.0 if f1 is None else f1)
+
+    def _ref_gn_bwd_reduce(self, idx, form, shapes, c, a, pre):
+        B, H, W, C = c["x"].shape
+        dv = collections.defaultdict(list)
+        for sl in chunks(B, H * W * C * 8 * 6, c["x"].device):
+            xh, dz, _, _ = self._gn_bwd_terms(c, sl)
+            dv["sum dz"].append(image_devs(a["a12"][sl, :, 0], dz.sum((1, 2))))
+            dv["sum dz*x_hat"].append(image_devs(a["a12"][sl, :, 1], (dz * xh).sum((1, 2))))
+        for what, devs in dv.items():
+            self._record(idx, "gn_bwd_reduce", form, what, torch.cat(devs), self.bounds["gn_bwd"], shapes)
+
+    def _ref_gn_bwd_apply(self, idx, form, shapes, c, a, pre):
+        B, H, W, C = c["x"].shape
+        G = c["groups"]
+        n = H * W * (C // G)
+        devs = []
+        for sl in chunks(B, H * W * C * 8 * 6, c["x"].device):
+            xh, dz, r, f1 = self._gn_bwd_terms(c, sl)
+            e = lambda t: t[sl].to(F64).repeat_interleave(C // G, 1)[:, None, None, :]
+            want = r * (dz * c["gamma"].to(F64) * f1 - (e(c["s1"]) + xh * e(c["s2"])) / n)
+            devs.append(image_devs(a["dx"][sl], want))
+        self._record(idx, "gn_bwd_apply", form, "dx", torch.cat(devs), self.bounds["gn_bwd"], shapes)
+
+    # -- training: attention backward, SpatialTransformer pieces -------------------------------------------------
+    @staticmethod
+    def _attention64(qkv, heads, order):
+        """softmax(q k^T / sqrt(d)) v of qkv [n, T, 3C] (fp64, differentiable) -> [n, T, C]."""
+        n, T, C3 = qkv.shape
+        d = C3 // 3 // heads
+        if order:
+            q, k, v = qkv.view(n, T, 3, heads, d).unbind(2)
+        else:
+            q, k, v = qkv.view(n, T, heads, 3, d).unbind(3)
+        s = torch.softmax(torch.einsum("nthd,nshd->nhts", q, k) / math.sqrt(d), dim=-1)
+        return torch.einsum("nhts,nshd->nthd", s, v).reshape(n, T, C3 // 3)
+
+    @staticmethod
+    def _cross64(q, kv, heads):
+        """softmax(q k^T / sqrt(d)) v for queries q [n, Tq, C] and k|v kv [n, Tkv, 2C] (fp64) -> [n, Tq, C]."""
+        n, Tq, C = q.shape
+        d = C // heads
+        sp = lambda t: t.reshape(n, t.shape[1], heads, d)
+        s = torch.softmax(torch.einsum("nthd,nshd->nhts", sp(q), sp(kv[..., :C])) / math.sqrt(d), dim=-1)
+        return torch.einsum("nhts,nshd->nthd", s, sp(kv[..., C:])).reshape(n, Tq, C)
+
+    def _ref_attention_bwd(self, idx, form, shapes, c, a, pre):
+        qkv = c["qkv"]
+        B, T, C3 = qkv.shape
+        devs = []
+        for sl in chunks(B, c["heads"] * T * T * 8 * 4 + T * C3 * 8 * 4, qkv.device):
+            q = qkv[sl].to(F64).requires_grad_(True)
+            with torch.enable_grad():
+                self._attention64(q, c["heads"], c["order"]).backward(c["dout"][sl].to(F64))
+            devs.append(image_devs(a["dqkv"][sl], q.grad))
+        self._record(idx, "attention_bwd", form, "dqkv", torch.cat(devs), self.bounds["attention_bwd"], shapes)
+
+    def _ref_attention_cross(self, idx, form, shapes, c, a, pre):
+        q, kv = planes(c["q_hi"], c["q_lo"]), planes(c["kv_hi"], c["kv_lo"])
+        B, Tq, _ = q.shape
+        dv = collections.defaultdict(list)
+        for sl in chunks(B, c["heads"] * Tq * kv.shape[1] * 8 * 3, q.device):
+            o = self._cross64(q[sl], kv[sl], c["heads"])
+            self._rows_out(dv, a, sl, o)
+        self._record_rows(idx, "attention_cross", form, shapes, dv, "attention_cross")
+
+    def _ref_attention_cross_bwd(self, idx, form, shapes, c, a, pre):
+        B, Tq, _ = c["q"].shape
+        Tkv = c["kv"].shape[1]
+        dq, dkv = [], []
+        for sl in chunks(B, c["heads"] * Tq * Tkv * 8 * 4, c["q"].device):
+            q, kv = c["q"][sl].to(F64).requires_grad_(True), c["kv"][sl].to(F64).requires_grad_(True)
+            with torch.enable_grad():
+                self._cross64(q, kv, c["heads"]).backward(c["dout"][sl].to(F64))
+            dq.append(image_devs(a["dq"][sl], q.grad))
+            dkv.append(image_devs(a["dkv"][sl], kv.grad))
+        for what, devs in (("dq", dq), ("dkv", dkv)):
+            self._record(idx, "attention_cross_bwd", form, what, torch.cat(devs), self.bounds["attention_cross_bwd"],
+                         shapes)
+
+    def _rows_out(self, dv, a, sl, want):
+        """Row outputs (out_f32 and / or split planes) of images sl against want."""
+        shp = lambda t: t[sl].reshape(want.shape)
+        if a["out_f32"] is not None:
+            dv["out"].append(image_devs(shp(a["out_f32"]), want))
+        if a["out_hi"] is not None:
+            hi, lo = shp(a["out_hi"]), shp(a["out_lo"])
+            if a["out_f32"] is None:
+                dv["out planes"].append(image_devs(planes(hi, lo), want))
+            dv["out planes split"].append(self._split_of(hi, lo, None if a["out_f32"] is None else
+                                                         a["out_f32"].reshape(a["out_f32"].shape[0], *want.shape[1:]),
+                                                         sl))
+
+    def _record_rows(self, idx, method, form, shapes, dv, key):
+        bound = {"out": self.bounds[key], "out planes": self.bounds.get(key + "_planes", self.bounds[key] + PAIR)}
+        for what, devs in dv.items():
+            self._record(idx, method, form, what, torch.cat(devs), bound.get(what, 0.0), shapes)
+
+    def _ref_layernorm_split(self, idx, form, shapes, c, a, pre):
+        x = c["x"]
+        C = x.shape[-1]
+        dv = collections.defaultdict(list)
+        for sl in chunks(x.shape[0], x[0].numel() * 8 * 3, x.device):
+            want = F.layer_norm(x[sl].to(F64), (C,), c["gamma"].to(F64), c["beta"].to(F64), c["eps"])
+            self._rows_out(dv, a, sl, want)
+        self._record_rows(idx, "layernorm_split", form, shapes, dv, "layernorm")
+
+    def _ref_layernorm_bwd(self, idx, form, shapes, c, a, pre):
+        x = c["x"]
+        C = x.shape[-1]
+        dx = []
+        dg = torch.zeros(C, dtype=F64, device=x.device)
+        db = torch.zeros_like(dg)
+        for sl in chunks(x.shape[0], x[0].numel() * 8 * 4, x.device):
+            xd = x[sl].to(F64).requires_grad_(True)
+            gd = c["gamma"].to(F64).requires_grad_(True)
+            bd = torch.zeros_like(gd, requires_grad=True)
+            with torch.enable_grad():
+                F.layer_norm(xd, (C,), gd, bd, c["eps"]).backward(c["dy"][sl].to(F64))
+            dx.append(image_devs(a["dx"][sl], xd.grad))
+            dg += gd.grad
+            db += bd.grad
+        b = self.bounds["layernorm_bwd"]
+        self._record(idx, "layernorm_bwd", form, "dx", torch.cat(dx), b, shapes)
+        self._record(idx, "layernorm_bwd", form, "dgamma", image_devs(a["dgamma"][None], dg[None]), b, shapes)
+        self._record(idx, "layernorm_bwd", form, "dbeta", image_devs(a["dbeta"][None], db[None]), b, shapes)
+
+    @staticmethod
+    def _geglu64(u):
+        v, g = u.chunk(2, dim=-1)
+        return v * F.gelu(g)
+
+    def _ref_geglu_split(self, idx, form, shapes, c, a, pre):
+        u = c["u"]
+        dv = collections.defaultdict(list)
+        for sl in chunks(u.shape[0], u[0].numel() * 8 * 3, u.device):
+            self._rows_out(dv, a, sl, self._geglu64(u[sl].to(F64)))
+        self._record_rows(idx, "geglu_split", form, shapes, dv, "geglu")
+
+    def _ref_geglu_bwd(self, idx, form, shapes, c, a, pre):
+        u = c["u"]
+        devs = []
+        for sl in chunks(u.shape[0], u[0].numel() * 8 * 4, u.device):
+            ud = u[sl].to(F64).requires_grad_(True)
+            with torch.enable_grad():
+                self._geglu64(ud).backward(c["dy"][sl].to(F64))
+            devs.append(image_devs(a["du"][sl], ud.grad))
+        self._record(idx, "geglu_bwd", form, "du", torch.cat(devs), self.bounds["geglu_bwd"], shapes)
+
+    # -- optimizer -----------------------------------------------------------------------------------------------
+    def _ref_adam_multi(self, idx, form, shapes, c, a, pre):
+        """Per parameter tensor: one fp64 torch.optim.Adam step from the pre-launch parameter, gradient and moments
+        (state step = step - 1).
+
+        The update dp = p_new - p_old is compared with the fp64 update, relative to the tensor's largest |dp|.  The
+        fp32 parameter cannot hold p_old + dp closer than half its own spacing (at lr 1e-4 that is up to 6e-4 of dp for
+        parameters near 1), so what counts is the distance beyond that half-ulp: a kernel that evaluates the update
+        exactly scores 0, and one whose update is wrong by more than the parameter's fp32 resolution shows."""
+        tab = a["tab"]
+        dp, mo, ema = [], [], []
+        for i, p in enumerate(tab.tensors):
+            g = pre["grads"][i]
+            if g is None:
+                continue
+            o, n = tab.offsets_host[i], tab.numel_host[i]
+            p0 = pre["params"][i]
+            q = torch.nn.Parameter(p0.to(F64))
+            q.grad = g.to(F64)
+            ref = torch.optim.Adam([q], lr=c["lr"], betas=(c["beta1"], c["beta2"]), eps=c["eps"],
+                                   weight_decay=c["weight_decay"], foreach=False)
+            ref.state[q] = {"step": torch.tensor(float(c["step"] - 1)),
+                            "exp_avg": pre["exp_avg"][o:o + n].view(p.shape).to(F64),
+                            "exp_avg_sq": pre["exp_avg_sq"][o:o + n].view(p.shape).to(F64)}
+            ref.step()
+            p1 = p.detach()
+            want = q.detach() - p0.to(F64)
+            spacing = (torch.nextafter(p1.abs(), torch.full_like(p1, math.inf)) - p1.abs()).to(F64)
+            beyond = ((p1.to(F64) - q.detach()).abs() - 0.5 * spacing).clamp_min(0)
+            d = beyond.max() / want.abs().max().clamp_min(1e-30)
+            dp.append(torch.nan_to_num(d, nan=math.inf).reshape(1))
+            st = ref.state[q]
+            mo.append(torch.maximum(image_devs(a["exp_avg"][o:o + n][None], st["exp_avg"].reshape(1, -1)),
+                                    image_devs(a["exp_avg_sq"][o:o + n][None], st["exp_avg_sq"].reshape(1, -1))))
+            if a["ema_shadow"] is not None:
+                s0 = pre["ema_shadow"][o:o + n].to(F64)
+                w = (1.0 - c["ema_decay"]) * p1.reshape(-1).to(F64) + c["ema_decay"] * s0
+                ema.append(image_devs(a["ema_shadow"][o:o + n][None], w[None]))
+        self._record(idx, "adam_multi", form, "dp beyond fp32 resolution", torch.cat(dp), self.bounds["adam_dp"],
+                     shapes)
+        self._record(idx, "adam_multi", form, "exp_avg, exp_avg_sq", torch.cat(mo), self.bounds["adam_moments"], shapes)
+        if ema:
+            self._record(idx, "adam_multi", form, "EMA shadow", torch.cat(ema), self.bounds["ema"], shapes)
+
+    def _ref_ema_multi(self, idx, form, shapes, c, a, pre):
+        tab = a["tab"]
+        devs = []
+        for i, p0 in enumerate(pre["params"]):
+            o, n = tab.offsets_host[i], tab.numel_host[i]
+            w = p0.reshape(-1).to(F64)
+            if c["with_decay"]:
+                w = (1.0 - c["decay"]) * w + c["decay"] * pre["shadow"][o:o + n].to(F64)
+            devs.append(image_devs(a["shadow"][o:o + n][None], w[None]))
+        self._record(idx, "ema_multi", form, "EMA shadow", torch.cat(devs), self.bounds["ema"], shapes)
+
 
 # ------------------------------------------------------------------------------------------------ coverage
 # (method, features that one launch's form must all have, features it must not have).  What the cfg2 routing issues: the
@@ -794,6 +1192,46 @@ CFG2_FORMS = [
 ]
 UPSAMPLE_FORMS = [("conv_umma", ("upsample2x",), ())]
 F43_FORMS = [("wino_input", ("F(4,3)",), ()), ("wino_output", ("F(4,3)",), ())]
+# What one training micro-step of the LBBDM-f4 UNet at batch 32 issues (q_sample, forward, backward, two FusedAdam
+# steps): the F(4,3) training forward (act planes for the weight gradient, fused residual) and data-gradient chain
+# (identity input transform of dY, flipped weight planes), the direct tensor-core forward and data gradient, the
+# resampling operand passes, the gradient split with and without the planes of a direct data gradient, the weight
+# gradients, the GroupNorm backward with and without FiLM and without activation (the attention block's qkv), the
+# attention backward, and Adam's first two steps.  (Every conv of the cfg3 UNet has a bias: the split without column
+# sums comes with the transformer's bias-free projections.)
+TRAIN_FORMS = [
+    ("q_sample", (), ()),
+    ("wino_input", ("F(4,3)", "act planes"), ()),
+    ("wino_output", ("F(4,3)", "res 1"), ()),
+    ("wino_input", ("F(4,3)", "identity"), ()),
+    ("wino_pack_weight", ("F(4,3)", "dgrad"), ()),
+    ("conv_umma", ("taps 9",), ("dgrad",)),
+    ("conv_umma", ("taps 9", "dgrad"), ()),
+    ("conv_umma", ("taps 1",), ()),
+    ("prep", ("resample 1",), ()),
+    ("prep", ("resample 2",), ()),
+    ("split_grad", ("planes", "colsum"), ()),
+    ("split_grad", ("colsum",), ("planes",)),
+    ("conv_wgrad", ("taps 9",), ()),
+    ("conv_wgrad", ("taps 1",), ()),
+    ("conv_direct", (), ()),
+    ("conv_wgrad_direct", (), ()),
+    ("gn_bwd_reduce", ("film",), ()),
+    ("gn_bwd_apply", ("film",), ()),
+    ("gn_bwd_apply", (), ("film", "no act")),
+    ("gn_bwd_apply", ("no act",), ()),
+    ("attention_tc", (), ()),
+    ("attention_bwd", (), ()),
+    ("adam_multi", ("step 1",), ()),
+    ("adam_multi", ("step 2",), ()),
+]
+# ... and with SpatialTransformers: LayerNorm and GEGLU operand passes and their backward, cross-attention and its
+# backward, the k|v projection of the 3-channel context (3 x 2C channel pairs) on the direct weight gradient
+ST_TRAIN_FORMS = TRAIN_FORMS + [
+    ("layernorm_split", (), ()), ("layernorm_bwd", (), ()), ("geglu_split", (), ()), ("geglu_bwd", (), ()),
+    ("attention_cross", (), ()), ("attention_cross_bwd", (), ()),
+    ("conv_wgrad_direct", ("beyond 1024 channel pairs",), ()), ("split_grad", (), ("colsum",)),
+]
 
 
 def missing_forms(shadow, required):

@@ -576,6 +576,32 @@ def test_fused_adam_and_ema_match_torch_over_10_steps():
             assert torch.allclose(sb[k][f], sa[k][f], rtol=1e-5, atol=1e-6), (k, f, rel_dev(sb[k][f], sa[k][f]))
 
 
+def test_fused_adam_moments_match_torch_adam_per_tensor():
+    """exp_avg and exp_avg_sq after the first and second step, per tensor, within fp32 rounding of torch.optim.Adam's
+    at the benchmarks' settings (lr 1e-4, default betas, loss-gradient magnitudes).  The hyper-parameters reach the
+    kernel as doubles: computed from an fp32-rounded beta2, 1 - 0.999 is 1.3e-5 off, and so was exp_avg_sq (found by
+    the training launch shadow on an H100 80GB HBM3; the 10-step test above hides it under its atol)."""
+    import torch.nn as nn
+    from bbdm_b200.optim import FusedAdam
+
+    def make():
+        torch.manual_seed(4)
+        return nn.ParameterList([nn.Parameter(0.02 * torch.randn(s, device=DEV)) for s in [(256, 128, 3, 3), (513,), (1,)]])
+    pa, pb = make(), make()
+    oa, ob = torch.optim.Adam(pa, lr=1e-4), FusedAdam(pb, lr=1e-4)
+    g = torch.Generator(device=DEV).manual_seed(6)
+    for it in range(2):
+        for a, b in zip(pa, pb):
+            gr = 1e-4 * torch.randn(a.shape, device=DEV, generator=g)
+            a.grad, b.grad = gr.clone(), gr.clone()
+        oa.step()
+        ob.step()
+        sa, sb = oa.state_dict()["state"], ob.state_dict()["state"]
+        for k in sa:
+            for f in ("exp_avg", "exp_avg_sq"):
+                assert rel_dev(sb[k][f], sa[k][f]) < 1e-6, (it, k, f, rel_dev(sb[k][f], sa[k][f]))
+
+
 def test_ema_update_bit_exact_vs_reference_expression():
     import torch.nn as nn
     from bbdm_b200.optim import FusedEMA
