@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BBDM_LIB selects another in-tree build of the same sources (A/B experiments, tools/); the product default is fixed
 LIB_PATH = os.environ.get("BBDM_LIB") or os.path.join(_HERE, "libbbdm_b200.so")
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 OBJ = {"grad": 0, "noise": 1, "ysubx": 2}
 RESAMPLE_NONE, RESAMPLE_UP2, RESAMPLE_DOWN2 = 0, 1, 2
 RES_NONE, RES_SAME, RES_UP2, RES_DOWN2 = 0, 1, 2, 3
@@ -75,7 +75,8 @@ class ConvArgs(C.Structure):
                 ("residual", C.c_void_p), ("res_mode", C.c_int),
                 ("out", C.c_void_p), ("out_hi", C.c_void_p), ("out_lo", C.c_void_p),
                 ("passes", C.c_int), ("out_nchw_channels", C.c_int), ("upsample2x", C.c_int),
-                ("stats_partial", C.c_void_p), ("weights_per_image", C.c_int), ("operand_f16", C.c_int)]
+                ("stats_partial", C.c_void_p), ("weights_per_image", C.c_int), ("operand_f16", C.c_int),
+                ("window_origin", C.c_int)]
 
 
 class WinoInputArgs(C.Structure):
@@ -138,7 +139,7 @@ def load():
     lib.bbdm_gn_finalize_partials.argtypes = [vp, i, i, vp, i, i, i, i, i, f, vp, vp, vp]
     lib.bbdm_split_grad.argtypes = [vp, i64, i, vp, vp, vp, vp, vp, vp, vp]
     lib.bbdm_conv_wgrad_workspace.argtypes = [i, i, i, i, i, i, C.POINTER(i), C.POINTER(i64)]
-    lib.bbdm_conv_wgrad.argtypes = [vp, vp, vp, vp, i, i, i, i, i, i, vp, vp, vp]
+    lib.bbdm_conv_wgrad.argtypes = [vp, vp, vp, vp, i, i, i, i, i, i, i, vp, vp, vp]
     lib.bbdm_conv_wgrad_direct.argtypes = [vp, vp, i, i, i, i, i, i, vp, vp, i64, vp]
     lib.bbdm_gn_bwd_reduce.argtypes = [vp, vp, i, i, i, i, i, vp, vp, vp, vp, vp, vp, i64, i, vp, vp, vp]
     lib.bbdm_gn_bwd_apply.argtypes = [vp, vp, i, i, i, i, i, vp, vp, vp, vp, vp, vp, i64, i, vp, vp, vp, vp]
@@ -250,6 +251,9 @@ class CudaBackend:
     wino_tensor_scale = True
     # Winograd output tile sizes: F(4x4,3x3) and F(6x6,3x3) (the wino_* methods' tile argument)
     wino_tiles = (4, 6)
+    # conv_umma / conv_wgrad take window_origin: the 2x2 window of taps = 4 at rows/cols -1..0 as well as 0..1 (the
+    # UNet's stride-2 conv on a space-to-depth operand and the adjoints of it and of the nearest-2x conv)
+    window_origin = True
 
     def __init__(self):
         self.lib = load()
@@ -371,11 +375,12 @@ class CudaBackend:
     def conv_umma(self, *, B, H, W, Cin, Cout, taps, a_hi, a_lo, w_hi, w_lo, bias=None, Cin2=0,
                   a2_hi=None, a2_lo=None, w2_hi=None, w2_lo=None, bias2=None, residual=None,
                   res_mode=RES_NONE, out=None, out_hi=None, out_lo=None, passes=3, out_nchw_channels=0,
-                  stats_partial=None, upsample2x=False, weights_per_image=False, operand_f16=False):
+                  stats_partial=None, upsample2x=False, weights_per_image=False, operand_f16=False, window_origin=0):
+        """window_origin (taps 4): 0 = 2x2 window at rows/cols 0..1, -1 = rows/cols -1..0."""
         a = ConvArgs(B, H, W, Cin, Cout, taps, ptr(a_hi), ptr(a_lo), ptr(w_hi), ptr(w_lo), ptr(bias),
                      Cin2, ptr(a2_hi), ptr(a2_lo), ptr(w2_hi), ptr(w2_lo), ptr(bias2),
                      ptr(residual), res_mode, ptr(out), ptr(out_hi), ptr(out_lo), passes, out_nchw_channels,
-                     int(upsample2x), ptr(stats_partial), int(weights_per_image), int(operand_f16))
+                     int(upsample2x), ptr(stats_partial), int(weights_per_image), int(operand_f16), int(window_origin))
         check(self.lib.bbdm_conv_umma(C.byref(a), stream()))
         LAUNCHES["n"] += 1
 
@@ -524,9 +529,10 @@ class CudaBackend:
         check(self.lib.bbdm_conv_wgrad_workspace(B, H, W, Cin, Cout, taps, C.byref(sp), C.byref(fl)))
         return sp.value, fl.value
 
-    def conv_wgrad(self, g_hi_t, g_lo_t, a_hi, a_lo, B, H, W, Cin, Cout, taps, dw, workspace):
+    def conv_wgrad(self, g_hi_t, g_lo_t, a_hi, a_lo, B, H, W, Cin, Cout, taps, dw, workspace, window_origin=0):
+        """taps 1, 9, or 4 with window_origin 0 / -1 (dw [Cout, Cin, 2, 2])."""
         check(self.lib.bbdm_conv_wgrad(ptr(g_hi_t), ptr(g_lo_t), ptr(a_hi), ptr(a_lo), B, H, W, Cin, Cout, taps,
-                                       ptr(_req(dw)), ptr(_req(workspace)), stream()))
+                                       int(window_origin), ptr(_req(dw)), ptr(_req(workspace)), stream()))
         LAUNCHES["n"] += 2
 
     def conv_wgrad_direct(self, dy, x, k, dw, workspace):

@@ -12,7 +12,7 @@ import os
 import torch
 
 from . import cabi
-from .weights import upsample_phase_weights
+from .weights import stride2_s2d_weights, upsample_phase_weights
 
 # Winograd F(4x4,3x3) for the stride-1 3x3 convs with at least WINO_MIN_C input and output channels (parity mode only;
 # below that the transform traffic outweighs the 4x MAC saving).  BBDM_WINOGRAD=0 disables it in the sampling
@@ -143,7 +143,8 @@ class WeightPacker:
 
     An entry has cout, cin, k, bias, f32 [k*k][Cin][Cout], and split-bf16 hi/lo [k*k][Cout][Cin] when both channel
     counts are multiples of 64.  The caller decides which convs also get a zero-padded head (padded_head), Winograd
-    planes (winograd) or the fused nearest-2x phase planes (up_phase)."""
+    planes (winograd), the fused nearest-2x phase planes (up_phase) or the space-to-depth planes of a stride-2 conv
+    (stride2)."""
 
     def __init__(self, be, device, old=None):
         self.be, self.device, self.old, self.w = be, device, old or {}, {}
@@ -207,6 +208,14 @@ class WeightPacker:
         ent["up_hi"] = self._buf(name, "up_hi", (16, ent["cout"], ent["cin"]), torch.bfloat16)
         ent["up_lo"] = self._buf(name, "up_lo", (16, ent["cout"], ent["cin"]), torch.bfloat16)
         self.be.pack_weight_split_taps(upsample_phase_weights(weight.detach()), ent["up_hi"], ent["up_lo"])
+
+    def stride2(self, name, weight):
+        """The 3x3 stride-2 padding-1 conv ``name`` (UNet Downsample) as a 2x2-tap conv on the space-to-depth operand
+        (bbdm_s2d_split): planes [4][Cout][4*Cin], window at rows/cols -1..0 (conv_umma window_origin -1)."""
+        ent = self.w[name]
+        ent["s2_hi"] = self._buf(name, "s2_hi", (4, ent["cout"], 4 * ent["cin"]), torch.bfloat16)
+        ent["s2_lo"] = self._buf(name, "s2_lo", (4, ent["cout"], 4 * ent["cin"]), torch.bfloat16)
+        self.be.pack_weight_split_taps(stride2_s2d_weights(weight.detach()), ent["s2_hi"], ent["s2_lo"])
 
     def up_phase_winograd(self, name, weight):
         """F(6x6,3x3) planes of nearest-2x + the packed 3x3 conv ``name`` as one 3x3 conv on the low-res map with

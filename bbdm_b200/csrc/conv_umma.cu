@@ -45,6 +45,7 @@ struct ConvParams {
   int K2;           // Cin2 / 64
   int taps;
   int up2;           // 1: fused nearest-2x upsample (4 output phases x 2x2 taps on the low-res input)
+  int origin;        // taps == 4: first row / column of the 2x2 window (0 or -1)
   int w_per_image;   // 1: the weight "tap" index is the image index of the tile (36 Winograd position GEMMs in one launch)
   int kb_per_chunk;  // K blocks accumulated inside wgmma before promotion to the fp32 register accumulator
   const float* bias; const float* bias2;
@@ -316,7 +317,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
               dx = (phase & 1) ? c : c - 1;
               wtap = phase * 4 + tap;
             } else if (p.taps == 9) { dy = tap / 3 - 1; dx = tap % 3 - 1; }
-            else if (p.taps == 4) { dy = tap >> 1; dx = tap & 1; }   // 2x2 window at (0..1, 0..1): zero pad bottom/right
+            else if (p.taps == 4) { dy = (tap >> 1) + p.origin; dx = (tap & 1) + p.origin; }   // 2x2 window at rows/cols
+                                                                     // origin..origin+1: zero fill bottom/right (0) or top/left (-1)
             else if (p.w_per_image) wtap = tb;                       // taps == 1: weights of transform position tb
             tma_load_4d(sbase, &map_a_hi, full, cb * UM_BK, w0 + dx, h0 + dy, b0);
             if (PASSES == 3) tma_load_4d(sbase + OFF_ALO, &map_a_lo, full, cb * UM_BK, w0 + dx, h0 + dy, b0);
@@ -504,6 +506,10 @@ extern "C" int bbdm_conv_umma(const BbdmConvArgs* a, void* stream) {
   BBDM_REQUIRE(a->res_mode >= 0 && a->res_mode <= 3 && (a->res_mode == 0 || a->residual), "conv_umma: bad residual");
   if (a->res_mode == BBDM_RES_UP2 && !a->upsample2x) BBDM_REQUIRE(a->H % 2 == 0 && a->W % 2 == 0, "conv_umma: RES_UP2 needs even H, W");
   BBDM_REQUIRE(a->W >= 4, "conv_umma: W < 4 not supported (use conv_direct)");
+  BBDM_REQUIRE(a->window_origin == 0 || a->window_origin == -1, "conv_umma: window_origin must be 0 or -1 (got %d)",
+               a->window_origin);
+  BBDM_REQUIRE(a->window_origin == 0 || (a->taps == 4 && !a->upsample2x),
+               "conv_umma: window_origin -1 needs taps == 4 and no upsample2x");
   const bool wpi = a->weights_per_image != 0, f16 = a->operand_f16 != 0;
   if (wpi) BBDM_REQUIRE(a->taps == 1 && a->Cin2 == 0 && !a->upsample2x, "conv_umma: weights_per_image needs taps == 1 and no fused operand");
 
@@ -527,6 +533,7 @@ extern "C" int bbdm_conv_umma(const BbdmConvArgs* a, void* stream) {
   p.K2 = a->Cin2 / UM_BK;
   p.taps = a->taps;
   p.up2 = a->upsample2x ? 1 : 0;
+  p.origin = a->window_origin;
   p.w_per_image = wpi ? 1 : 0;
   // chunk length: 4 K-blocks (direct conv, split operands), 8 (single pass).  The Winograd position GEMMs promote
   // more often, because their output transform amplifies the truncation error of the tensor core's accumulator:

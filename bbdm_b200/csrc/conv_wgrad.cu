@@ -2,6 +2,9 @@
 //
 //   dW[tap][co][ci] = sum over pixels p of  dY[p][co] * A[p + tap][ci]
 //
+// taps: 1 (1x1), 9 (3x3 window at offsets -1..1), or 4 (2x2 window at offsets origin..origin+1, origin 0 or -1: the
+// stride-2 3x3 conv on a space-to-depth operand, and its adjoint).
+//
 // GEMM view per filter tap:  M = Cout (tile 128), N = Cin (tile BN), K = pixels (blocks of 64).
 //   * A operand  = dY^T planes [Cout][P] (K-major: 64 consecutive pixels = one 128-byte row), written by
 //     bbdm_split_grad; 2-D TMA map, SWIZZLE_128B.
@@ -21,7 +24,7 @@ constexpr int WG_BK = 64;    // pixels per K block
 constexpr int WG_THREADS = 288;
 
 struct WgradParams {
-  int Cout, Cin, taps;
+  int Cout, Cin, taps, origin;
   int n_co, n_ci;            // tiles along Cout / Cin
   int TW, TH, TB, tiles_w, tiles_h, tiles_b;   // 64-pixel box geometry of a K block
   int kblocks;               // total K blocks (= pixel boxes)
@@ -77,6 +80,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_g_hi, const __grid_con
         const int split = r / p.taps;
         int dy = 0, dx = 0;
         if (p.taps == 9) { dy = tap / 3 - 1; dx = tap % 3 - 1; }
+        else if (p.taps == 4) { dy = (tap >> 1) + p.origin; dx = (tap & 1) + p.origin; }
         const int kb0 = split * p.kb_per_split;
         const int kb1 = kb0 + p.kb_per_split < p.kblocks ? kb0 + p.kb_per_split : p.kblocks;
         for (int kb = kb0; kb < kb1; ++kb) {
@@ -318,7 +322,8 @@ int bbdm_split_grad(const float* src, int64_t P, int C, void* hi, void* lo, void
 }
 
 int bbdm_conv_wgrad_workspace(int B, int H, int W, int Cin, int Cout, int taps, int* splits, int64_t* floats) {
-  BBDM_REQUIRE(B > 0 && H > 0 && W > 0 && Cin % 64 == 0 && Cout % 64 == 0 && (taps == 1 || taps == 9), "wgrad_workspace: bad shape");
+  BBDM_REQUIRE(B > 0 && H > 0 && W > 0 && Cin % 64 == 0 && Cout % 64 == 0 && (taps == 1 || taps == 4 || taps == 9),
+               "wgrad_workspace: bad shape");
   const int64_t P = (int64_t)B * H * W;
   const int64_t kblocks = (P + 63) / 64;
   const int BN = wgrad_bn(Cin);
@@ -333,13 +338,16 @@ int bbdm_conv_wgrad_workspace(int B, int H, int W, int Cin, int Cout, int taps, 
 }
 
 int bbdm_conv_wgrad(const void* g_hi_t, const void* g_lo_t, const void* a_hi, const void* a_lo, int B, int H,
-                    int W, int Cin, int Cout, int taps, float* dw, float* workspace, void* stream) {
+                    int W, int Cin, int Cout, int taps, int window_origin, float* dw, float* workspace, void* stream) {
   BBDM_REQUIRE(g_hi_t && g_lo_t && a_hi && a_lo && dw && workspace, "conv_wgrad: null pointer");
-  BBDM_REQUIRE(Cin % 64 == 0 && Cout % 64 == 0 && (taps == 1 || taps == 9) && W >= 4, "conv_wgrad: unsupported shape");
+  BBDM_REQUIRE(Cin % 64 == 0 && Cout % 64 == 0 && (taps == 1 || taps == 4 || taps == 9) && W >= 4,
+               "conv_wgrad: unsupported shape");
+  BBDM_REQUIRE(window_origin == 0 || (taps == 4 && window_origin == -1),
+               "conv_wgrad: window_origin -1 needs taps == 4 (got origin %d, taps %d)", window_origin, taps);
   const int64_t P = (int64_t)B * H * W;
   BBDM_REQUIRE(P % 64 == 0 && (P * 2) % 16 == 0, "conv_wgrad: B*H*W must be a multiple of 64");
   WgradParams p;
-  p.Cout = Cout; p.Cin = Cin; p.taps = taps;
+  p.Cout = Cout; p.Cin = Cin; p.taps = taps; p.origin = window_origin;
   // 64-pixel box: as wide as possible in w, then h, then b (same order as the flattened pixel index)
   int tw = 1; while (tw * 2 <= W && tw * 2 <= 64 && W % (tw * 2) == 0) tw *= 2;
   int th = 1; while (tw * th * 2 <= 64 && th * 2 <= H && H % (th * 2) == 0) th *= 2;

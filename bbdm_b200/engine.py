@@ -122,10 +122,11 @@ class KernelExecutor:
 
     def _conv(self, pool, ent, *, a_f32=None, a_hi=None, a_lo=None, shape, bias=None, residual=None,
               res_mode=cabi.RES_NONE, second=None, out_split=False, want_f32=True, stride=1, out=None,
-              stats=False, planes=None, taps=None, upsample2x=False):
+              stats=False, planes=None, taps=None, upsample2x=False, window_origin=0):
         """One convolution.  shape = (B,H,W) of the INPUT; returns (out_f32, out_hi, out_lo).  On the tensor-core
-        path planes = (w_hi, w_lo) [taps][Cout][Cin] replaces the entry's hi/lo (e.g. its up-phase planes), and
-        upsample2x runs the fused nearest-2x conv (output at twice the input's resolution)."""
+        path planes = (w_hi, w_lo) [taps][Cout][Cin] replaces the entry's hi/lo (e.g. its up-phase planes),
+        upsample2x runs the fused nearest-2x conv (output at twice the input's resolution), and window_origin -1 puts
+        a 4-tap conv's 2x2 window at rows/cols -1..0."""
         B, H, W = shape
         bias = ent["bias"] if bias is None else bias
         if a_hi is not None:
@@ -139,10 +140,10 @@ class KernelExecutor:
             oh = ol = None
             if out_split:
                 oh, ol = pool.get(oshape, torch.bfloat16), pool.get(oshape, torch.bfloat16)
-            kw = {}
+            kw = {} if not window_origin else dict(window_origin=window_origin)
             if second is not None:
                 e2, r_hi, r_lo = second
-                kw = dict(Cin2=e2["cin"], a2_hi=r_hi, a2_lo=r_lo, w2_hi=e2["hi"], w2_lo=e2["lo"], bias2=e2["bias"])
+                kw.update(Cin2=e2["cin"], a2_hi=r_hi, a2_lo=r_lo, w2_hi=e2["hi"], w2_lo=e2["lo"], bias2=e2["bias"])
             part = None
             if stats and out is not None:
                 rows = f * f * self._geom(H, W)
@@ -489,6 +490,11 @@ class UNetEngine(KernelExecutor):
                 low = sizes[name] // 2
                 if self.wino and 6 in getattr(be, "wino_tiles", (4,)) and convs.wino_tile(low, low) == 6:
                     packer.up_phase_winograd(name + ".in_layers.2", m.in_layers[2].weight)
+        if getattr(be, "window_origin", False):
+            for name, m in u.named_modules():
+                if isinstance(m, Downsample) and m.use_conv and m.channels % 64 == 0 and m.out_channels % 64 == 0:
+                    # Downsample conv: 2x2 taps on the space-to-depth operand instead of the fp32 stride-2 kernel
+                    packer.stride2(name + ".op", m.op.weight)
         if old and old.get("film_n") == off and old["film_w"].device == dev:
             w["film_w"], w["film_b"] = old["film_w"], old["film_b"]
             torch.cat(film_w, 0, out=w["film_w"])
@@ -677,7 +683,19 @@ class UNetEngine(KernelExecutor):
             return self._upsample(pool, x, self._w[name + ".conv"] if m.use_conv else None)
         if not m.use_conv:
             return self._avg_pool2(pool, x)
-        out, _, _ = self._conv(pool, self._w[name + ".op"], a_f32=x, shape=x.shape[:3], stride=2)
+        ent = self._w[name + ".op"]
+        B, H, W, Cc = x.shape
+        if "s2_hi" in ent and H % 2 == 0 and W % 2 == 0 and W // 2 >= 4:
+            # stride-2 conv on the tensor cores: space-to-depth split, then the 2x2-tap conv at origin -1 on the
+            # half-resolution grid, GroupNorm partial sums of the result in its epilogue
+            hi = pool.get((B, H // 2, W // 2, 4 * Cc), torch.bfloat16)
+            lo = pool.get((B, H // 2, W // 2, 4 * Cc), torch.bfloat16)
+            self.be.s2d_split(x, hi, lo)
+            out, _, _ = self._conv(pool, ent, a_hi=hi, a_lo=lo, shape=(B, H // 2, W // 2),
+                                   planes=(ent["s2_hi"], ent["s2_lo"]), taps=4, stats=True, window_origin=-1)
+            pool.put(hi, lo)
+            return out
+        out, _, _ = self._conv(pool, ent, a_f32=x, shape=x.shape[:3], stride=2)
         return out
 
     def _run_block(self, pool, prefix, block: TimestepEmbedSequential, h, skip, film, release_input):

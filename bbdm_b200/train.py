@@ -17,6 +17,8 @@ from __future__ import annotations
 import torch
 
 from . import cabi, convs
+from .weights import (stride2_dgrad_weights, stride2_fold_wgrad, stride2_s2d_weights, upsample_dgrad_weights,
+                      upsample_fold_wgrad, upsample_phase_weights)
 
 _BACKEND = None
 
@@ -70,6 +72,10 @@ def _tc_ok(x: torch.Tensor, cin: int, cout: int) -> bool:
     if not _on_device(x) or x.dtype != torch.float32 or x.dim() != 4:
         return False
     B, _, H, W = x.shape
+    return _tc_grid_ok(B, H, W, cin, cout)
+
+
+def _tc_grid_ok(B, H, W, cin, cout):
     return cin % 64 == 0 and cout % 64 == 0 and W >= 4 and (B * H * W) % 64 == 0 and _box64_ok(B, H, W)
 
 
@@ -188,6 +194,178 @@ def _conv_backward(be, ctx_shape, a_hi, a_lo, weight, dy, need_dx, need_dw, need
         dw = torch.empty((Cout, Cin, k, k), dtype=torch.float32, device=dev)
         be.conv_wgrad(gt_hi, gt_lo, a_hi, a_lo, B, H, W, Cin, Cout, k * k, dw, ws)
     return dxn, dw, dbias
+
+
+def _pack_taps(be, w, dev):
+    """w [Cout', Cin', taps] fp32 -> split planes [taps][Cout'][Cin']."""
+    hi = torch.empty((w.shape[2], w.shape[0], w.shape[1]), dtype=torch.bfloat16, device=dev)
+    lo = torch.empty_like(hi)
+    be.pack_weight_split_taps(w, hi, lo)
+    return hi, lo
+
+
+def _split_dy(be, dyn, need_dx, need_db):
+    """dY [B, H, W, C] fp32 (contiguous) -> split planes (g_hi, g_lo) [B, H, W, C] if need_dx, the transposed planes
+    (gt_hi, gt_lo) [C][P] of the weight-gradient GEMM, and the column sums [C] if need_db."""
+    B, H, W, Cc = dyn.shape
+    P, dev = B * H * W, dyn.device
+    g_hi = g_lo = dsum = ws = None
+    if need_dx:
+        g_hi = torch.empty(dyn.shape, dtype=torch.bfloat16, device=dev)
+        g_lo = torch.empty_like(g_hi)
+    gt_hi = torch.empty((Cc, P), dtype=torch.bfloat16, device=dev)
+    gt_lo = torch.empty_like(gt_hi)
+    if need_db:
+        dsum = torch.empty((Cc,), dtype=torch.float32, device=dev)
+        ws = torch.empty(((P + 63) // 64) * Cc, dtype=torch.float32, device=dev)
+    be.split_grad(dyn, g_hi, g_lo, gt_hi, gt_lo, dsum, ws)
+    return g_hi, g_lo, gt_hi, gt_lo, dsum
+
+
+def _wgrad(be, gt_hi, gt_lo, a_hi, a_lo, B, H, W, Cin, Cout, taps, window_origin=0):
+    """conv_wgrad into a fresh [Cout, Cin, k, k] tensor (k = 2 for taps 4)."""
+    dev = gt_hi.device
+    _, fl = be.wgrad_workspace(B, H, W, Cin, Cout, taps)
+    ws = torch.empty((fl,), dtype=torch.float32, device=dev)
+    k = {1: 1, 4: 2, 9: 3}[taps]
+    dw = torch.empty((Cout, Cin, k, k), dtype=torch.float32, device=dev)
+    be.conv_wgrad(gt_hi, gt_lo, a_hi, a_lo, B, H, W, Cin, Cout, taps, dw, ws, window_origin=window_origin)
+    return dw
+
+
+class Stride2Conv2dFn(torch.autograd.Function):
+    """3x3 conv, stride 2, padding 1 (the UNet Downsample, openaimodel.py:137-163) on the tensor cores.  With the
+    space-to-depth operand x' (bbdm_s2d_split: 4*Cin phase-major channels on the H/2 x W/2 grid) it is a 2x2-tap conv
+    whose window sits at rows/cols -1..0 (weights.stride2_s2d_weights):
+      forward          conv_umma, taps 4, window_origin -1, over x'
+      data gradient    the transposed, tap-flipped 2x2 conv over dY (window_origin 0) gives dx', depth-to-space dx
+      weight gradient  conv_wgrad, taps 4, window_origin -1, over (x', dY), folded back to [Cout][Cin][3][3]
+      bias gradient    the column sums of dY (bbdm_split_grad)
+    x: [B, Cin, H, W] with H, W even -> [B, Cout, H/2, W/2] (channels_last strides)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias):
+        be = backend()
+        B, Cin, H, W = x.shape
+        Cout = weight.shape[0]
+        Ho, Wo = H // 2, W // 2
+        dev = x.device
+        xn = _nhwc(x.detach()).contiguous()
+        a_hi = torch.empty((B, Ho, Wo, 4 * Cin), dtype=torch.bfloat16, device=dev)
+        a_lo = torch.empty_like(a_hi)
+        be.s2d_split(xn, a_hi, a_lo)
+        w_hi, w_lo = _pack_taps(be, stride2_s2d_weights(weight.detach()), dev)
+        out = torch.empty((B, Ho, Wo, Cout), dtype=torch.float32, device=dev)
+        be.conv_umma(B=B, H=Ho, W=Wo, Cin=4 * Cin, Cout=Cout, taps=4, a_hi=a_hi, a_lo=a_lo, w_hi=w_hi, w_lo=w_lo,
+                     bias=None if bias is None else bias.detach(), out=out, passes=3, window_origin=-1)
+        ctx.save_for_backward(a_hi, a_lo, weight)
+        ctx.has_bias = bias is not None
+        return out.permute(0, 3, 1, 2)
+
+    @staticmethod
+    def backward(ctx, dy):
+        be = backend()
+        a_hi, a_lo, weight = ctx.saved_tensors
+        B, Ho, Wo, Cin4 = a_hi.shape
+        Cin, Cout = Cin4 // 4, weight.shape[0]
+        dev = dy.device
+        need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        need_db = ctx.has_bias and ctx.needs_input_grad[2]
+        g_hi, g_lo, gt_hi, gt_lo, db = _split_dy(be, _nhwc(dy).contiguous(), need_dx, need_db)
+        dx = dw = None
+        if need_dx:
+            wd_hi, wd_lo = _pack_taps(be, stride2_dgrad_weights(weight.detach()), dev)
+            dxs = torch.empty((B, Ho, Wo, Cin4), dtype=torch.float32, device=dev)
+            be.conv_umma(B=B, H=Ho, W=Wo, Cin=Cout, Cout=Cin4, taps=4, a_hi=g_hi, a_lo=g_lo, w_hi=wd_hi, w_lo=wd_lo,
+                         out=dxs, passes=3)
+            # depth-to-space: channel (a*2 + b)*Cin + ci of pixel (i, j) -> pixel (2i + a, 2j + b)
+            dxn = dxs.view(B, Ho, Wo, 2, 2, Cin).permute(0, 1, 3, 2, 4, 5).reshape(B, 2 * Ho, 2 * Wo, Cin)
+            dx = dxn.permute(0, 3, 1, 2)
+        if need_dw:
+            dw = stride2_fold_wgrad(_wgrad(be, gt_hi, gt_lo, a_hi, a_lo, B, Ho, Wo, Cin4, Cout, 4, window_origin=-1))
+        return dx, dw, db
+
+
+class Up2Conv2dFn(torch.autograd.Function):
+    """Nearest-2x upsample followed by a 3x3 'same' conv (the UNet Upsample, openaimodel.py:93-121) on the tensor
+    cores, never materialising the upsampled tensor:
+      forward          the fused 4-phase conv (conv_umma upsample2x, weights.upsample_phase_weights) on x
+      data gradient    a stride-1 3x3 conv on the low-res grid over dY' = space-to-depth(dY) (4*Cout channels)
+      weight gradient  conv_wgrad, taps 9, over (x, dY'), folded back to [Cout][Cin][3][3]
+      bias gradient    the column sums of dY' summed over the 4 phases
+    (weights.upsample_dgrad_weights / upsample_fold_wgrad).  x: [B, Cin, H, W] -> [B, Cout, 2H, 2W]."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias):
+        be = backend()
+        B, Cin, H, W = x.shape
+        Cout = weight.shape[0]
+        dev = x.device
+        xn = _nhwc(x.detach())
+        a_hi = torch.empty((B, H, W, Cin), dtype=torch.bfloat16, device=dev)
+        a_lo = torch.empty_like(a_hi)
+        be.prep(xn, None, raw_hi=a_hi, raw_lo=a_lo)
+        w_hi, w_lo = _pack_taps(be, upsample_phase_weights(weight.detach()), dev)
+        out = torch.empty((B, 2 * H, 2 * W, Cout), dtype=torch.float32, device=dev)
+        be.conv_umma(B=B, H=H, W=W, Cin=Cin, Cout=Cout, taps=4, a_hi=a_hi, a_lo=a_lo, w_hi=w_hi, w_lo=w_lo,
+                     bias=None if bias is None else bias.detach(), out=out, passes=3, upsample2x=True)
+        ctx.save_for_backward(a_hi, a_lo, weight)
+        ctx.has_bias = bias is not None
+        return out.permute(0, 3, 1, 2)
+
+    @staticmethod
+    def backward(ctx, dy):
+        be = backend()
+        a_hi, a_lo, weight = ctx.saved_tensors
+        B, H, W, Cin = a_hi.shape
+        Cout = weight.shape[0]
+        dev = dy.device
+        need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        need_db = ctx.has_bias and ctx.needs_input_grad[2]
+        # space-to-depth of dY: pixel (2i + a, 2j + b), channel co -> pixel (i, j), channel (a*2 + b)*Cout + co
+        dys = _nhwc(dy).reshape(B, H, 2, W, 2, Cout).permute(0, 1, 3, 2, 4, 5).reshape(B, H, W, 4 * Cout)
+        g_hi, g_lo, gt_hi, gt_lo, db4 = _split_dy(be, dys.contiguous(), need_dx, need_db)
+        dx = dw = db = None
+        if need_dx:
+            wd_hi, wd_lo = _pack_taps(be, upsample_dgrad_weights(weight.detach()), dev)
+            dxn = torch.empty((B, H, W, Cin), dtype=torch.float32, device=dev)
+            be.conv_umma(B=B, H=H, W=W, Cin=4 * Cout, Cout=Cin, taps=9, a_hi=g_hi, a_lo=g_lo, w_hi=wd_hi, w_lo=wd_lo,
+                         out=dxn, passes=3)
+            dx = dxn.permute(0, 3, 1, 2)
+        if need_dw:
+            dw = upsample_fold_wgrad(_wgrad(be, gt_hi, gt_lo, a_hi, a_lo, B, H, W, Cin, 4 * Cout, 9))
+        if need_db:
+            db = db4.view(4, Cout).sum(0)
+        return dx, dw, db
+
+
+def _resample_ok(x, cin, cout):
+    """Operand checks shared by the resampling convs: a backend with the 2x2 window origin, fp32 [B, C, H, W] on the
+    device."""
+    return (_on_device(x) and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == cin
+            and getattr(backend(), "window_origin", False))
+
+
+def downsample_conv(conv: torch.nn.Conv2d, x: torch.Tensor, enabled: bool = True):
+    """The Downsample's 3x3 stride-2 padding-1 conv on Stride2Conv2dFn, or None where the kernels do not take the
+    shape (Cin, Cout multiples of 64, H and W even, and the half-resolution grid one the tensor-core kernels cover)."""
+    if not (enabled and _resample_ok(x, conv.in_channels, conv.out_channels)):
+        return None
+    B, Cin, H, W = x.shape
+    if Cin % 64 or H % 2 or W % 2 or not _tc_grid_ok(B, H // 2, W // 2, 4 * Cin, conv.out_channels):
+        return None
+    return Stride2Conv2dFn.apply(x, conv.weight, conv.bias)
+
+
+def upsample_conv(conv: torch.nn.Conv2d, x: torch.Tensor, enabled: bool = True):
+    """conv(nearest-2x(x)) of the Upsample on Up2Conv2dFn, or None where the kernels do not take the shape (Cin, Cout
+    multiples of 64 and a low-res grid the tensor-core kernels cover)."""
+    if not (enabled and _resample_ok(x, conv.in_channels, conv.out_channels)):
+        return None
+    B, Cin, H, W = x.shape
+    if not _tc_grid_ok(B, H, W, Cin, conv.out_channels):
+        return None
+    return Up2Conv2dFn.apply(x, conv.weight, conv.bias)
 
 
 class GNActConv2dFn(torch.autograd.Function):

@@ -28,7 +28,8 @@ import torch.nn.functional as F
 
 from .transformer import SpatialTransformer
 from .train import (attention_core as _attention_core, conv1x1 as _conv1x1, conv2d as _conv2d,
-                    gn_act_conv2d as _gn_act_conv2d, gn_conv1x1 as _gn_conv1x1)
+                    downsample_conv as _downsample_conv, gn_act_conv2d as _gn_act_conv2d, gn_conv1x1 as _gn_conv1x1,
+                    upsample_conv as _upsample_conv)
 
 # training path: ResBlock convolutions on the wgmma fwd / dgrad / wgrad kernels (bbdm_b200/train.py);
 # set False to run the whole training graph on stock PyTorch kernels
@@ -88,6 +89,11 @@ class Upsample(nn.Module):
             self.conv = nn.Conv2d(self.channels, self.out_channels, 3, padding=1)
 
     def forward(self, x):
+        if self.use_conv and NATIVE_TRAIN_CONV:
+            # nearest-2x + conv as one tensor-core Function (no upsampled copy) where the shape qualifies
+            y = _upsample_conv(self.conv, x)
+            if y is not None:
+                return y
         x = F.interpolate(x, scale_factor=2, mode="nearest")
         return self.conv(x) if self.use_conv else x
 
@@ -105,6 +111,10 @@ class Downsample(nn.Module):
             self.op = nn.AvgPool2d(2, 2)
 
     def forward(self, x):
+        if self.use_conv and NATIVE_TRAIN_CONV:
+            y = _downsample_conv(self.op, x)          # stride-2 conv on the tensor cores where the shape qualifies
+            if y is not None:
+                return y
         return self.op(x)
 
 

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define BBDM_ABI_VERSION 5
+#define BBDM_ABI_VERSION 6
 
 enum {
   BBDM_OK = 0,
@@ -188,9 +188,9 @@ enum { BBDM_RES_NONE = 0, BBDM_RES_SAME = 1, BBDM_RES_UP2 = 2, BBDM_RES_DOWN2 = 
  * TMA (4-D tiled maps, OOB zero fill = the conv padding), accumulate in wgmma register fragments (fp32).
  * passes = 3: A_hi.W_hi + A_lo.W_hi + A_hi.W_lo  (fp32-class accuracy, the parity mode)
  * passes = 1: A_hi.W_hi                           (plain bf16)
- * Requirements: Cin % 64 == 0, Cin2 % 64 == 0, Cout % 64 == 0, taps in {1, 9}, or 4 (2x2 window at rows/cols (0..1), zero
- * padding bottom/right -- the stride-2 conv on a space-to-depth operand, bbdm_s2d_split; with upsample2x the 4 taps
- * are per output phase), W >= 4.
+ * Requirements: Cin % 64 == 0, Cin2 % 64 == 0, Cout % 64 == 0, taps in {1, 9}, or 4 (2x2 window at rows/cols
+ * window_origin..window_origin+1 -- the stride-2 conv on a space-to-depth operand, bbdm_s2d_split; with upsample2x the
+ * 4 taps are per output phase), W >= 4.
  * Replaces nn.Conv2d 3x3 / 1x1 in ResBlock (openaimodel.py:207,233,244), the qkv / proj_out
  * nn.Conv1d of AttentionBlock (:307,315) and the residual adds (:278,327). */
 typedef struct {
@@ -227,6 +227,11 @@ typedef struct {
                                  transform positions of the Winograd path, bbdm_wino_*).  Needs H*W >= 128.  */
   int operand_f16;            /* 1: every operand plane is IEEE fp16 (hi = fp16(x), lo = fp16(x - hi)) instead of
                                  bf16 -- 22 instead of 16 mantissa bits, values must stay below 65504        */
+  int window_origin;          /* taps == 4 without upsample2x: first row / column of the 2x2 window.  0: rows/cols 0..1,
+                                 zero fill at the bottom/right (the VQGAN Downsample's (0,1,0,1) padding, and the data
+                                 gradient of the UNet's stride-2 conv); -1: rows/cols -1..0, zero fill at the top/left
+                                 (the UNet Downsample, 3x3 stride 2 padding 1, openaimodel.py:137-163, on the
+                                 space-to-depth operand).  Must be 0 otherwise.                                    */
 } BbdmConvArgs;
 int bbdm_conv_umma(const BbdmConvArgs* a, void* stream);
 
@@ -378,10 +383,12 @@ int bbdm_conv_wgrad_workspace(int B, int H, int W, int Cin, int Cout, int taps, 
 /* dW[co][ci][ky][kx] (OIHW fp32, overwritten) = sum_p dY[p][co] * A[p + tap][ci] on wgmma:
  * g_hi_t/g_lo_t = dY^T planes [Cout][P] from bbdm_split_grad, a_hi/a_lo = the forward conv's
  * operand planes [B,H,W,Cin].  M = Cout, N = Cin, K = pixels; split-bf16 x3; split-K partials
- * reduced in a fixed order.  Requirements: Cin, Cout % 64 == 0, taps in {1, 9}, B*H*W % 64 == 0. */
+ * reduced in a fixed order.  Requirements: Cin, Cout % 64 == 0, taps in {1, 9} (window_origin 0), or 4 (2x2 window at
+ * rows/cols window_origin..window_origin+1, window_origin 0 or -1, as in BbdmConvArgs; dw is then [Cout][Cin][2][2]),
+ * B*H*W % 64 == 0. */
 int bbdm_conv_wgrad(const void* g_hi_t, const void* g_lo_t, const void* a_hi, const void* a_lo,
-                    int B, int H, int W, int Cin, int Cout, int taps, float* dw, float* workspace,
-                    void* stream);
+                    int B, int H, int W, int Cin, int Cout, int taps, int window_origin, float* dw,
+                    float* workspace, void* stream);
 
 /* Weight gradient of the small-channel fp32 convolutions (UNet stem / head, the SpatialTransformer's k|v
  * projection of the few-channel context; Cin*Cout <= 2^24):
