@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BBDM_LIB selects another in-tree build of the same sources (A/B experiments, tools/); the product default is fixed
 LIB_PATH = os.environ.get("BBDM_LIB") or os.path.join(_HERE, "libbbdm_b200.so")
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 OBJ = {"grad": 0, "noise": 1, "ysubx": 2}
 RESAMPLE_NONE, RESAMPLE_UP2, RESAMPLE_DOWN2 = 0, 1, 2
 RES_NONE, RES_SAME, RES_UP2, RES_DOWN2 = 0, 1, 2, 3
@@ -137,9 +137,9 @@ def load():
     lib.bbdm_attention.argtypes = [vp, i, i, i, i, i, vp, vp, vp, vp]
     lib.bbdm_conv_umma_geometry.argtypes = [i, i, C.POINTER(i), C.POINTER(i), C.POINTER(i), C.POINTER(i)]
     lib.bbdm_gn_finalize_partials.argtypes = [vp, i, i, vp, i, i, i, i, i, f, vp, vp, vp]
-    lib.bbdm_split_grad.argtypes = [vp, i64, i, vp, vp, vp, vp, vp, vp, vp]
+    lib.bbdm_split_grad.argtypes = [vp, i64, i, vp, vp, vp, vp, i64, vp, vp, vp]
     lib.bbdm_conv_wgrad_workspace.argtypes = [i, i, i, i, i, i, C.POINTER(i), C.POINTER(i64)]
-    lib.bbdm_conv_wgrad.argtypes = [vp, vp, vp, vp, i, i, i, i, i, i, i, vp, vp, vp]
+    lib.bbdm_conv_wgrad.argtypes = [vp, vp, i64, vp, vp, i, i, i, i, i, i, i, vp, vp, vp]
     lib.bbdm_conv_wgrad_direct.argtypes = [vp, vp, i, i, i, i, i, i, vp, vp, i64, vp]
     lib.bbdm_gn_bwd_reduce.argtypes = [vp, vp, i, i, i, i, i, vp, vp, vp, vp, vp, vp, i64, i, vp, vp, vp]
     lib.bbdm_gn_bwd_apply.argtypes = [vp, vp, i, i, i, i, i, vp, vp, vp, vp, vp, vp, i64, i, vp, vp, vp, vp]
@@ -236,6 +236,13 @@ LAUNCHES = {"n": 0}
 def _req(t, dtype=torch.float32):
     assert t.is_cuda and t.is_contiguous() and t.dtype == dtype, (t.device, t.dtype, t.is_contiguous())
     return t
+
+
+def _pitch(hi_t, lo_t, rows, cols):
+    """Row pitch (elements) of a pair of transposed [rows, cols] planes whose rows may be padded."""
+    assert hi_t.is_cuda and tuple(hi_t.shape) == (rows, cols) and hi_t.stride(1) == 1, (hi_t.shape, hi_t.stride())
+    assert lo_t.shape == hi_t.shape and lo_t.stride() == hi_t.stride(), (hi_t.stride(), lo_t.stride())
+    return hi_t.stride(0)
 
 
 @_guard_all
@@ -519,8 +526,10 @@ class CudaBackend:
 
     # -- training gradients -----------------------------------------------------------------------
     def split_grad(self, src, hi, lo, hi_t, lo_t, colsum=None, workspace=None):
+        """hi_t / lo_t: [C, P], rows possibly padded (train._transposed_planes)."""
         P, Cc = src.numel() // src.shape[-1], src.shape[-1]
-        check(self.lib.bbdm_split_grad(ptr(_req(src)), P, Cc, ptr(hi), ptr(lo), ptr(hi_t), ptr(lo_t), ptr(colsum),
+        ld = _pitch(hi_t, lo_t, Cc, P)
+        check(self.lib.bbdm_split_grad(ptr(_req(src)), P, Cc, ptr(hi), ptr(lo), ptr(hi_t), ptr(lo_t), ld, ptr(colsum),
                                        ptr(workspace), stream()))
         LAUNCHES["n"] += 1 + (colsum is not None)
 
@@ -531,7 +540,8 @@ class CudaBackend:
 
     def conv_wgrad(self, g_hi_t, g_lo_t, a_hi, a_lo, B, H, W, Cin, Cout, taps, dw, workspace, window_origin=0):
         """taps 1, 9, or 4 with window_origin 0 / -1 (dw [Cout, Cin, 2, 2])."""
-        check(self.lib.bbdm_conv_wgrad(ptr(g_hi_t), ptr(g_lo_t), ptr(a_hi), ptr(a_lo), B, H, W, Cin, Cout, taps,
+        ld = _pitch(g_hi_t, g_lo_t, Cout, B * H * W)
+        check(self.lib.bbdm_conv_wgrad(ptr(g_hi_t), ptr(g_lo_t), ld, ptr(a_hi), ptr(a_lo), B, H, W, Cin, Cout, taps,
                                        int(window_origin), ptr(_req(dw)), ptr(_req(workspace)), stream()))
         LAUNCHES["n"] += 2
 

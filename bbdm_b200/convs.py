@@ -1,5 +1,5 @@
 """Convolution decisions shared by the UNet and VQGAN executors (engine.py, vqgan_engine.py) and the training
-Functions (train.py): when a 3x3 conv takes the Winograd path, the Winograd launch sequence itself, and the packed
+Functions (train.py): which convs run on the tensor cores, when a 3x3 conv takes the Winograd path, the Winograd launch sequence itself, and the packed
 weight planes the executors cache.
 
 A leaf module (torch, cabi and the torch-only weights helper): train.py is imported by unet.py, which engine.py
@@ -25,6 +25,14 @@ WINO_MIN_C = int(os.environ.get("BBDM_WINO_MIN_C", "256"))
 # ... and at least this many 4x4 tiles per launch: below it the 36 position GEMMs have too few M tiles each
 # (measured: cfg1, 256 tiles, graph replay 3.9 -> 4.4 ms with Winograd; cfg3, 2048 tiles, 20.2 -> 17.1 ms)
 WINO_MIN_TILES = int(os.environ.get("BBDM_WINO_MIN_TILES", "512"))
+
+
+def tensor_core_ok(cin, cout, w):
+    """Convolutions the tensor-core kernels take, in sampling (bbdm_conv_umma) and in training (its data gradient and
+    bbdm_conv_wgrad): channel counts that are multiples of 64 and a map at least 4 pixels wide.  Any height and batch:
+    the forward covers ragged map edges with zero-filled tile boxes, the weight gradient reads its 64-pixel K blocks in
+    TMA im2col mode wherever they wrap across rows and images."""
+    return cin % 64 == 0 and cout % 64 == 0 and w >= 4
 
 
 def wino_channels_ok(cin, cout, min_c, tile=4):

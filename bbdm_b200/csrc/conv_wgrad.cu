@@ -6,11 +6,14 @@
 // stride-2 3x3 conv on a space-to-depth operand, and its adjoint).
 //
 // GEMM view per filter tap:  M = Cout (tile 128), N = Cin (tile BN), K = pixels (blocks of 64).
-//   * A operand  = dY^T planes [Cout][P] (K-major: 64 consecutive pixels = one 128-byte row), written by
-//     bbdm_split_grad; 2-D TMA map, SWIZZLE_128B.
-//   * B operand  = the forward conv's input planes [B,H,W,Cin]: the same shifted 64-pixel box the
-//     forward kernel loads (4-D TMA map, OOB zero fill = padding), consumed as an MN-major operand
-//     (channels contiguous); BN/64 swizzle atoms side by side, LBO = one atom (8 KiB).
+//   * A operand  = dY^T planes [Cout][P] with a row pitch of ld_g >= P pixels (K-major: 64 consecutive pixels = one
+//     128-byte row), written by bbdm_split_grad; 2-D TMA map, SWIZZLE_128B, OOB zero fill past pixel P.
+//   * B operand  = the forward conv's input planes [B,H,W,Cin], loaded in TMA im2col mode: K block kb is the pixels
+//     [64 kb, 64 kb + 64) of the flattened (b, h, w) index, wherever the run wraps across rows or images, each read
+//     at the filter tap's offset (the im2col offsets; OOB zero fill = the conv padding and everything past the last
+//     image).  64 channels per pixel = one 128-byte SWIZZLE_128B row, so the shared-memory image is the one a
+//     tiled box of the same 64 pixels gives.  Consumed as an MN-major operand (channels contiguous); BN/64 swizzle
+//     atoms side by side, LBO = one atom (8 KiB).
 //   * two consumer warpgroups (couts 0-63 / 64-127 of the tile) + one TMA producer warp; split-bf16 x3
 //     products, chunked wgmma -> fp32-register promotion (as conv_umma.cu).
 //   * K is split across CTAs (the pixel range); every CTA writes its partial [split][tap][Cout][Cin]
@@ -26,8 +29,9 @@ constexpr int WG_THREADS = 288;
 struct WgradParams {
   int Cout, Cin, taps, origin;
   int n_co, n_ci;            // tiles along Cout / Cin
-  int TW, TH, TB, tiles_w, tiles_h, tiles_b;   // 64-pixel box geometry of a K block
-  int kblocks;               // total K blocks (= pixel boxes)
+  int H, W;                  // map geometry (the K block's first pixel -> im2col coordinates)
+  int lo;                    // im2col bounding-box corner: the window's first row / column offset (-1, 0)
+  int kblocks;               // total K blocks = ceil(P / 64)
   int splits, kb_per_split;
   int kb_per_chunk;
   float* partial;            // [splits][taps][Cout][Cin]
@@ -78,17 +82,16 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_g_hi, const __grid_con
         const int co_t = r % p.n_co; r /= p.n_co;
         const int tap = r % p.taps;
         const int split = r / p.taps;
-        int dy = 0, dx = 0;
-        if (p.taps == 9) { dy = tap / 3 - 1; dx = tap % 3 - 1; }
-        else if (p.taps == 4) { dy = (tap >> 1) + p.origin; dx = (tap & 1) + p.origin; }
+        // tap offset within the window, counted from its first row / column (the map's bounding-box corner p.lo)
+        uint16_t oy = 0, ox = 0;
+        if (p.taps == 9) { oy = (uint16_t)(tap / 3); ox = (uint16_t)(tap % 3); }
+        else if (p.taps == 4) { oy = (uint16_t)(tap >> 1); ox = (uint16_t)(tap & 1); }
         const int kb0 = split * p.kb_per_split;
         const int kb1 = kb0 + p.kb_per_split < p.kblocks ? kb0 + p.kb_per_split : p.kblocks;
         for (int kb = kb0; kb < kb1; ++kb) {
-          int mt = kb;
-          const int tw = mt % p.tiles_w; mt /= p.tiles_w;
-          const int th = mt % p.tiles_h;
-          const int tb = mt / p.tiles_h;
-          mbar_wait(bar_empty + 8 * stage, phase ^ 1, abort_flag, p.fault, 0xC1000000ull | (unsigned)kb);
+          const int px = kb * WG_BK;                   // first pixel of the K block
+          const int pw = px % p.W, ph = (px / p.W) % p.H, pb = px / (p.W * p.H);
+          mbar_wait(bar_empty + 8 * stage, phase ^ 1, abort_flag, p.fault, 0xC5000000ull | (unsigned)kb);
           const uint32_t sb = tiles_base + stage * STAGE_BYTES, full = bar_full + 8 * stage;
           mbar_expect_tx(full, STAGE_BYTES);
           // dY^T tile: rows = 128 couts, 64 consecutive pixels (flattened index kb*64)
@@ -97,8 +100,9 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_g_hi, const __grid_con
 #pragma unroll
           for (int at = 0; at < BN / 64; ++at) {
             const int c0 = ci_t * BN + at * 64;
-            tma_load_4d(sb + 2 * G_BYTES + at * A_ATOM, &map_a_hi, full, c0, tw * p.TW + dx, th * p.TH + dy, tb * p.TB);
-            tma_load_4d(sb + 2 * G_BYTES + A_BYTES + at * A_ATOM, &map_a_lo, full, c0, tw * p.TW + dx, th * p.TH + dy, tb * p.TB);
+            tma_load_4d_im2col(sb + 2 * G_BYTES + at * A_ATOM, &map_a_hi, full, c0, pw + p.lo, ph + p.lo, pb, ox, oy);
+            tma_load_4d_im2col(sb + 2 * G_BYTES + A_BYTES + at * A_ATOM, &map_a_lo, full, c0, pw + p.lo, ph + p.lo, pb,
+                               ox, oy);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
@@ -192,13 +196,13 @@ wgrad_reduce_kernel(const float* __restrict__ partial, int splits, int taps, int
 // ---------------------------------------------------------------------------------------------
 // fp32 NHWC gradient [P][C] -> split planes in both orientations + per-channel sums (bias grad):
 //   hi/lo   [P][C]  (K = channel major: A operand of the data-gradient conv)
-//   hi_t/lo_t [C][P] (K = pixel major: A operand of the weight-gradient GEMM)
+//   hi_t/lo_t [C][P] with row pitch ld_t (K = pixel major: A operand of the weight-gradient GEMM)
 // 32x32 tiles through shared memory; colsum partials per tile row-block, reduced in fixed order.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 split_grad_kernel(const float* __restrict__ src, int64_t P, int C, __nv_bfloat16* __restrict__ hi,
                   __nv_bfloat16* __restrict__ lo, __nv_bfloat16* __restrict__ hi_t, __nv_bfloat16* __restrict__ lo_t,
-                  float* __restrict__ colsum_part) {
+                  int64_t ld_t, float* __restrict__ colsum_part) {
   __shared__ float tile[64][65];
   const int64_t p0 = (int64_t)blockIdx.x * 64;
   const int c0 = blockIdx.y * 64;
@@ -223,8 +227,8 @@ split_grad_kernel(const float* __restrict__ src, int64_t P, int C, __nv_bfloat16
     if (c < C && pp < P) {
       __nv_bfloat16 h, l;
       split_bf16(tile[tx][r], h, l);
-      hi_t[(int64_t)c * P + pp] = h;
-      lo_t[(int64_t)c * P + pp] = l;
+      hi_t[(int64_t)c * ld_t + pp] = h;
+      lo_t[(int64_t)c * ld_t + pp] = l;
     }
   }
   if (colsum_part && ty == 0 && c0 + tx < C) {
@@ -253,11 +257,11 @@ colsum_reduce_kernel(const float* __restrict__ part, int64_t nblk, int C, float*
   }
 }
 
-static int make_gt_map(CUtensorMap* m, const void* ptr, int Cout, int64_t P) {
+static int make_gt_map(CUtensorMap* m, const void* ptr, int Cout, int64_t P, int64_t ld) {
   EncodeTiledFn enc = get_encode();
   BBDM_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled entry point not available");
   cuuint64_t dims[2] = {(cuuint64_t)P, (cuuint64_t)Cout};
-  cuuint64_t strides[1] = {(cuuint64_t)P * 2};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
   cuuint32_t box[2] = {(cuuint32_t)WG_BK, (cuuint32_t)WG_BM};
   cuuint32_t es[2] = {1, 1};
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, es,
@@ -267,17 +271,21 @@ static int make_gt_map(CUtensorMap* m, const void* ptr, int Cout, int64_t P) {
   return BBDM_OK;
 }
 
-static int make_act64_map(CUtensorMap* m, const void* ptr, int B, int H, int W, int C, int TW, int TH, int TB) {
-  EncodeTiledFn enc = get_encode();
-  BBDM_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled entry point not available");
+// im2col map of the activation planes: 64 pixels x 64 channels per load.  The bounding box of each image runs from
+// row / column lo to H-1+lo / W-1+lo (H x W positions, one per output pixel); a load's coordinates are the first output
+// pixel shifted by lo, and the tap's offset within the window (0..2) is the im2col offset.
+static int make_act_im2col_map(CUtensorMap* m, const void* ptr, int B, int H, int W, int C, int lo) {
+  EncodeIm2colFn enc = get_encode_im2col();
+  BBDM_REQUIRE(enc != nullptr, "cuTensorMapEncodeIm2col entry point not available");
   cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
   cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {64, (cuuint32_t)TW, (cuuint32_t)TH, (cuuint32_t)TB};
+  const int lower[2] = {lo, lo}, upper[2] = {lo, lo};
   cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  BBDM_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(wgrad activation) failed: %d", (int)r);
+  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, lower, upper, 64,
+                   (cuuint32_t)WG_BK, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  BBDM_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeIm2col(wgrad activation) failed: %d (B=%d H=%d W=%d C=%d)", (int)r,
+               B, H, W, C);
   return BBDM_OK;
 }
 
@@ -302,9 +310,11 @@ using namespace bbdm;
 
 extern "C" {
 
-int bbdm_split_grad(const float* src, int64_t P, int C, void* hi, void* lo, void* hi_t, void* lo_t,
+int bbdm_split_grad(const float* src, int64_t P, int C, void* hi, void* lo, void* hi_t, void* lo_t, int64_t ld_t,
                     float* colsum, float* workspace, void* stream) {
   BBDM_REQUIRE(src && hi_t && lo_t && P > 0 && C > 0, "split_grad: bad args");
+  BBDM_REQUIRE(ld_t >= P, "split_grad: row pitch %lld of the transposed planes < P = %lld", (long long)ld_t,
+               (long long)P);
   BBDM_REQUIRE((hi == nullptr) == (lo == nullptr), "split_grad: hi/lo in pairs");
   BBDM_REQUIRE(colsum == nullptr || workspace != nullptr, "split_grad: colsum needs a workspace of ceil(P/64)*C floats");
   const int64_t nb = (P + 63) / 64;
@@ -312,7 +322,7 @@ int bbdm_split_grad(const float* src, int64_t P, int C, void* hi, void* lo, void
   dim3 grid((unsigned)nb, (C + 63) / 64);
   cudaStream_t s = (cudaStream_t)stream;
   split_grad_kernel<<<grid, 256, 0, s>>>(src, P, C, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, (__nv_bfloat16*)hi_t,
-                                         (__nv_bfloat16*)lo_t, colsum ? workspace : nullptr);
+                                         (__nv_bfloat16*)lo_t, ld_t, colsum ? workspace : nullptr);
   BBDM_LAUNCH_CHECK();
   if (colsum) {
     colsum_reduce_kernel<<<(C + 31) / 32, 256, 0, s>>>(workspace, nb, C, colsum);
@@ -337,26 +347,24 @@ int bbdm_conv_wgrad_workspace(int B, int H, int W, int Cin, int Cout, int taps, 
   return BBDM_OK;
 }
 
-int bbdm_conv_wgrad(const void* g_hi_t, const void* g_lo_t, const void* a_hi, const void* a_lo, int B, int H,
-                    int W, int Cin, int Cout, int taps, int window_origin, float* dw, float* workspace, void* stream) {
+int bbdm_conv_wgrad(const void* g_hi_t, const void* g_lo_t, int64_t ld_g, const void* a_hi, const void* a_lo, int B,
+                    int H, int W, int Cin, int Cout, int taps, int window_origin, float* dw, float* workspace,
+                    void* stream) {
   BBDM_REQUIRE(g_hi_t && g_lo_t && a_hi && a_lo && dw && workspace, "conv_wgrad: null pointer");
   BBDM_REQUIRE(Cin % 64 == 0 && Cout % 64 == 0 && (taps == 1 || taps == 4 || taps == 9) && W >= 4,
                "conv_wgrad: unsupported shape");
   BBDM_REQUIRE(window_origin == 0 || (taps == 4 && window_origin == -1),
                "conv_wgrad: window_origin -1 needs taps == 4 (got origin %d, taps %d)", window_origin, taps);
   const int64_t P = (int64_t)B * H * W;
-  BBDM_REQUIRE(P % 64 == 0 && (P * 2) % 16 == 0, "conv_wgrad: B*H*W must be a multiple of 64");
+  BBDM_REQUIRE(B > 0 && H > 0 && P < (1ll << 31) - WG_BK, "conv_wgrad: bad pixel count (B=%d H=%d W=%d)", B, H, W);
+  // TMA global strides are multiples of 16 bytes: the dY^T rows need a pitch of a multiple of 8 pixels
+  BBDM_REQUIRE(ld_g >= P && ld_g % 8 == 0, "conv_wgrad: dY^T row pitch %lld must be >= P = %lld and a multiple of 8",
+               (long long)ld_g, (long long)P);
   WgradParams p;
   p.Cout = Cout; p.Cin = Cin; p.taps = taps; p.origin = window_origin;
-  // 64-pixel box: as wide as possible in w, then h, then b (same order as the flattened pixel index)
-  int tw = 1; while (tw * 2 <= W && tw * 2 <= 64 && W % (tw * 2) == 0) tw *= 2;
-  int th = 1; while (tw * th * 2 <= 64 && th * 2 <= H && H % (th * 2) == 0) th *= 2;
-  int tb = 64 / (tw * th);
-  BBDM_REQUIRE(W % tw == 0 && H % th == 0 && (tw == W || th == 1) && (th == H || tb == 1) && B % tb == 0,
-               "conv_wgrad: a 64-pixel run must be a box (W=%d H=%d B=%d)", W, H, B);
-  p.TW = tw; p.TH = th; p.TB = tb;
-  p.tiles_w = W / tw; p.tiles_h = H / th; p.tiles_b = B / tb;
-  p.kblocks = (int)(P / 64);
+  p.H = H; p.W = W;
+  p.lo = taps == 9 ? -1 : (taps == 4 ? window_origin : 0);
+  p.kblocks = (int)((P + WG_BK - 1) / WG_BK);
   int splits; int64_t fl;
   int rc = bbdm_conv_wgrad_workspace(B, H, W, Cin, Cout, taps, &splits, &fl);
   if (rc) return rc;
@@ -371,10 +379,10 @@ int bbdm_conv_wgrad(const void* g_hi_t, const void* g_lo_t, const void* a_hi, co
   p.n_co = (Cout + WG_BM - 1) / WG_BM;
   p.n_ci = Cin / BN;
   CUtensorMap maps[4];
-  if ((rc = make_gt_map(&maps[0], g_hi_t, Cout, P))) return rc;
-  if ((rc = make_gt_map(&maps[1], g_lo_t, Cout, P))) return rc;
-  if ((rc = make_act64_map(&maps[2], a_hi, B, H, W, Cin, tw, th, tb))) return rc;
-  if ((rc = make_act64_map(&maps[3], a_lo, B, H, W, Cin, tw, th, tb))) return rc;
+  if ((rc = make_gt_map(&maps[0], g_hi_t, Cout, P, ld_g))) return rc;
+  if ((rc = make_gt_map(&maps[1], g_lo_t, Cout, P, ld_g))) return rc;
+  if ((rc = make_act_im2col_map(&maps[2], a_hi, B, H, W, Cin, p.lo))) return rc;
+  if ((rc = make_act_im2col_map(&maps[3], a_lo, B, H, W, Cin, p.lo))) return rc;
   const int64_t total = (int64_t)p.splits * taps * p.n_co * p.n_ci;
   const int grid = (int)(total < num_sms() ? total : num_sms());
   cudaStream_t s = (cudaStream_t)stream;

@@ -49,6 +49,15 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
       " [%0], [%1, {%3, %4, %5, %6}], [%2];"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
+// im2col mode over an NHWC map: `pixelsPerColumn` pixels of the map's bounding box, starting at (c0, w, h, n) and
+// walking w, then h, then n (across rows and images), each pixel read at (w + off_w, h + off_h); OOB zero fill.
+__device__ __forceinline__ void tma_load_4d_im2col(uint32_t dst, const CUtensorMap* map, uint32_t bar,
+                                                   int c0, int w, int h, int n, uint16_t off_w, uint16_t off_h) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(w), "r"(h), "r"(n), "h"(off_w), "h"(off_h) : "memory");
+}
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
@@ -171,5 +180,21 @@ static inline EncodeTiledFn get_encode() {
   return fn;
 }
 
+typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                   const cuuint64_t*, const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*,
+                                   CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                   CUtensorMapFloatOOBfill);
+
+static inline EncodeIm2colFn get_encode_im2col() {
+  static EncodeIm2colFn fn = nullptr;
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &p, cudaEnableDefault, &qres) == cudaSuccess &&
+        qres == cudaDriverEntryPointSuccess)
+      fn = (EncodeIm2colFn)p;
+  }
+  return fn;
+}
 
 }  // namespace bbdm

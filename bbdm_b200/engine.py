@@ -81,7 +81,7 @@ class KernelExecutor:
         self._wino_geom = {}
 
     def _umma_ok(self, cin, cout, w):
-        return cin % 64 == 0 and cout % 64 == 0 and w >= 4
+        return convs.tensor_core_ok(cin, cout, w)
 
     # ------------------------------------------------------------------------------ helpers
     def _pool(self, device, shape_key=None):

@@ -67,16 +67,11 @@ def _on_device(x: torch.Tensor) -> bool:
 
 
 def _tc_ok(x: torch.Tensor, cin: int, cout: int) -> bool:
-    """Operands the tensor-core fwd/dgrad/wgrad kernels take: fp32 [B, C, H, W] on the device, channel counts that
-    are multiples of 64, and a pixel grid the 64-pixel tile box covers."""
+    """Operands the tensor-core fwd/dgrad/wgrad kernels take: fp32 [B, C, H, W] on the device and the shapes of
+    convs.tensor_core_ok (any map size and batch)."""
     if not _on_device(x) or x.dtype != torch.float32 or x.dim() != 4:
         return False
-    B, _, H, W = x.shape
-    return _tc_grid_ok(B, H, W, cin, cout)
-
-
-def _tc_grid_ok(B, H, W, cin, cout):
-    return cin % 64 == 0 and cout % 64 == 0 and W >= 4 and (B * H * W) % 64 == 0 and _box64_ok(B, H, W)
+    return convs.tensor_core_ok(cin, cout, x.shape[3])
 
 
 def native_ok(conv: torch.nn.Conv2d, x: torch.Tensor) -> bool:
@@ -86,15 +81,12 @@ def native_ok(conv: torch.nn.Conv2d, x: torch.Tensor) -> bool:
             and conv.groups == 1 and conv.dilation == (1, 1) and _tc_ok(x, conv.in_channels, conv.out_channels))
 
 
-def _box64_ok(B, H, W):
-    tw = 1
-    while tw * 2 <= W and tw * 2 <= 64 and W % (tw * 2) == 0:
-        tw *= 2
-    th = 1
-    while tw * th * 2 <= 64 and th * 2 <= H and H % (th * 2) == 0:
-        th *= 2
-    tb = 64 // (tw * th)
-    return W % tw == 0 and H % th == 0 and (tw == W or th == 1) and (th == H or tb == 1) and B % tb == 0
+def _transposed_planes(C, P, dev):
+    """Split planes (hi, lo) of dY^T for bbdm_split_grad / bbdm_conv_wgrad: [C, P] views of [C, P rounded up to 8]
+    buffers -- the weight-gradient kernel reads the rows through a TMA map, whose row pitch must be a multiple of 16
+    bytes.  The padding columns are never read (the map ends at P)."""
+    ld = -(-P // 8) * 8
+    return tuple(torch.empty((C, ld), dtype=torch.bfloat16, device=dev)[:, :P] for _ in range(2))
 
 
 def _nhwc(x):
@@ -157,8 +149,7 @@ def _conv_backward(be, ctx_shape, a_hi, a_lo, weight, dy, need_dx, need_dw, need
     if need_dx and not wino_dx:
         g_hi = torch.empty((B, H, W, Cout), dtype=torch.bfloat16, device=dev)
         g_lo = torch.empty_like(g_hi)
-    gt_hi = torch.empty((Cout, P), dtype=torch.bfloat16, device=dev)
-    gt_lo = torch.empty_like(gt_hi)
+    gt_hi, gt_lo = _transposed_planes(Cout, P, dev)
     dbias = ws_b = None
     if need_db:
         dbias = torch.empty((Cout,), dtype=torch.float32, device=dev)
@@ -213,8 +204,7 @@ def _split_dy(be, dyn, need_dx, need_db):
     if need_dx:
         g_hi = torch.empty(dyn.shape, dtype=torch.bfloat16, device=dev)
         g_lo = torch.empty_like(g_hi)
-    gt_hi = torch.empty((Cc, P), dtype=torch.bfloat16, device=dev)
-    gt_lo = torch.empty_like(gt_hi)
+    gt_hi, gt_lo = _transposed_planes(Cc, P, dev)
     if need_db:
         dsum = torch.empty((Cc,), dtype=torch.float32, device=dev)
         ws = torch.empty(((P + 63) // 64) * Cc, dtype=torch.float32, device=dev)
@@ -348,22 +338,22 @@ def _resample_ok(x, cin, cout):
 
 def downsample_conv(conv: torch.nn.Conv2d, x: torch.Tensor, enabled: bool = True):
     """The Downsample's 3x3 stride-2 padding-1 conv on Stride2Conv2dFn, or None where the kernels do not take the
-    shape (Cin, Cout multiples of 64, H and W even, and the half-resolution grid one the tensor-core kernels cover)."""
+    shape (Cin, Cout multiples of 64, H and W even, and a half-resolution grid at least 4 wide)."""
     if not (enabled and _resample_ok(x, conv.in_channels, conv.out_channels)):
         return None
     B, Cin, H, W = x.shape
-    if Cin % 64 or H % 2 or W % 2 or not _tc_grid_ok(B, H // 2, W // 2, 4 * Cin, conv.out_channels):
+    if Cin % 64 or H % 2 or W % 2 or not convs.tensor_core_ok(4 * Cin, conv.out_channels, W // 2):
         return None
     return Stride2Conv2dFn.apply(x, conv.weight, conv.bias)
 
 
 def upsample_conv(conv: torch.nn.Conv2d, x: torch.Tensor, enabled: bool = True):
     """conv(nearest-2x(x)) of the Upsample on Up2Conv2dFn, or None where the kernels do not take the shape (Cin, Cout
-    multiples of 64 and a low-res grid the tensor-core kernels cover)."""
+    multiples of 64 and a low-res grid at least 4 wide)."""
     if not (enabled and _resample_ok(x, conv.in_channels, conv.out_channels)):
         return None
     B, Cin, H, W = x.shape
-    if not _tc_grid_ok(B, H, W, Cin, conv.out_channels):
+    if not convs.tensor_core_ok(Cin, conv.out_channels, W):
         return None
     return Up2Conv2dFn.apply(x, conv.weight, conv.bias)
 

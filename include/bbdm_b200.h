@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define BBDM_ABI_VERSION 6
+#define BBDM_ABI_VERSION 7
 
 enum {
   BBDM_OK = 0,
@@ -370,10 +370,11 @@ int bbdm_conv_direct_pad(const float* src, const float* w_packed, const float* b
 
 /* fp32 NHWC gradient src [P][C] (P = B*H*W) -> split-bf16 planes in both orientations
  *   hi/lo     [P][C]  (may be NULL)  : A operand of the data-gradient conv
- *   hi_t/lo_t [C][P]                 : A operand (K = pixels) of the weight-gradient GEMM
+ *   hi_t/lo_t [C][P], rows ld_t >= P elements apart : A operand (K = pixels) of the weight-gradient GEMM
+ *                                    (which needs ld_t % 8 == 0: allocate P rounded up to 8)
  * and, if colsum != NULL, colsum[c] = sum_p src[p][c] (the bias gradient; deterministic).
  * workspace: ceil(P/64)*C floats (only needed with colsum). */
-int bbdm_split_grad(const float* src, int64_t P, int C, void* hi, void* lo, void* hi_t, void* lo_t,
+int bbdm_split_grad(const float* src, int64_t P, int C, void* hi, void* lo, void* hi_t, void* lo_t, int64_t ld_t,
                     float* colsum, float* workspace, void* stream);
 
 /* split-K factor and workspace size (floats) bbdm_conv_wgrad needs for this problem. */
@@ -381,12 +382,13 @@ int bbdm_conv_wgrad_workspace(int B, int H, int W, int Cin, int Cout, int taps, 
                               int64_t* floats);
 
 /* dW[co][ci][ky][kx] (OIHW fp32, overwritten) = sum_p dY[p][co] * A[p + tap][ci] on wgmma:
- * g_hi_t/g_lo_t = dY^T planes [Cout][P] from bbdm_split_grad, a_hi/a_lo = the forward conv's
- * operand planes [B,H,W,Cin].  M = Cout, N = Cin, K = pixels; split-bf16 x3; split-K partials
- * reduced in a fixed order.  Requirements: Cin, Cout % 64 == 0, taps in {1, 9} (window_origin 0), or 4 (2x2 window at
- * rows/cols window_origin..window_origin+1, window_origin 0 or -1, as in BbdmConvArgs; dw is then [Cout][Cin][2][2]),
- * B*H*W % 64 == 0. */
-int bbdm_conv_wgrad(const void* g_hi_t, const void* g_lo_t, const void* a_hi, const void* a_lo,
+ * g_hi_t/g_lo_t = dY^T planes [Cout][P] from bbdm_split_grad, rows ld_g elements apart (ld_g >= P, a multiple of 8),
+ * a_hi/a_lo = the forward conv's operand planes [B,H,W,Cin].  M = Cout, N = Cin, K = pixels in blocks of 64 consecutive
+ * pixels of the flattened (b, h, w) index (any map size and batch; the last block is zero-filled past P); split-bf16
+ * x3; split-K partials reduced in a fixed order.  Requirements: Cin, Cout % 64 == 0, W >= 4, taps in {1, 9}
+ * (window_origin 0), or 4 (2x2 window at rows/cols window_origin..window_origin+1, window_origin 0 or -1, as in
+ * BbdmConvArgs; dw is then [Cout][Cin][2][2]). */
+int bbdm_conv_wgrad(const void* g_hi_t, const void* g_lo_t, int64_t ld_g, const void* a_hi, const void* a_lo,
                     int B, int H, int W, int Cin, int Cout, int taps, int window_origin, float* dw,
                     float* workspace, void* stream);
 

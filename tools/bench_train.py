@@ -2,7 +2,12 @@
 """Training micro-step (q_sample + UNet forward + L1 loss + backward) at the UNet shape of BASELINE
 configs[2] (LBBDM-f4: latents [32,3,64,64] per rank, nocond) -- tensor-core conv autograd path
 (bbdm_b200/train.py) vs the stock PyTorch graph in fp32 / TF32 / bf16-autocast.  VQGAN encodes are
-outside this measurement (frozen reference module)."""
+outside this measurement (frozen reference module).
+
+    python tools/bench_train.py cfg2 --size 224 --batch 8 --modes native,fp32,tf32
+
+--size / --batch train the config's UNet at another map size and batch (the FLOP count is scaled by pixels and batch).
+"""
 import json
 import os
 import sys
@@ -71,9 +76,21 @@ def run(mode, cfg, steps=3, warmup=2, ddp=False):
             "train_tflops_per_s": 3 * cfg["flops_per_step"] / ms / 1e9, "max_mem_gb": torch.cuda.max_memory_allocated() / 1e9}
 
 
+def _arg(flag, default):
+    return type(default)(sys.argv[sys.argv.index(flag) + 1]) if flag in sys.argv else default
+
+
+def resized(cfg, size, batch):
+    """cfg with the UNet trained at size x size, batch images (FLOPs scaled by the pixel count)."""
+    f = (size / cfg["size"]) ** 2 * batch / cfg["batch"]
+    return dict(cfg, unet=dict(cfg["unet"], image_size=size), size=size, batch=batch,
+                flops_per_step=cfg["flops_per_step"] * f, name=f"{cfg['name']} -- trained at {size}x{size}, batch {batch}")
+
+
 if __name__ == "__main__":
-    name = sys.argv[1] if len(sys.argv) > 1 else "cfg3"
+    name = sys.argv[1] if len(sys.argv) > 1 and not sys.argv[1].startswith("--") else "cfg3"
     cfg = bench.CONFIGS[name]
+    cfg = resized(cfg, _arg("--size", cfg["size"]), _arg("--batch", cfg["batch"]))
     if "--ddp" in sys.argv:
         import torch.distributed as dist
         dist.init_process_group("nccl")
