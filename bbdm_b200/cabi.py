@@ -42,7 +42,7 @@ SYMBOLS = [
     "bbdm_conv_wgrad_direct", "bbdm_attention_bwd", "bbdm_conv_direct_pad", "bbdm_softmax_rows_split", "bbdm_vq_nearest", "bbdm_s2d_split", "bbdm_pack_weight_split_both",
     "bbdm_wino_geometry", "bbdm_wino_input", "bbdm_wino_output", "bbdm_wino_pack_weight",
     "bbdm_wino6_geometry", "bbdm_wino6_input", "bbdm_wino6_output", "bbdm_wino6_pack_weight",
-    "bbdm_optim_chunk_elems", "bbdm_adam_multi", "bbdm_ema_multi", "bbdm_denorm_to_uint8",
+    "bbdm_optim_chunk_elems", "bbdm_adam_multi", "bbdm_adam_multi_dev", "bbdm_ema_multi", "bbdm_denorm_to_uint8",
     "bbdm_layernorm_split", "bbdm_geglu_split", "bbdm_attention_cross", "bbdm_conv_stem", "bbdm_spatial_rescale",
     "bbdm_layernorm_bwd", "bbdm_geglu_bwd", "bbdm_attention_cross_bwd",
 ]
@@ -170,6 +170,8 @@ def load():
     lib.bbdm_optim_chunk_elems.argtypes = []
     lib.bbdm_adam_multi.argtypes = [vp, vp, vp, vp, vp, vp, i, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double,
                                      C.c_double, i64, vp, C.c_double, vp]
+    lib.bbdm_adam_multi_dev.argtypes = [vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp, C.c_double, C.c_double, C.c_double,
+                                         C.c_double, vp, C.c_double, vp]
     lib.bbdm_ema_multi.argtypes = [vp, vp, vp, vp, vp, i, vp, C.c_double, i, vp]
     for s in SYMBOLS:
         fn = getattr(lib, s)
@@ -510,6 +512,16 @@ class CudaBackend:
                                        ptr(_req(exp_avg_sq)), lr, beta1, beta2, eps, weight_decay, int(step),
                                        ptr(ema_shadow), float(ema_decay), stream()))
         LAUNCHES["n"] += 1
+
+    def adam_multi_dev(self, tab, exp_avg, exp_avg_sq, *, step, lr, beta1, beta2, eps, weight_decay, ema_shadow=None,
+                       ema_decay=0.0):
+        """Capturable form: step (fp32 [] tensor, incremented here on the device) and lr (fp64 [] tensor) are read
+        from device memory."""
+        check(self.lib.bbdm_adam_multi_dev(ptr(tab.params), ptr(tab.grads), ptr(tab.numel), ptr(tab.offsets),
+                                           ptr(tab.chunk_tensor), ptr(tab.chunk_index), tab.n_chunks, ptr(_req(exp_avg)),
+                                           ptr(_req(exp_avg_sq)), ptr(_req(step)), ptr(_req(lr, torch.float64)),
+                                           beta1, beta2, eps, weight_decay, ptr(ema_shadow), float(ema_decay), stream()))
+        LAUNCHES["n"] += 2
 
     def ema_multi(self, tab, shadow, decay, with_decay=True):
         check(self.lib.bbdm_ema_multi(ptr(tab.params), ptr(tab.numel), ptr(tab.offsets), ptr(tab.chunk_tensor),

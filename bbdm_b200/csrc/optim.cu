@@ -5,6 +5,7 @@
 //                      runners/BaseRunner.py:413): grad (+ wd * p), exp_avg.lerp_(grad, 1-b1),
 //                      exp_avg_sq = b2*exp_avg_sq + (1-b2)*grad^2, p -= step_size * exp_avg / (sqrt(exp_avg_sq)/bc2s + eps),
 //                      optionally followed IN THE SAME PASS by the EMA update of the freshly written parameter.
+//   adam_multi_dev_kernel  the same update with step and lr in device memory (bbdm_adam_multi_dev: capturable).
 //   ema_multi_kernel   shadow = (1-d)*p + d*shadow  (runners/base/EMA.py:21-29), or shadow = p (with_decay=False).
 //
 // Parameters and gradients stay the separate nn.Parameter / .grad tensors of the module (pointer table); the optimizer
@@ -27,12 +28,29 @@ __device__ __forceinline__ float ema_lerp(float p, float s, float d, float one_m
   return __fadd_rn(__fmul_rn(one_minus_d, p), __fmul_rn(d, s));
 }
 
-__global__ void __launch_bounds__(256)
-adam_multi_kernel(float* const* __restrict__ params, const float* const* __restrict__ grads,
-                  const int64_t* __restrict__ numel, const int64_t* __restrict__ state_off,
-                  const int32_t* __restrict__ chunk_tensor, const int32_t* __restrict__ chunk_index,
-                  float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq, float* __restrict__ ema_shadow,
-                  const AdamScalars a) {
+// the scalar preparation of torch.optim.adam._single_tensor_adam (python floats = fp64), each scalar rounded to fp32
+// once at the end.  The hyper-parameters must arrive as doubles: 1 - beta2 of an fp32-rounded beta2 0.999 is 1.3e-5
+// off, and with it exp_avg_sq and the bias correction.  Host (bbdm_adam_multi) and device (bbdm_adam_multi_dev, step
+// and lr read from device memory) run the same expressions.
+__host__ __device__ inline AdamScalars adam_scalars(double lr, double beta1, double beta2, double eps, double weight_decay,
+                                                    double step, bool ema, double ema_decay) {
+  const double bc1 = 1.0 - pow(beta1, step), bc2 = 1.0 - pow(beta2, step);
+  AdamScalars a;
+  a.lr_over_bc1 = (float)(lr / bc1);
+  a.beta1 = (float)beta1; a.beta2 = (float)beta2; a.eps = (float)eps; a.weight_decay = (float)weight_decay;
+  a.inv_bc2_sqrt = (float)(1.0 / sqrt(bc2));
+  a.one_minus_beta1 = (float)(1.0 - beta1);
+  a.one_minus_beta2 = (float)(1.0 - beta2);
+  a.ema_decay = ema ? (float)ema_decay : -1.0f;
+  a.ema_one_minus = (float)(1.0 - ema_decay);
+  return a;
+}
+
+__device__ __forceinline__ void adam_chunk(float* const* __restrict__ params, const float* const* __restrict__ grads,
+                                           const int64_t* __restrict__ numel, const int64_t* __restrict__ state_off,
+                                           const int32_t* __restrict__ chunk_tensor, const int32_t* __restrict__ chunk_index,
+                                           float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
+                                           float* __restrict__ ema_shadow, const AdamScalars& a) {
   const int t = chunk_tensor[blockIdx.x];
   const int64_t n = numel[t], start = (int64_t)chunk_index[blockIdx.x] * OPT_CHUNK;
   float* __restrict__ p = params[t];
@@ -55,6 +73,36 @@ adam_multi_kernel(float* const* __restrict__ params, const float* const* __restr
     p[i] = pn;
     if (s && a.ema_decay >= 0.f) s[i] = ema_lerp(pn, s[i], a.ema_decay, a.ema_one_minus);
   }
+}
+
+__global__ void __launch_bounds__(256)
+adam_multi_kernel(float* const* __restrict__ params, const float* const* __restrict__ grads,
+                  const int64_t* __restrict__ numel, const int64_t* __restrict__ state_off,
+                  const int32_t* __restrict__ chunk_tensor, const int32_t* __restrict__ chunk_index,
+                  float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq, float* __restrict__ ema_shadow,
+                  const AdamScalars a) {
+  adam_chunk(params, grads, numel, state_off, chunk_tensor, chunk_index, exp_avg, exp_avg_sq, ema_shadow, a);
+}
+
+// step += 1 on the device, ahead of the update launch that reads it (stream order: every CTA sees the new count)
+__global__ void adam_step_increment_kernel(float* step) { *step += 1.0f; }
+
+// the capturable form: step (fp32, already incremented) and lr (fp64) in device memory, so a captured graph
+// replays with the counter advancing and the learning rate its owner last wrote; the bias corrections are formed
+// once per CTA from them
+__global__ void __launch_bounds__(256)
+adam_multi_dev_kernel(float* const* __restrict__ params, const float* const* __restrict__ grads,
+                      const int64_t* __restrict__ numel, const int64_t* __restrict__ state_off,
+                      const int32_t* __restrict__ chunk_tensor, const int32_t* __restrict__ chunk_index,
+                      float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq, float* __restrict__ ema_shadow,
+                      const float* __restrict__ step, const double* __restrict__ lr, double beta1, double beta2,
+                      double eps, double weight_decay, double ema_decay) {
+  __shared__ AdamScalars sa;
+  if (threadIdx.x == 0)
+    sa = adam_scalars(*lr, beta1, beta2, eps, weight_decay, (double)*step, ema_shadow != nullptr, ema_decay);
+  __syncthreads();
+  const AdamScalars a = sa;
+  adam_chunk(params, grads, numel, state_off, chunk_tensor, chunk_index, exp_avg, exp_avg_sq, ema_shadow, a);
 }
 
 __global__ void __launch_bounds__(256)
@@ -85,21 +133,27 @@ int bbdm_adam_multi(void* const* params, const void* const* grads, const int64_t
   BBDM_REQUIRE(params && grads && numel && state_off && chunk_tensor && chunk_index && exp_avg && exp_avg_sq,
                "adam_multi: null pointer");
   BBDM_REQUIRE(n_chunks > 0 && step >= 1, "adam_multi: need n_chunks > 0 and step >= 1");
-  // scalar preparation exactly as torch.optim.adam._single_tensor_adam does it (python floats = fp64), each scalar
-  // rounded to fp32 once at the end.  The hyper-parameters must arrive as doubles: 1 - beta2 of an fp32-rounded beta2
-  // 0.999 is 1.3e-5 off, and with it exp_avg_sq and the bias correction.
-  const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
-  AdamScalars a;
-  a.lr_over_bc1 = (float)(lr / bc1);
-  a.beta1 = (float)beta1; a.beta2 = (float)beta2; a.eps = (float)eps; a.weight_decay = (float)weight_decay;
-  a.inv_bc2_sqrt = (float)(1.0 / sqrt(bc2));
-  a.one_minus_beta1 = (float)(1.0 - beta1);
-  a.one_minus_beta2 = (float)(1.0 - beta2);
-  a.ema_decay = ema_shadow ? (float)ema_decay : -1.0f;
-  a.ema_one_minus = (float)(1.0 - ema_decay);
+  const AdamScalars a = adam_scalars(lr, beta1, beta2, eps, weight_decay, (double)step, ema_shadow != nullptr, ema_decay);
   adam_multi_kernel<<<n_chunks, 256, 0, (cudaStream_t)stream>>>((float* const*)params, (const float* const*)grads, numel,
                                                                state_off, chunk_tensor, chunk_index, exp_avg, exp_avg_sq,
                                                                ema_shadow, a);
+  BBDM_LAUNCH_CHECK();
+  return BBDM_OK;
+}
+
+int bbdm_adam_multi_dev(void* const* params, const void* const* grads, const int64_t* numel, const int64_t* state_off,
+                        const int32_t* chunk_tensor, const int32_t* chunk_index, int n_chunks, float* exp_avg,
+                        float* exp_avg_sq, float* step, const double* lr, double beta1, double beta2, double eps,
+                        double weight_decay, float* ema_shadow, double ema_decay, void* stream) {
+  BBDM_REQUIRE(params && grads && numel && state_off && chunk_tensor && chunk_index && exp_avg && exp_avg_sq && step && lr,
+               "adam_multi_dev: null pointer");
+  BBDM_REQUIRE(n_chunks > 0, "adam_multi_dev: need n_chunks > 0");
+  adam_step_increment_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step);
+  BBDM_LAUNCH_CHECK();
+  adam_multi_dev_kernel<<<n_chunks, 256, 0, (cudaStream_t)stream>>>((float* const*)params, (const float* const*)grads,
+                                                                   numel, state_off, chunk_tensor, chunk_index, exp_avg,
+                                                                   exp_avg_sq, ema_shadow, step, lr, beta1, beta2, eps,
+                                                                   weight_decay, ema_decay);
   BBDM_LAUNCH_CHECK();
   return BBDM_OK;
 }

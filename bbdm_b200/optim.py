@@ -4,7 +4,9 @@
 (``bbdm_adam_multi``) instead of ~10 elementwise launches per tensor; same constructor, same hyper-parameters,
 same ``state_dict`` layout (``step`` / ``exp_avg`` / ``exp_avg_sq`` per parameter -- the per-parameter tensors
 are views into two flat buffers), so optimizer checkpoints written by the reference runner
-(runners/BaseRunner.py:141-152) load and save unchanged.  The reference builds its optimizer in
+(runners/BaseRunner.py:141-152) load and save unchanged.  ``capturable=True`` keeps the step counter and the learning
+rate on the device (``bbdm_adam_multi_dev``), so ``step()`` can be captured into a CUDA graph like
+``torch.optim.Adam(capturable=True)``; checkpoints of both forms and of torch.optim.Adam load into either.  The reference builds its optimizer in
 runners/utils.py:48-57; the one-line switch is shown in INTEGRATION.md.
 
 ``FusedEMA`` has the interface of the reference ``EMA`` (runners/base/EMA.py:4-43: register / reset_device /
@@ -59,25 +61,34 @@ class TensorTable:
     def views(self, flat):
         return [flat[o:o + n].view(t.shape) for o, n, t in zip(self.offsets_host, self.numel_host, self.tensors)]
 
-    def refresh(self, with_grads=False):
+    def key(self, with_grads=False):
+        """(parameter addresses, gradient addresses or None) as the device tables should hold them."""
         pk = tuple(t.data_ptr() for t in self.tensors)
+        if not with_grads:
+            return pk, None
+        gk = []
+        for t in self.tensors:
+            g = t.grad
+            if g is None:
+                gk.append(0)
+                continue
+            if g.dtype != torch.float32 or not g.is_contiguous() or g.is_sparse:
+                raise ValueError("bbdm_b200.optim: gradients must be dense contiguous fp32")
+            gk.append(g.data_ptr())
+        return pk, tuple(gk)
+
+    def refresh(self, with_grads=False):
+        pk, gk = self.key(with_grads)
         if pk != self._pkey:
             self.params.copy_(torch.tensor(pk, dtype=torch.int64), non_blocking=False)
             self._pkey = pk
-        if with_grads:
-            gk = []
-            for t in self.tensors:
-                g = t.grad
-                if g is None:
-                    gk.append(0)
-                    continue
-                if g.dtype != torch.float32 or not g.is_contiguous() or g.is_sparse:
-                    raise ValueError("bbdm_b200.optim: gradients must be dense contiguous fp32")
-                gk.append(g.data_ptr())
-            gk = tuple(gk)
-            if gk != self._gkey:
-                self.grads.copy_(torch.tensor(gk, dtype=torch.int64), non_blocking=False)
-                self._gkey = gk
+        if with_grads and gk != self._gkey:
+            self.grads.copy_(torch.tensor(gk, dtype=torch.int64), non_blocking=False)
+            self._gkey = gk
+
+
+def _capturing():
+    return torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
 
 
 def _backend_for(t, factory):
@@ -95,41 +106,53 @@ class FusedAdam(torch.optim.Adam):
     backend_factory = staticmethod(lambda: cabi.CudaBackend())
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, amsgrad=False, **kw):
-        if amsgrad or any(kw.get(k) for k in ("maximize", "capturable", "differentiable", "decoupled_weight_decay")):
-            raise NotImplementedError("FusedAdam: amsgrad / maximize / capturable / differentiable / "
-                                      "decoupled_weight_decay are not implemented")
+        if amsgrad or any(kw.get(k) for k in ("maximize", "differentiable", "decoupled_weight_decay")):
+            raise NotImplementedError("FusedAdam: amsgrad / maximize / differentiable / decoupled_weight_decay are not "
+                                      "implemented")
         kw.pop("foreach", None)
         kw.pop("fused", None)
+        self._capturable = bool(kw.get("capturable", False))
         super().__init__(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=False, **kw)
         self._be = None
-        self._flat = {}            # group index -> dict(table, exp_avg, exp_avg_sq, step)
+        self._flat = {}            # group index -> dict(table, exp_avg, exp_avg_sq, step[, lr])
 
     def _group_state(self, gi, group):
         st = self._flat.get(gi)
         plist = [p for p in group["params"] if p.requires_grad]
         if st is not None and len(st["table"].tensors) == len(plist) and all(a is b for a, b in zip(st["table"].tensors, plist)):
             return st
+        if self._capturable and _capturing():
+            raise RuntimeError("FusedAdam(capturable=True): the optimizer state is created by the first step(); run one "
+                               "eager step (e.g. in the warm-up before the capture) first")
         if self._be is None:
             self._be = _backend_for(plist[0], self.backend_factory)
         tab = TensorTable(plist, self._be.optim_chunk_elems())
         m = torch.zeros(tab.total, dtype=torch.float32, device=tab.device)
         v = torch.zeros(tab.total, dtype=torch.float32, device=tab.device)
-        step = torch.tensor(0.0, dtype=torch.float32)
+        count = 0.0
         # adopt state loaded through load_state_dict (or left by a previous table) into the flat buffers
+        olds = []
         for p, mv, vv in zip(plist, tab.views(m), tab.views(v)):
             old = self.state.get(p)
             if old and "exp_avg" in old:
                 mv.copy_(old["exp_avg"])
                 vv.copy_(old["exp_avg_sq"])
-                step = torch.as_tensor(float(old["step"]), dtype=torch.float32)
+                count = float(old["step"])
+            olds.append((mv, vv))
+        # one shared counter per group: a host scalar, or (capturable) an fp32 scalar on the parameters' device that
+        # the update kernel increments, as torch.optim.Adam(capturable=True) keeps it
+        step = torch.tensor(count, dtype=torch.float32, device=tab.device if self._capturable else "cpu")
+        for p, (mv, vv) in zip(plist, olds):
             self.state[p] = {"step": step, "exp_avg": mv, "exp_avg_sq": vv}
-        for p in plist:
-            self.state[p]["step"] = step          # one shared counter per group
         st = self._flat[gi] = {"table": tab, "exp_avg": m, "exp_avg_sq": v, "step": step}
+        if self._capturable:
+            st["lr"] = torch.zeros((), dtype=torch.float64, device=tab.device)
         return st
 
     def load_state_dict(self, state_dict):
         super().load_state_dict(state_dict)
+        for group in self.param_groups:             # a checkpoint of either form loads into either form
+            group["capturable"] = self._capturable
         self._flat = {}                             # re-adopt the loaded tensors on the next step
 
     def state_dict(self):
@@ -143,10 +166,15 @@ class FusedAdam(torch.optim.Adam):
 
     @torch.no_grad()
     def step(self, closure=None, ema=None, ema_update=False):
+        """capturable=True: the step counter and the learning rate are device scalars.  Outside a CUDA graph capture
+        every call first writes group["lr"] into that scalar (so LR schedulers keep working); inside a capture the
+        scalar is read as it stands when the graph replays.  A captured step needs the gradients at the addresses
+        they had in the last eager step (e.g. ``zero_grad(set_to_none=False)``)."""
         loss = None
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
+        capturing = self._capturable and _capturing()
         for gi, group in enumerate(self.param_groups):
             have = [p.grad is not None for p in group["params"] if p.requires_grad]
             if not any(have):
@@ -157,15 +185,27 @@ class FusedAdam(torch.optim.Adam):
                                           "the same steps (true for the BBDM UNet); use torch.optim.Adam otherwise")
             st = self._group_state(gi, group)
             tab = st["table"]
-            tab.refresh(with_grads=True)
-            st["step"] += 1
+            if capturing:
+                # the pointer tables are refreshed by a blocking host-to-device copy, which a capture cannot hold
+                if tab.key(with_grads=True) != (tab._pkey, tab._gkey):
+                    raise RuntimeError("FusedAdam(capturable=True): a parameter or gradient changed address since the "
+                                       "last eager step; a captured step needs them where the eager step saw them")
+            else:
+                tab.refresh(with_grads=True)
             beta1, beta2 = group["betas"]
             shadow, decay = None, 0.0
             if ema is not None and ema_update and ema.covers(tab):
                 shadow, decay = ema.flat, ema.ema_decay
-            self._be.adam_multi(tab, st["exp_avg"], st["exp_avg_sq"], lr=float(group["lr"]), beta1=float(beta1),
-                                beta2=float(beta2), eps=float(group["eps"]), weight_decay=float(group["weight_decay"]),
-                                step=int(st["step"]), ema_shadow=shadow, ema_decay=decay)
+            hyper = dict(beta1=float(beta1), beta2=float(beta2), eps=float(group["eps"]),
+                         weight_decay=float(group["weight_decay"]), ema_shadow=shadow, ema_decay=decay)
+            if self._capturable:
+                if not capturing:
+                    st["lr"].fill_(float(group["lr"]))
+                self._be.adam_multi_dev(tab, st["exp_avg"], st["exp_avg_sq"], step=st["step"], lr=st["lr"], **hyper)
+            else:
+                st["step"] += 1
+                self._be.adam_multi(tab, st["exp_avg"], st["exp_avg_sq"], lr=float(group["lr"]), step=int(st["step"]),
+                                    **hyper)
         return loss
 
 

@@ -17,10 +17,13 @@ Execution:
     forward / data gradient / weight gradient, fused GroupNorm+FiLM+SiLU backward, flash-style
     attention backward); skip concats, residual adds, the time-embedding MLP and the loss stay
     stock tensor ops.  ``NATIVE_TRAIN_CONV = False`` runs the whole graph on library kernels.
+    With ``UNetModel.train_graph`` on, that graph runs as two CUDA-graph replays (forward, backward;
+    ``bbdm_b200/train_graph.py``).
 """
 from __future__ import annotations
 
 import math
+import os
 
 import torch
 import torch.nn as nn
@@ -230,6 +233,10 @@ class UNetModel(nn.Module):
     """Same constructor surface as the reference UNetModel (openaimodel.py:446-473); unknown
     template keys (conv_resample, dims, num_heads, context_dim, ...) are accepted alike."""
 
+    # training forward and backward on CUDA-graph replays (bbdm_b200/train_graph.py); BBDM_TRAIN_GRAPH=1 turns it on
+    # for every model, the attribute per class or instance
+    train_graph = os.environ.get("BBDM_TRAIN_GRAPH", "0") != "0"
+
     def __init__(self, image_size, in_channels, model_channels, out_channels, num_res_blocks,
                  attention_resolutions, dropout=0, channel_mult=(1, 2, 4, 8), conv_resample=True,
                  dims=2, num_classes=None, use_checkpoint=False, use_fp16=False, num_heads=-1,
@@ -329,6 +336,12 @@ class UNetModel(nn.Module):
         needs_grad = torch.is_grad_enabled() and (
             x.requires_grad or any(p.requires_grad for p in self.parameters()))
         if needs_grad:
+            if self.train_graph and x.is_cuda:
+                # the same graph on CUDA-graph replays (bbdm_b200/train_graph.py); None where it must run eagerly
+                from . import train_graph
+                emb = timestep_embedding(timesteps, self.model_channels)
+                out = train_graph.forward(self, x, emb, context)
+                return out if out is not None else self._forward_emb(x, emb, context)
             return self._forward_autograd(x, timesteps, context)
         eng = self.engine()       # raises if libbbdm_b200.so is not built
         if not x.is_cuda and getattr(eng.be, "requires_cuda", True):
@@ -339,7 +352,12 @@ class UNetModel(nn.Module):
 
     def _forward_autograd(self, x, timesteps, context):
         """Training graph: plain PyTorch ops over the same parameters (openaimodel.py:721-759)."""
-        emb = self.time_embed(timestep_embedding(timesteps, self.model_channels))
+        return self._forward_emb(x, timestep_embedding(timesteps, self.model_channels), context)
+
+    def _forward_emb(self, x, temb, context):
+        """The training graph from the sinusoidal timestep embedding on (what train_graph captures: the embedding
+        itself is computed from a host-side frequency table, which a CUDA graph cannot copy in)."""
+        emb = self.time_embed(temb)
         if self.condition_key != "nocond":
             x = torch.cat([x, context], dim=1)
         h, hs = x, []

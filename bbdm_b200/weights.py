@@ -19,9 +19,11 @@ def upsample_phase_weights(w: torch.Tensor) -> torch.Tensor:
     """w [Cout, Cin, 3, 3] -> [Cout, Cin, 16], index phase*4 + r*2 + c with phase = a*2 + b."""
     assert w.dim() == 4 and w.shape[2] == 3 and w.shape[3] == 3
     # row-combination matrices R[a][r, dy]: which 3x3 rows feed source row r of phase a
-    R = torch.tensor([[[1., 0., 0.], [0., 1., 1.]],      # a = 0: r=0 <- dy=-1 ; r=1 <- dy=0,+1
-                      [[1., 1., 0.], [0., 0., 1.]]],     # a = 1: r=0 <- dy=-1,0 ; r=1 <- dy=+1
-                     dtype=w.dtype, device=w.device)
+    # (filled on the device rather than copied from a host list: a host-to-device copy cannot be captured into the
+    # training step's CUDA graph)
+    R = torch.zeros(2, 2, 3, dtype=w.dtype, device=w.device)
+    R[0, 0, 0] = R[0, 1, 1] = R[0, 1, 2] = 1.0           # a = 0: r=0 <- dy=-1 ; r=1 <- dy=0,+1
+    R[1, 0, 0] = R[1, 0, 1] = R[1, 1, 2] = 1.0           # a = 1: r=0 <- dy=-1,0 ; r=1 <- dy=+1
     # out[o,i,a,b,r,c] = sum_{dy,dx} R[a,r,dy] * R[b,c,dx] * w[o,i,dy,dx]
     out = torch.einsum("ary,bcx,oiyx->oiabrc", R, R, w)
     return out.reshape(w.shape[0], w.shape[1], 16).contiguous()

@@ -487,6 +487,17 @@ int bbdm_adam_multi(void* const* params, const void* const* grads, const int64_t
                     float* exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay, int64_t step,
                     float* ema_shadow, double ema_decay, void* stream);
 
+/* The same update in the capturable form of torch.optim.Adam(capturable=True): the step count and the learning rate
+ * live in DEVICE memory, so a CUDA graph that captures this call replays it with the count advancing and the rate its
+ * owner last wrote.  `step` (fp32 scalar) is incremented on the device first, then the update reads it (the 1-based
+ * count of this update); `lr` is an fp64 scalar.  The bias corrections are formed in the kernel from those values with
+ * the expressions of bbdm_adam_multi, in fp64, so an eager sequence of calls matches bbdm_adam_multi with the same
+ * counts.  ema_shadow / ema_decay as in bbdm_adam_multi.  Two launches (increment, update). */
+int bbdm_adam_multi_dev(void* const* params, const void* const* grads, const int64_t* numel, const int64_t* state_off,
+                        const int32_t* chunk_tensor, const int32_t* chunk_index, int n_chunks, float* exp_avg,
+                        float* exp_avg_sq, float* step, const double* lr, double beta1, double beta2, double eps,
+                        double weight_decay, float* ema_shadow, double ema_decay, void* stream);
+
 /* EMA.update (runners/base/EMA.py:21-29): shadow = (1-decay)*param + decay*shadow (the reference's operation
  * order with the python-float scalars (1.0 - decay) and decay each rounded to fp32: bit-exact), or shadow = param
  * when with_decay == 0.  decay is a double like the python attribute. */
