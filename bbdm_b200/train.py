@@ -14,7 +14,11 @@ DDP's bucketed NCCL allreduce works unchanged.
 """
 from __future__ import annotations
 
+import contextlib
+import threading
+
 import torch
+import torch.utils.checkpoint
 
 from . import cabi, convs
 from .weights import (stride2_dgrad_weights, stride2_fold_wgrad, stride2_s2d_weights, upsample_dgrad_weights,
@@ -46,6 +50,77 @@ def _library_path(what, x):
 def _wino_ok(be, B, H, W, Cin, Cout, k):
     return bool(WINO_TRAIN and k == 3 and hasattr(be, "wino_geometry")
                 and convs.winograd_ok(be.wino_geometry(B, H, W), Cin, Cout, WINO_MIN_C, WINO_MIN_TILES))
+
+
+# Trimmed recompute of checkpointed blocks: the recompute reuses the GroupNorm statistics of the original forward and,
+# in a ResBlock's tail (unread_outputs), skips the convolutions whose outputs nothing in the backward reads.  False
+# recomputes the whole block; both give bit-identical gradients (the tests compare them).
+RECOMPUTE_TRIM = True
+
+_TLS = threading.local()       # .block: the _BlockRun of the checkpointed block running on this thread; .unread
+
+
+class _BlockRun:
+    """One checkpointed block call: the GroupNorm (mean, rstd) pairs its forward computed, in order, for its recompute."""
+
+    def __init__(self):
+        self.stats, self.recompute, self.next = [], False, 0
+
+
+@contextlib.contextmanager
+def _running(run, recompute):
+    prev = getattr(_TLS, "block", None)
+    _TLS.block, run.recompute, run.next = run, recompute, 0
+    try:
+        yield
+    finally:
+        _TLS.block = prev
+
+
+def _block_contexts():
+    """checkpoint's context_fn: the same _BlockRun around the forward and around the recompute."""
+    run = _BlockRun()
+    return _running(run, False), _running(run, True)
+
+
+def _trimmed_recompute():
+    run = getattr(_TLS, "block", None)
+    return run if RECOMPUTE_TRIM and run is not None and run.recompute else None
+
+
+@contextlib.contextmanager
+def unread_outputs():
+    """Around a block's tail whose convolution outputs only feed the block's output: in a trimmed recompute those
+    convolutions write their backward's operand planes and launch no GEMM (the output tensors stay unwritten)."""
+    prev = getattr(_TLS, "unread", False)
+    _TLS.unread = _trimmed_recompute() is not None
+    try:
+        yield
+    finally:
+        _TLS.unread = prev
+
+
+def _unread():
+    return getattr(_TLS, "unread", False)
+
+
+def _unwritten(shape, dev):
+    """The output of a convolution skipped under unread_outputs: the right shape, no storage behind it."""
+    return torch.empty((1,) * len(shape), dtype=torch.float32, device=dev).expand(*shape)
+
+
+def checkpointed(block, fn, *args):
+    """fn(*args), the forward of a UNet block; with block.use_checkpoint on and autograd recording, only the arguments are
+    kept and fn runs again in the backward (non-reentrant torch.utils.checkpoint, so torch.autograd.grad -- the graph
+    capture's warm-up and DDP -- works).  The recompute issues the forward's own launches on the same operands, minus
+    what RECOMPUTE_TRIM drops: the gradients are bit-identical to the plain graph's.  The RNG state is stashed only where
+    a Dropout of p > 0 is active, so that the recompute draws the forward's masks; reading the generator state is not
+    allowed inside a CUDA graph capture, which such a block never reaches (train_graph.fallback_reason)."""
+    if not (block.use_checkpoint and torch.is_grad_enabled()):
+        return fn(*args)
+    dropout = any(isinstance(m, torch.nn.Dropout) and m.p > 0 and m.training for m in block.modules())
+    return torch.utils.checkpoint.checkpoint(fn, *args, use_reentrant=False, preserve_rng_state=dropout,
+                                             context_fn=_block_contexts)
 
 
 def backend():
@@ -121,9 +196,12 @@ class Conv2dFn(torch.autograd.Function):
         a_lo = torch.empty_like(a_hi)
         be.prep(xn, None, raw_hi=a_hi, raw_lo=a_lo)                      # operand split (one HBM pass)
         w_hi, w_lo, wd_hi, wd_lo = _pack_weights(be, weight, ctx.needs_input_grad[0])
-        out = torch.empty((B, H, W, Cout), dtype=torch.float32, device=dev)
-        be.conv_umma(B=B, H=H, W=W, Cin=Cin, Cout=Cout, taps=k * k, a_hi=a_hi, a_lo=a_lo, w_hi=w_hi, w_lo=w_lo,
-                     bias=None if bias is None else bias.detach(), out=out, passes=3)
+        if _unread():
+            out = _unwritten((B, H, W, Cout), dev)
+        else:
+            out = torch.empty((B, H, W, Cout), dtype=torch.float32, device=dev)
+            be.conv_umma(B=B, H=H, W=W, Cin=Cin, Cout=Cout, taps=k * k, a_hi=a_hi, a_lo=a_lo, w_hi=w_hi, w_lo=w_lo,
+                         bias=None if bias is None else bias.detach(), out=out, passes=3)
         ctx.save_for_backward(a_hi, a_lo, weight, wd_hi, wd_lo)
         ctx.has_bias = bias is not None
         ctx.shape = (B, H, W, Cin, Cout, k)
@@ -373,17 +451,32 @@ class GNActConv2dFn(torch.autograd.Function):
         Cout, _, k, _ = weight.shape
         dev = x.device
         xn = _nhwc(x.detach())
-        mean = torch.empty((B, 32), dtype=torch.float32, device=dev)
-        rstd = torch.empty_like(mean)
-        ws = torch.empty((B * 32 * cabi.GN_MAX_SLICES * 2,), dtype=torch.float64, device=dev)
-        be.gn_stats(xn, None, 32, eps, mean, rstd, ws)
+        run = getattr(_TLS, "block", None)
+        if _trimmed_recompute() is not None:      # the statistics the block's forward reduced, in the same order
+            mean, rstd = run.stats[run.next]
+            run.next += 1
+        else:
+            mean = torch.empty((B, 32), dtype=torch.float32, device=dev)
+            rstd = torch.empty_like(mean)
+            ws = torch.empty((B * 32 * cabi.GN_MAX_SLICES * 2,), dtype=torch.float64, device=dev)
+            be.gn_stats(xn, None, 32, eps, mean, rstd, ws)
+            if run is not None and not run.recompute:
+                run.stats.append((mean, rstd))
+        unread = _unread()
         fs = fh = None
         if scale is not None:
             fs, fh = scale.detach().contiguous().float(), shift.detach().contiguous().float()
         a_hi = torch.empty((B, H, W, Cin), dtype=torch.bfloat16, device=dev)
         a_lo = torch.empty_like(a_hi)
-        rn = None if residual is None else _nhwc(residual.detach())       # + skip(x), fused in the epilogue
-        if resample == 0 and _wino_ok(be, B, H, W, Cin, Cout, k):
+        rn = None if residual is None or unread else _nhwc(residual.detach())      # + skip(x), fused in the epilogue
+        if resample == 0 and _wino_ok(be, B, H, W, Cin, Cout, k) and unread:
+            # a trimmed recompute of the Winograd route: only the activated planes (prep computes them bit for bit as
+            # the input transform does)
+            be.prep(xn, None, groups=32, mean=mean, rstd=rstd, gamma=gamma.detach(), beta=beta.detach(), film_scale=fs,
+                    film_shift=fh, film_stride=0 if fs is None else fs.shape[1], silu=act, act_hi=a_hi, act_lo=a_lo)
+            out = _unwritten((B, H, W, Cout), dev)
+            wd_hi = wd_lo = None
+        elif resample == 0 and _wino_ok(be, B, H, W, Cin, Cout, k):
             # Winograd forward; the input transform also writes the activated split planes the weight gradient needs
             out = convs.wino_conv(be, convs.FreshBuffers(dev), be.wino_geometry(B, H, W), xn.contiguous(), None,
                                   cout=Cout, weight=weight, bias=None if bias is None else bias.detach(),
@@ -397,10 +490,13 @@ class GNActConv2dFn(torch.autograd.Function):
                     film_shift=fh, film_stride=0 if fs is None else fs.shape[1], silu=act, resample=resample,
                     act_hi=a_hi, act_lo=a_lo)
             w_hi, w_lo, wd_hi, wd_lo = _pack_weights(be, weight, True)
-            out = torch.empty((B, H, W, Cout), dtype=torch.float32, device=dev)
-            be.conv_umma(B=B, H=H, W=W, Cin=Cin, Cout=Cout, taps=k * k, a_hi=a_hi, a_lo=a_lo, w_hi=w_hi, w_lo=w_lo,
-                         bias=None if bias is None else bias.detach(), residual=rn,
-                         res_mode=cabi.RES_NONE if rn is None else cabi.RES_SAME, out=out, passes=3)
+            if unread:
+                out = _unwritten((B, H, W, Cout), dev)
+            else:
+                out = torch.empty((B, H, W, Cout), dtype=torch.float32, device=dev)
+                be.conv_umma(B=B, H=H, W=W, Cin=Cin, Cout=Cout, taps=k * k, a_hi=a_hi, a_lo=a_lo, w_hi=w_hi,
+                             w_lo=w_lo, bias=None if bias is None else bias.detach(), residual=rn,
+                             res_mode=cabi.RES_NONE if rn is None else cabi.RES_SAME, out=out, passes=3)
         ctx.save_for_backward(xn, mean, rstd, gamma, beta, fs, fh, a_hi, a_lo, weight, wd_hi, wd_lo)
         ctx.has_bias = bias is not None
         ctx.shape = (B, H, W, Cin, Cout, k)

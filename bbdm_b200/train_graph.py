@@ -65,9 +65,12 @@ def cache_key(unet, x, emb, context):
         return None if t is None else (tuple(t.shape), tuple(t.stride()), t.dtype, t.device, t.requires_grad)
 
     params = list(unet.parameters())
+    # the blocks' own checkpoint switches (UNetModel.use_checkpoint sets them all): the backward graph holds the recompute
+    ckpt = tuple(m.use_checkpoint for m in unet.modules() if isinstance(getattr(m, "use_checkpoint", None), bool))
     return (desc(x), desc(emb), desc(context),
             tuple(p.data_ptr() for p in params), tuple(p.requires_grad for p in params),
-            unet.training, unet_mod.NATIVE_TRAIN_CONV, train.WINO_TRAIN, train.WINO_MIN_C, train.WINO_MIN_TILES)
+            unet.training, unet_mod.NATIVE_TRAIN_CONV, train.WINO_TRAIN, train.WINO_MIN_C, train.WINO_MIN_TILES, ckpt,
+            train.RECOMPUTE_TRIM)
 
 
 class _GraphState:

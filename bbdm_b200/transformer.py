@@ -84,8 +84,12 @@ class CrossAttention(nn.Module):
 
 
 class BasicTransformerBlock(nn.Module):
-    def __init__(self, dim, n_heads, d_head, dropout=0.0, context_dim=None, gated_ff=True):
+    """checkpoint: recompute the block in the backward (the reference's default is on, attention.py:200-212; here it
+    follows the UNet's use_checkpoint -- the native attention cores store no attention matrix either way)."""
+
+    def __init__(self, dim, n_heads, d_head, dropout=0.0, context_dim=None, gated_ff=True, checkpoint=False):
         super().__init__()
+        self.use_checkpoint = checkpoint
         self.attn1 = CrossAttention(query_dim=dim, heads=n_heads, dim_head=d_head, dropout=dropout)      # self-attention
         self.ff = FeedForward(dim, dropout=dropout, glu=gated_ff)
         self.attn2 = CrossAttention(query_dim=dim, context_dim=context_dim, heads=n_heads, dim_head=d_head,
@@ -123,14 +127,15 @@ class SpatialTransformer(nn.Module):
     """GroupNorm(eps 1e-6) -> 1x1 proj_in -> depth x BasicTransformerBlock over 'b (h w) c' -> 1x1 proj_out -> + x
     (attention.py:218-264)."""
 
-    def __init__(self, in_channels, n_heads, d_head, depth=1, dropout=0.0, context_dim=None):
+    def __init__(self, in_channels, n_heads, d_head, depth=1, dropout=0.0, context_dim=None, use_checkpoint=False):
         super().__init__()
         self.in_channels, self.n_heads, self.d_head, self.context_dim = in_channels, n_heads, d_head, context_dim
         inner = n_heads * d_head
         self.norm = nn.GroupNorm(num_groups=32, num_channels=in_channels, eps=1e-6, affine=True)
         self.proj_in = nn.Conv2d(in_channels, inner, kernel_size=1)
         self.transformer_blocks = nn.ModuleList(
-            [BasicTransformerBlock(inner, n_heads, d_head, dropout=dropout, context_dim=context_dim) for _ in range(depth)])
+            [BasicTransformerBlock(inner, n_heads, d_head, dropout=dropout, context_dim=context_dim,
+                                   checkpoint=use_checkpoint) for _ in range(depth)])
         self.proj_out = _zero(nn.Conv2d(inner, in_channels, kernel_size=1))
 
     def _native_ok(self, x, context):
@@ -152,7 +157,7 @@ class SpatialTransformer(nn.Module):
             if self._native_ok(x, context):
                 h = train.gn_act_conv2d(self.norm, self.proj_in, x, act=False)
                 for blk in self.transformer_blocks:
-                    h = blk.forward_native(h, context)
+                    h = train.checkpointed(blk, blk.forward_native, h, context)
                 return train.conv2d(self.proj_out, h) + x
             train._library_path("SpatialTransformer", x)
         b, c, h, w = x.shape
@@ -160,6 +165,6 @@ class SpatialTransformer(nn.Module):
         x = self.proj_in(self.norm(x))
         x = x.flatten(2).transpose(1, 2)
         for blk in self.transformer_blocks:
-            x = blk(x, context=context)
+            x = train.checkpointed(blk, blk, x, context)
         x = x.transpose(1, 2).reshape(b, -1, h, w)
         return self.proj_out(x) + x_in

@@ -29,10 +29,10 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from .transformer import SpatialTransformer
-from .train import (attention_core as _attention_core, conv1x1 as _conv1x1, conv2d as _conv2d,
-                    downsample_conv as _downsample_conv, gn_act_conv2d as _gn_act_conv2d, gn_conv1x1 as _gn_conv1x1,
-                    upsample_conv as _upsample_conv)
+from .transformer import BasicTransformerBlock, SpatialTransformer
+from .train import (attention_core as _attention_core, checkpointed as _checkpointed, conv1x1 as _conv1x1,
+                    conv2d as _conv2d, downsample_conv as _downsample_conv, gn_act_conv2d as _gn_act_conv2d,
+                    gn_conv1x1 as _gn_conv1x1, unread_outputs as _unread_outputs, upsample_conv as _upsample_conv)
 
 # training path: ResBlock convolutions on the wgmma fwd / dgrad / wgrad kernels (bbdm_b200/train.py);
 # set False to run the whole training graph on stock PyTorch kernels
@@ -126,9 +126,10 @@ class ResBlock(TimestepBlock):
     (openaimodel.py:166-278)."""
 
     def __init__(self, channels, emb_channels, dropout, out_channels=None, use_conv=False,
-                 use_scale_shift_norm=False, up=False, down=False):
+                 use_scale_shift_norm=False, use_checkpoint=False, up=False, down=False):
         super().__init__()
         self.channels, self.out_channels = channels, out_channels or channels
+        self.use_checkpoint = use_checkpoint
         self.use_scale_shift_norm, self.up, self.down = use_scale_shift_norm, up, down
         self.dropout = dropout
         self.in_layers = nn.Sequential(GroupNorm32(32, channels), nn.SiLU(),
@@ -148,7 +149,11 @@ class ResBlock(TimestepBlock):
 
     def forward(self, x, emb):
         """Training / autograd graph.  On CUDA the GN+SiLU(+FiLM)+conv chains run as fused autograd
-        Functions over the tensor-core kernels (bbdm_b200/train.py) when shapes qualify."""
+        Functions over the tensor-core kernels (bbdm_b200/train.py) when shapes qualify.  With use_checkpoint the
+        block keeps only its inputs and runs its forward again in the backward."""
+        return _checkpointed(self, self._forward, x, emb)
+
+    def _forward(self, x, emb):
         nat = NATIVE_TRAIN_CONV
         if self.up or self.down:
             h = _gn_act_conv2d(self.in_layers[0], self.in_layers[2], x, None, None, nat, resample=1 if self.up else 2)
@@ -156,31 +161,34 @@ class ResBlock(TimestepBlock):
         else:
             h = _gn_act_conv2d(self.in_layers[0], self.in_layers[2], x, None, None, nat)
         e = self.emb_layers(emb).type(h.dtype)[:, :, None, None]
-        skip_is_conv = isinstance(self.skip_connection, nn.Conv2d)
-        if self.use_scale_shift_norm and self.dropout == 0:
-            scale, shift = torch.chunk(e, 2, dim=1)
-            # the skip path (identity or 1x1 conv of x) is added in the conv epilogue
-            sk = _conv2d(self.skip_connection, x, nat) if skip_is_conv else x
-            return _gn_act_conv2d(self.out_layers[0], self.out_layers[3], h, scale, shift, nat, residual=sk)
-        else:
-            if self.use_scale_shift_norm:
+        with _unread_outputs():       # a recompute needs none of the convolution outputs from here on
+            skip_is_conv = isinstance(self.skip_connection, nn.Conv2d)
+            if self.use_scale_shift_norm and self.dropout == 0:
                 scale, shift = torch.chunk(e, 2, dim=1)
-                h = self.out_layers[0](h) * (1 + scale) + shift
+                # the skip path (identity or 1x1 conv of x) is added in the conv epilogue
+                sk = _conv2d(self.skip_connection, x, nat) if skip_is_conv else x
+                return _gn_act_conv2d(self.out_layers[0], self.out_layers[3], h, scale, shift, nat, residual=sk)
             else:
-                h = self.out_layers[0](h + e)
-            h = self.out_layers[2](self.out_layers[1](h))            # SiLU, Dropout
-            h = _conv2d(self.out_layers[3], h, nat)
-        if isinstance(self.skip_connection, nn.Conv2d):
-            return _conv2d(self.skip_connection, x, nat) + h
-        return x + h
+                if self.use_scale_shift_norm:
+                    scale, shift = torch.chunk(e, 2, dim=1)
+                    h = self.out_layers[0](h) * (1 + scale) + shift
+                else:
+                    h = self.out_layers[0](h + e)
+                h = self.out_layers[2](self.out_layers[1](h))            # SiLU, Dropout
+                h = _conv2d(self.out_layers[3], h, nat)
+            if isinstance(self.skip_connection, nn.Conv2d):
+                return _conv2d(self.skip_connection, x, nat) + h
+            return x + h
 
 
 class AttentionBlock(nn.Module):
     """GN -> qkv 1x1 -> multi-head softmax attention -> proj 1x1 -> +x (openaimodel.py:281-413)."""
 
-    def __init__(self, channels, num_heads=1, num_head_channels=-1, use_new_attention_order=False):
+    def __init__(self, channels, num_heads=1, num_head_channels=-1, use_checkpoint=False,
+                 use_new_attention_order=False):
         super().__init__()
         self.channels = channels
+        self.use_checkpoint = use_checkpoint
         if num_head_channels == -1:
             self.num_heads = num_heads
         else:
@@ -193,8 +201,11 @@ class AttentionBlock(nn.Module):
         self.proj_out = zero_module(nn.Conv1d(channels, channels, 1))
 
     def forward(self, x):
-        # Training forward.  The reference wraps this in its CheckpointFunction (util.py:119-148): same
-        # values; the native attention core never stores the T x T matrix, so nothing is recomputed.
+        # Training forward.  The reference always wraps this in its CheckpointFunction (openaimodel.py:318); here the
+        # native attention core never stores the T x T matrix, so the block is recomputed only with use_checkpoint.
+        return _checkpointed(self, self._forward, x)
+
+    def _forward(self, x):
         b, c, *spatial = x.shape
         nat = NATIVE_TRAIN_CONV and x.dim() == 4
         q4 = None
@@ -276,16 +287,17 @@ class UNetModel(nn.Module):
         self.time_embed = nn.Sequential(nn.Linear(model_channels, ted), nn.SiLU(), nn.Linear(ted, ted))
 
         def res(cin, cout, **kw):
-            return ResBlock(cin, ted, dropout, out_channels=cout,
-                            use_scale_shift_norm=use_scale_shift_norm, **kw)
+            return ResBlock(cin, ted, dropout, out_channels=cout, use_scale_shift_norm=use_scale_shift_norm,
+                            use_checkpoint=use_checkpoint, **kw)
 
         def attn(ch, heads):
             if use_spatial_transformer:
                 # openaimodel.py:547-564 (legacy=True): heads follow num_head_channels when given, d_head = ch // heads
                 n_heads = num_heads if num_head_channels == -1 else ch // num_head_channels
-                return SpatialTransformer(ch, n_heads, ch // n_heads, depth=transformer_depth, context_dim=context_dim)
+                return SpatialTransformer(ch, n_heads, ch // n_heads, depth=transformer_depth, context_dim=context_dim,
+                                          use_checkpoint=use_checkpoint)
             return AttentionBlock(ch, num_heads=heads, num_head_channels=num_head_channels,
-                                  use_new_attention_order=use_new_attention_order)
+                                  use_checkpoint=use_checkpoint, use_new_attention_order=use_new_attention_order)
 
         self.input_blocks = nn.ModuleList(
             [TimestepEmbedSequential(nn.Conv2d(in_channels, model_channels, 3, padding=1))])
@@ -321,7 +333,22 @@ class UNetModel(nn.Module):
                 self.output_blocks.append(TimestepEmbedSequential(*layers))
         self.out = nn.Sequential(GroupNorm32(32, ch), nn.SiLU(),
                                  zero_module(nn.Conv2d(model_channels, out_channels, 3, padding=1)))
+        self.use_checkpoint = use_checkpoint
         self._engine = None
+
+    @property
+    def use_checkpoint(self):
+        """Gradient checkpointing of the training graph: every ResBlock, AttentionBlock and transformer block keeps only
+        its inputs in the forward and recomputes the rest in the backward (openaimodel.py:253-254, attention.py:211-212).
+        Setting it sets the blocks' own switches; sampling ignores it."""
+        return self._use_checkpoint
+
+    @use_checkpoint.setter
+    def use_checkpoint(self, on):
+        self._use_checkpoint = bool(on)
+        for m in self.modules():
+            if isinstance(m, (ResBlock, AttentionBlock, BasicTransformerBlock)):
+                m.use_checkpoint = bool(on)
 
     # ------------------------------------------------------------------------------ dispatch
     def engine(self):

@@ -4,9 +4,11 @@ configs[2] (LBBDM-f4: latents [32,3,64,64] per rank, nocond) -- tensor-core conv
 (bbdm_b200/train.py) vs the stock PyTorch graph in fp32 / TF32 / bf16-autocast.  VQGAN encodes are
 outside this measurement (frozen reference module).
 
-    python tools/bench_train.py cfg2 --size 224 --batch 8 --modes native,fp32,tf32
+    python tools/bench_train.py cfg2 --size 224 --batch 8 --modes native,fp32,tf32 [--checkpoint]
 
 --size / --batch train the config's UNet at another map size and batch (the FLOP count is scaled by pixels and batch).
+--checkpoint sets UNetModel.use_checkpoint (every block recomputed in the backward); --whole-recompute with it recomputes
+the whole block (train.RECOMPUTE_TRIM = False).  A mode that runs out of memory is reported as an error row.
 """
 import json
 import os
@@ -17,6 +19,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench  # noqa: E402
 import bbdm_b200.unet as U  # noqa: E402
+from bbdm_b200 import train  # noqa: E402
 from model.BrownianBridge.BrownianBridgeModel import BrownianBridgeModel  # noqa: E402
 
 
@@ -29,6 +32,8 @@ def run(mode, cfg, steps=3, warmup=2, ddp=False):
     torch.backends.cudnn.benchmark = True
     net = BrownianBridgeModel(bench.namespace(cfg["unet"], cfg["sample_step"])).train()
     bench.init_weights(net.denoise_fn)
+    net.denoise_fn.use_checkpoint = "--checkpoint" in sys.argv
+    train.RECOMPUTE_TRIM = "--whole-recompute" not in sys.argv
     net = net.to(dev)
     if mode == "bf16":
         net.denoise_fn.to(memory_format=torch.channels_last)
@@ -72,8 +77,11 @@ def run(mode, cfg, steps=3, warmup=2, ddp=False):
         dist.all_reduce(lo, op=dist.ReduceOp.MIN)
         dist.all_reduce(hi, op=dist.ReduceOp.MAX)
         extra = {"ddp_world": dist.get_world_size(), "grads_identical_across_ranks": bool(torch.equal(lo, hi))}
-    return {**extra, "mode": mode, "optimizer": type(opt).__name__, "ms_per_micro_step": ms, "micro_steps_per_s": 1e3 / ms, "loss": float(loss),
-            "train_tflops_per_s": 3 * cfg["flops_per_step"] / ms / 1e9, "max_mem_gb": torch.cuda.max_memory_allocated() / 1e9}
+    return {**extra, "mode": mode, "optimizer": type(opt).__name__, "use_checkpoint": net.denoise_fn.use_checkpoint,
+            "recompute_trim": train.RECOMPUTE_TRIM,
+            "ms_per_micro_step": ms, "micro_steps_per_s": 1e3 / ms, "loss": float(loss),
+            "train_tflops_per_s": 3 * cfg["flops_per_step"] / ms / 1e9, "max_mem_gb": torch.cuda.max_memory_allocated() / 1e9,
+            "max_reserved_gb": torch.cuda.max_memory_reserved() / 1e9}
 
 
 def _arg(flag, default):

@@ -3,10 +3,14 @@
 of the reference's training templates.  A step is q_sample + the UNet forward + L1 loss + backward + FusedAdam; the
 VQGAN encodes of the latent models are not part of it (the latents are synthetic).
 
-    python tools/bench_train_graph.py [--shapes f16,f8,f4,cfg2] [--steps 20] [--warmup 3] [--profile] [--out FILE]
+    python tools/bench_train_graph.py [--shapes f16,f8,f4,cfg2] [--steps 20] [--warmup 3] [--profile] [--checkpoint]
+                                      [--whole-recompute] [--out FILE]
 
-Per shape and mode: ms/step (host clock around --steps steps that end in a device synchronise), peak reserved memory, and
-whether the two modes' losses agree bit for bit over three steps from the same weights and seeds.  --profile adds, for
+Per shape and mode: ms/step (host clock around --steps steps that end in a device synchronise), peak allocated and
+reserved memory, and
+whether the two modes' losses agree bit for bit over three steps from the same weights and seeds.  --checkpoint trains
+with UNetModel.use_checkpoint on (every block recomputed in the backward); --whole-recompute recomputes the whole block
+(train.RECOMPUTE_TRIM = False).  --profile adds, for
 each mode, the summed device time of the kernels of one step (torch.profiler) -- set against the step time it says how
 much of an eager step the GPU is idle, waiting for the host.  The card name, power limit and SM clocks of the run are
 recorded with the numbers.
@@ -42,12 +46,13 @@ SHAPES = {
 }
 
 
-def _model(unet, graph, dev):
+def _model(unet, graph, dev, checkpoint=False):
     torch.manual_seed(0)              # the constructor's own initialisation (biases, GroupNorm) as well as the weights
     net = BrownianBridgeModel(bench.namespace(unet, 200)).train()
     bench.init_weights(net.denoise_fn)
     net = net.to(dev)
     net.denoise_fn.train_graph = graph
+    net.denoise_fn.use_checkpoint = checkpoint
     from bbdm_b200.optim import FusedAdam
     return net, FusedAdam(net.get_parameters(), lr=1e-4)
 
@@ -73,15 +78,17 @@ def _kernel_ms(net, opt, x, y, dev):
     return tot / 1000.0
 
 
-def run_shape(name, steps, warmup, profile, dev):
+def run_shape(name, steps, warmup, profile, dev, checkpoint=False):
     unet, B, C, S = SHAPES[name]
     x = bench.synth((B, C, S, S), 1).to(dev)
     y = bench.synth((B, C, S, S), 2).to(dev)
     from bbdm_b200 import train_graph
-    row = {"shape": name, "batch": B, "map": S, "channels": C}
+    from bbdm_b200 import train
+    row = {"shape": name, "batch": B, "map": S, "channels": C, "use_checkpoint": checkpoint,
+           "recompute_trim": train.RECOMPUTE_TRIM}
     losses = {}
     for mode, graph in (("eager", False), ("graph", True)):
-        net, opt = _model(unet, graph, dev)
+        net, opt = _model(unet, graph, dev, checkpoint)
         # the parity check first: three steps from the initial weights under fixed seeds
         ls = []
         for s in range(3):
@@ -99,7 +106,8 @@ def run_shape(name, steps, warmup, profile, dev):
         torch.cuda.synchronize(dev)
         ms = (time.perf_counter() - t0) * 1000.0 / steps
         # reserved, not allocated: the graph's private pool holds its activations as cached (reserved) blocks
-        row[mode] = {"ms_per_step": round(ms, 3), "peak_reserved_gb": round(torch.cuda.max_memory_reserved(dev) / 2**30, 3),
+        row[mode] = {"ms_per_step": round(ms, 3), "peak_allocated_gb": round(torch.cuda.max_memory_allocated(dev) / 2**30, 3),
+                     "peak_reserved_gb": round(torch.cuda.max_memory_reserved(dev) / 2**30, 3),
                      "captures_in_timed_window": train_graph.CAPTURES["n"] - n_cap}
         if profile:
             row[mode]["kernel_ms_per_step"] = round(_kernel_ms(net, opt, x, y, dev), 3)
@@ -127,14 +135,18 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--profile", action="store_true")
+    ap.add_argument("--checkpoint", action="store_true")
+    ap.add_argument("--whole-recompute", action="store_true")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("bench_train_graph: needs a CUDA device")
     dev = torch.device("cuda", 0)
+    from bbdm_b200 import train
+    train.RECOMPUTE_TRIM = not a.whole_recompute
     rows = {"gpu_before": gpu_info(), "rows": []}
     for name in a.shapes.split(","):
-        r = run_shape(name, a.steps, a.warmup, a.profile, dev)
+        r = run_shape(name, a.steps, a.warmup, a.profile, dev, a.checkpoint)
         print(json.dumps(r), flush=True)
         rows["rows"].append(r)
     rows["gpu_after"] = gpu_info()
