@@ -160,7 +160,7 @@ class BridgeOps:
         graph = torch.cuda.CUDAGraph()
         # explicit capture stream on THIS device: torch.cuda.graph's default capture stream is created once per
         # process on whatever device was current then (a model on cuda:1 after one on cuda:0 captured nothing)
-        with torch.cuda.graph(graph, stream=side):
+        with cabi.collector_paused(), torch.cuda.graph(graph, stream=side):
             step()
         st["graph"] = graph
         self._graphs[key] = st

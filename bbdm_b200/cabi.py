@@ -6,6 +6,7 @@ eager/PyTorch fallback for the kernels.  ``python -m bbdm_b200.build`` (or
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import gc
 import os
@@ -21,9 +22,30 @@ OBJ = {"grad": 0, "noise": 1, "ysubx": 2}
 RESAMPLE_NONE, RESAMPLE_UP2, RESAMPLE_DOWN2 = 0, 1, 2
 RES_NONE, RES_SAME, RES_UP2, RES_DOWN2 = 0, 1, 2, 3
 GN_MAX_SLICES = 64
-ATTN_HEAD_DIMS = (16, 32, 64, 128)       # head sizes the attention kernels are built for
-ATTN_TC_HEAD_DIMS = (64, 128)            # ... of which bbdm_attention_tc (wgmma) takes these
+ATTN_HEAD_DIM_RULE = "multiples of 8 up to 128"
+ATTN_TC_HEAD_DIMS = (64, 128)            # head sizes bbdm_attention_tc (wgmma) takes; bbdm_attention_split takes the rest
 LN_MAX_C = 2048                          # bbdm_layernorm_split / _bwd: C even, <= this
+
+
+def attn_head_dim_ok(d):
+    """True for the head sizes the attention kernels are built for: a multiple of 8 (each head's columns stay
+    16-byte aligned in the bf16 operand planes) up to 128 (the flash backward's tiles fit in shared memory)."""
+    return d % 8 == 0 and 8 <= d <= 128
+
+
+@contextlib.contextmanager
+def collector_paused():
+    """Collect the dead reference cycles now and keep Python's cycle collector off until the block ends; wraps every
+    CUDA-graph capture.  A collection inside a capture can destroy CUDA objects held by dead cycles (a discarded
+    model's graphs and their memory pools), and those calls invalidate the capture."""
+    was = gc.isenabled()
+    gc.collect()
+    gc.disable()
+    try:
+        yield
+    finally:
+        if was:
+            gc.enable()
 
 
 def layernorm_bwd_workspace(rows, C):

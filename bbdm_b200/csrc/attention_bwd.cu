@@ -14,12 +14,17 @@
 // Exact fp32 FMA arithmetic on CUDA cores (64x64 tiles, 4x4 register micro-tiles, operands staged in
 // shared memory in both orientations); deterministic (no atomics).  The attention core is <= 1.7 % of
 // the UNet's FLOPs, so this kernel is about correctness and memory, not the tensor pipe.
+// A head_dim D that is not a multiple of 16 is staged at DP = D rounded up to 16 columns, zero past D, so that the
+// 16 column threads of dQ / dK / dV hold DP / 16 columns each; only the columns < D are stored.  With D == DP the
+// padding tests are compile-time constants.
 #include "common.cuh"
 
 namespace bbdm {
 
 constexpr int AB_T = 64;           // tile edge (queries and keys)
 constexpr int AB_LD = AB_T + 4;    // row stride of the P / dS tiles (float4-aligned, conflict-free)
+template <int D>
+constexpr int ab_dp() { return (D + 15) / 16 * 16; }   // head_dim padded to the 16 column threads
 
 // Queries come from q [B, Tq, ldq], keys and values from kv [B, Tkv, ldkv] (the same tensor for self-attention);
 // head h reads columns q_base + h*q_hstride (q), k_base / v_base + h*kv_hstride (k, v) and its gradients go to the
@@ -39,18 +44,20 @@ __device__ __forceinline__ void head_offsets(const AttnBwdParams& p, int head, i
   voff = p.v_base + head * p.kv_hstride;
 }
 
-// 64 rows x D columns of a [*, ld] fp32 matrix -> transposed tile dst_t[D][64] (and row-major dst_r[64][D])
+// 64 rows x D columns of a [*, ld] fp32 matrix -> transposed tile dst_t[DP][64] (and row-major dst_r[64][DP]),
+// zero past row T and past column D
 template <int D>
 __device__ __forceinline__ void load_tile(const float* __restrict__ src, int64_t ld, int t0, int T, float* dst_t, float* dst_r) {
-  for (int i = threadIdx.x; i < AB_T * (D / 4); i += 256) {
+  constexpr int DP = ab_dp<D>();
+  for (int i = threadIdx.x; i < AB_T * (DP / 4); i += 256) {
     const int row = i % AB_T, ch = i / AB_T;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (t0 + row < T) v = ld_f4(src + (int64_t)(t0 + row) * ld + ch * 4);
+    if (t0 + row < T && (D == DP || ch * 4 < D)) v = ld_f4(src + (int64_t)(t0 + row) * ld + ch * 4);
     dst_t[(ch * 4 + 0) * AB_T + row] = v.x;
     dst_t[(ch * 4 + 1) * AB_T + row] = v.y;
     dst_t[(ch * 4 + 2) * AB_T + row] = v.z;
     dst_t[(ch * 4 + 3) * AB_T + row] = v.w;
-    if (dst_r) *reinterpret_cast<float4*>(dst_r + row * D + ch * 4) = v;
+    if (dst_r) *reinterpret_cast<float4*>(dst_r + row * DP + ch * 4) = v;
   }
 }
 
@@ -90,14 +97,15 @@ __device__ __forceinline__ float group16_sum(float v) {
 template <int D>
 __global__ void __launch_bounds__(256)
 attn_bwd_dq_kernel(const AttnBwdParams p) {
-  constexpr int DC = D / 16;        // dQ columns per thread
+  constexpr int DP = ab_dp<D>();
+  constexpr int DC = DP / 16;       // dQ columns per thread
   extern __shared__ __align__(16) float sm[];
-  float* Qt = sm;                   // [D][64]
-  float* dOt = Qt + D * AB_T;       // [D][64]
-  float* Kt = dOt + D * AB_T;       // [D][64]
-  float* Vt = Kt + D * AB_T;        // [D][64]
-  float* Ks = Vt + D * AB_T;        // [64][D]
-  float* dSs = Ks + AB_T * D;       // [64][AB_LD]
+  float* Qt = sm;                   // [DP][64]
+  float* dOt = Qt + DP * AB_T;      // [DP][64]
+  float* Kt = dOt + DP * AB_T;      // [DP][64]
+  float* Vt = Kt + DP * AB_T;       // [DP][64]
+  float* Ks = Vt + DP * AB_T;       // [64][DP]
+  float* dSs = Ks + AB_T * DP;      // [64][AB_LD]
   float* delta_s = dSs + AB_T * AB_LD;   // [64]
 
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
@@ -197,7 +205,7 @@ attn_bwd_dq_kernel(const AttnBwdParams p) {
     for (int k = 0; k < AB_T; ++k) {
       float kv[DC];
 #pragma unroll
-      for (int c = 0; c < DC; ++c) kv[c] = Ks[k * D + tx * DC + c];
+      for (int c = 0; c < DC; ++c) kv[c] = Ks[k * DP + tx * DC + c];
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const float a = dSs[(ty * 4 + i) * AB_LD + k];
@@ -212,7 +220,8 @@ attn_bwd_dq_kernel(const AttnBwdParams p) {
     if (q >= p.Tq) continue;
     float* dst = p.dq + ((int64_t)b * p.Tq + q) * p.ldq + qoff + tx * DC;
 #pragma unroll
-    for (int c = 0; c < DC; ++c) dst[c] = dq[i][c] * p.scale2;
+    for (int c = 0; c < DC; ++c)
+      if (D == DP || tx * DC + c < D) dst[c] = dq[i][c] * p.scale2;
   }
 }
 
@@ -222,15 +231,16 @@ attn_bwd_dq_kernel(const AttnBwdParams p) {
 template <int D>
 __global__ void __launch_bounds__(256)
 attn_bwd_dkv_kernel(const AttnBwdParams p) {
-  constexpr int DC = D / 16;
+  constexpr int DP = ab_dp<D>();
+  constexpr int DC = DP / 16;
   extern __shared__ __align__(16) float sm[];
-  float* Kt = sm;                   // [D][64]
-  float* Vt = Kt + D * AB_T;
-  float* Qt = Vt + D * AB_T;
-  float* dOt = Qt + D * AB_T;
-  float* Qs = dOt + D * AB_T;       // [64][D]
-  float* dOs = Qs + AB_T * D;       // [64][D]
-  float* Ps = dOs + AB_T * D;       // [64 q][AB_LD]
+  float* Kt = sm;                   // [DP][64]
+  float* Vt = Kt + DP * AB_T;
+  float* Qt = Vt + DP * AB_T;
+  float* dOt = Qt + DP * AB_T;
+  float* Qs = dOt + DP * AB_T;      // [64][DP]
+  float* dOs = Qs + AB_T * DP;      // [64][DP]
+  float* Ps = dOs + AB_T * DP;      // [64 q][AB_LD]
   float* dSs = Ps + AB_T * AB_LD;   // [64 q][AB_LD]
   float* lse_s = dSs + AB_T * AB_LD;
   float* delta_s = lse_s + AB_T;
@@ -290,7 +300,7 @@ attn_bwd_dkv_kernel(const AttnBwdParams p) {
       const float pv[4] = {pa.x, pa.y, pa.z, pa.w}, dsv[4] = {da.x, da.y, da.z, da.w};
       float qv[DC], dov[DC];
 #pragma unroll
-      for (int c = 0; c < DC; ++c) { qv[c] = Qs[q * D + tx * DC + c]; dov[c] = dOs[q * D + tx * DC + c]; }
+      for (int c = 0; c < DC; ++c) { qv[c] = Qs[q * DP + tx * DC + c]; dov[c] = dOs[q * DP + tx * DC + c]; }
 #pragma unroll
       for (int i = 0; i < 4; ++i)
 #pragma unroll
@@ -307,6 +317,7 @@ attn_bwd_dkv_kernel(const AttnBwdParams p) {
     float* row = p.dkv + ((int64_t)b * p.Tkv + k) * p.ldkv;
 #pragma unroll
     for (int c = 0; c < DC; ++c) {
+      if (D != DP && tx * DC + c >= D) continue;
       row[koff + tx * DC + c] = dk[i][c] * p.scale2;
       row[voff + tx * DC + c] = dv[i][c];
     }
@@ -315,8 +326,9 @@ attn_bwd_dkv_kernel(const AttnBwdParams p) {
 
 template <int D>
 static int launch_bwd(const AttnBwdParams& p, int B, cudaStream_t s) {
-  const size_t sm1 = (size_t)(5 * D * AB_T + AB_T * AB_LD + AB_T) * sizeof(float);
-  const size_t sm2 = (size_t)(6 * D * AB_T + 2 * AB_T * AB_LD + 2 * AB_T) * sizeof(float);
+  constexpr int DP = ab_dp<D>();
+  const size_t sm1 = (size_t)(5 * DP * AB_T + AB_T * AB_LD + AB_T) * sizeof(float);
+  const size_t sm2 = (size_t)(6 * DP * AB_T + 2 * AB_T * AB_LD + 2 * AB_T) * sizeof(float);
   BBDM_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dq_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1));
   BBDM_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dkv_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2));
   attn_bwd_dq_kernel<D><<<dim3((p.Tq + AB_T - 1) / AB_T, B * p.heads), 256, sm1, s>>>(p);
@@ -336,14 +348,15 @@ static int attention_bwd_launch(const char* what, AttnBwdParams p, int B, void* 
   p.scale2 = (float)(scale * scale);
   p.scale_log2 = (float)(scale * scale * 1.4426950408889634);
   cudaStream_t s = (cudaStream_t)stream;
+  // at D = 128 kernel 2 takes 231,936 B of the 232,448 B opt-in shared memory; DP <= 128 takes no more
+#define BBDM_AB(DD) \
+  case DD: return launch_bwd<DD>(p, B, s);
   switch (D) {
-    case 16: return launch_bwd<16>(p, B, s);
-    case 32: return launch_bwd<32>(p, B, s);
-    case 64: return launch_bwd<64>(p, B, s);
-    case 128: return launch_bwd<128>(p, B, s);     // kernel 2: 231,936 B of the 232,448 B opt-in shared memory
+    BBDM_FOR_ATTN_HEAD_DIMS(BBDM_AB)
     default:
-      BBDM_REQUIRE(false, "%s: head_dim %d not supported (16, 32, 64, 128)", what, D);
+      BBDM_REQUIRE(false, "%s: head_dim %d not supported (a multiple of 8 up to 128)", what, D);
   }
+#undef BBDM_AB
   return BBDM_OK;
 }
 

@@ -107,11 +107,12 @@ def _capture(unet, x, emb, context, key):
     st.fwd, st.bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
     # an explicit capture stream on the tensors' device (torch.cuda.graph's default stream is created once per process
     # on whatever device was current then)
-    with torch.cuda.graph(st.fwd, pool=pool, stream=side):
-        st.out = unet._forward_emb(st.x, st.emb, st.ctx)
-    st.gout = torch.zeros_like(st.out)
-    with torch.cuda.graph(st.bwd, pool=pool, stream=side):
-        grads = torch.autograd.grad(st.out, diff, grad_outputs=st.gout, allow_unused=True)
+    with cabi.collector_paused():
+        with torch.cuda.graph(st.fwd, pool=pool, stream=side):
+            st.out = unet._forward_emb(st.x, st.emb, st.ctx)
+        st.gout = torch.zeros_like(st.out)
+        with torch.cuda.graph(st.bwd, pool=pool, stream=side):
+            grads = torch.autograd.grad(st.out, diff, grad_outputs=st.gout, allow_unused=True)
     st.grads = list(grads)
     # the parameter gradients are copied out into one flat buffer per backward (one multi-tensor copy); its layout
     st.pidx = [i for i, g in enumerate(st.grads[len(st.inputs):]) if g is not None]

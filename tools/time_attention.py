@@ -7,9 +7,12 @@
 Default: the cfg2 middle-block shape (B=16, T=4096, C=1024) as 16 heads x 64 and as 8 heads x 128.  For each
 head_dim it times the --kernels (default: bbdm_attention_tc with split-bf16 planes in and split planes out, and
 bbdm_attention_bwd in exact fp32; also available: the mma.sync forwards bbdm_attention, fp32 qkv in and fp32 out, and
-bbdm_attention_split, split planes in and out, for head_dim 16 / 32 / 64 / 128), alternating the variants over
-rounds and reporting the median.  Algorithmic FLOPs: forward 4 B T^2 C (QK^T, PV),
-backward 10 B T^2 C (the five T x T x D products of FlashAttention's backward), whatever the kernels recompute.
+bbdm_attention_split, split planes in and out, and stock_fwd_bwd, the stock PyTorch attention core that training
+runs on shapes the kernels do not take (AttentionBlock._attention_torch, fp32, forward and autograd backward through
+the stored T x T matrix)), alternating the variants over rounds and reporting the median.  attention_tc takes
+head_dim 64 and 128; attention, attention_split and attention_bwd take any multiple of 8 up to 128.
+Algorithmic FLOPs: forward 4 B T^2 C (QK^T, PV), backward 10 B T^2 C (the five T x T x D products of
+FlashAttention's backward), whatever the kernels recompute; stock_fwd_bwd counts both (14 B T^2 C).
 One JSON line per (kernel, head_dim), each tagged with the card's name and power limit read in the same run."""
 import argparse
 import json
@@ -18,10 +21,13 @@ import statistics
 import subprocess
 import sys
 
+from types import SimpleNamespace
+
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from bbdm_b200 import cabi  # noqa: E402
+from bbdm_b200.unet import AttentionBlock  # noqa: E402
 
 
 def card():
@@ -56,7 +62,7 @@ def main():
     ap.add_argument("--fwd-iters", type=int, default=10)
     ap.add_argument("--bwd-iters", type=int, default=2)
     ap.add_argument("--kernels", nargs="+", default=["attention_tc", "attention_bwd"],
-                    choices=["attention_tc", "attention_bwd", "attention", "attention_split"])
+                    choices=["attention_tc", "attention_bwd", "attention", "attention_split", "stock_fwd_bwd"])
     ap.add_argument("--out", default=None, help="also append the JSON lines to this file")
     a = ap.parse_args()
     if a.shape:
@@ -64,6 +70,11 @@ def main():
             ap.error("positional form: B T C heads, with C divisible by heads")
         a.B, a.T, a.C = a.shape[:3]
         a.head_dims = [a.shape[2] // a.shape[3]]
+    for d in a.head_dims:
+        if not cabi.attn_head_dim_ok(d):
+            ap.error(f"head_dim {d}: the kernels take {cabi.ATTN_HEAD_DIM_RULE}")
+        if "attention_tc" in a.kernels and d not in cabi.ATTN_TC_HEAD_DIMS:
+            ap.error(f"attention_tc takes head_dim {cabi.ATTN_TC_HEAD_DIMS}, not {d}")
     assert torch.cuda.is_available(), "time_attention.py needs a GPU"
     B, T, C = a.B, a.T, a.C
     be = cabi.CudaBackend()
@@ -76,6 +87,12 @@ def main():
     out = torch.empty(B, T, C, device="cuda")
     dout = torch.randn(B, T, C, device="cuda", generator=g)
     dqkv = torch.empty_like(qkv)
+    qkv_bct = qkv.permute(0, 2, 1).contiguous()                    # the stock core's [B, 3C, T] layout
+
+    def stock_fwd_bwd(heads):
+        x = qkv_bct.detach().requires_grad_(True)
+        AttentionBlock._attention_torch(SimpleNamespace(num_heads=heads, new_order=False), x).backward(
+            dout.permute(0, 2, 1))
 
     runs = []                                                      # (kernel, head_dim, heads, fn, iters, flops)
     for d in a.head_dims:
@@ -87,9 +104,10 @@ def main():
                "attention_bwd": (lambda h=heads, l=lse, dl=delta: be.attention_bwd(qkv, out, dout, h, 0, dqkv, l, dl),
                                  a.bwd_iters, 10.0),
                "attention": (lambda h=heads: be.attention(qkv, h, 0, out, None, None), a.fwd_iters, 4.0),
-               "attention_split": (lambda h=heads: be.attention_split(hi, lo, h, 0, None, o_hi, o_lo), a.fwd_iters, 4.0)}
+               "attention_split": (lambda h=heads: be.attention_split(hi, lo, h, 0, None, o_hi, o_lo), a.fwd_iters, 4.0),
+               "stock_fwd_bwd": (lambda h=heads: stock_fwd_bwd(h), a.bwd_iters, 14.0)}
         if "attention_bwd" in a.kernels:
-            be.attention_tc(hi, lo, heads, 0, out, None, None)     # the forward output the backward is given
+            be.attention(qkv, heads, 0, out, None, None)           # the forward output the backward is given
         for k in a.kernels:
             fns[k][0]()                                            # warm up every shape timed below
             runs.append((k, d, heads, *fns[k], []))
