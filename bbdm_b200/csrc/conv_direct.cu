@@ -1,6 +1,8 @@
 // General fp32 convolution on CUDA cores (SIMT implicit GEMM, 64 pixels x TN couts per CTA).
 // Serves the UNet edges (stem Cin=3..32, head Cout=3..16), conv-mode Down/Upsample and any
-// channel count the wgmma kernel does not take.  Exact fp32 FMA accumulation.
+// channel count the wgmma kernel does not take.  fp32 FMA accumulation, two-level: each 16-channel chunk of a tap is
+// summed on its own and then added to the output's total, so the rounding error grows with Cin / 16 + k*k*Cin / 16
+// additions instead of k*k*Cin (a 3x3 conv over 1024 channels sums 9216 products).
 #include "common.cuh"
 
 namespace bbdm {
@@ -60,6 +62,11 @@ conv_direct_kernel(const float* __restrict__ src, const float* __restrict__ wp,
         Ws[kk][n] = (c < Cin && co < Cout) ? wp[((int64_t)tap * Cin + c) * Cout + co] : 0.f;
       }
       __syncthreads();
+      float part[PM][4];
+#pragma unroll
+      for (int i = 0; i < PM; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) part[i][j] = 0.f;
 #pragma unroll
       for (int kk = 0; kk < CD_TK; ++kk) {
         float a[PM], w[4];
@@ -70,8 +77,12 @@ conv_direct_kernel(const float* __restrict__ src, const float* __restrict__ wp,
 #pragma unroll
         for (int i = 0; i < PM; ++i)
 #pragma unroll
-          for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], w[j], acc[i][j]);
+          for (int j = 0; j < 4; ++j) part[i][j] = fmaf(a[i], w[j], part[i][j]);
       }
+#pragma unroll
+      for (int i = 0; i < PM; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] += part[i][j];
       __syncthreads();
     }
   }
@@ -129,6 +140,12 @@ conv_stem_kernel(const float* __restrict__ src, const float* __restrict__ wp, co
       const int dy = tap / 3, dx = tap % 3;
       const float* arow = as + (dy * 34 + warp * 4 + dx) * Cin;
       const float* wrow = ws + tap * Cin * Cout + lane;
+      // the general kernel's two-level order (Cin <= 16 is one chunk per tap): bit-identical results
+      float part[4][NJ];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) part[i][j] = 0.f;
       for (int c = 0; c < Cin; ++c) {
         float w[NJ];
 #pragma unroll
@@ -137,9 +154,13 @@ conv_stem_kernel(const float* __restrict__ src, const float* __restrict__ wp, co
         for (int i = 0; i < 4; ++i) {
           const float a = arow[i * Cin + c];
 #pragma unroll
-          for (int j = 0; j < NJ; ++j) acc[i][j] = fmaf(a, w[j], acc[i][j]);
+          for (int j = 0; j < NJ; ++j) part[i][j] = fmaf(a, w[j], part[i][j]);
         }
       }
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) acc[i][j] += part[i][j];
     }
 #pragma unroll
     for (int i = 0; i < 4; ++i) {

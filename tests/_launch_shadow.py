@@ -23,6 +23,12 @@ pointer arrays rather than tensor arguments.  Training packs its Winograd weight
 wino_pack_weight itself maps the U planes to the weight they hold (for the data gradient the flipped, channel-swapped
 kernel), and the output transform that consumes them takes the entry out again.
 
+The sampling and VQGAN launches are checked the same way: the bridge update (p_sample, and p_sample_dev with its
+coefficients read from the device before the launch) and the uint8 output path bit for bit against the reference's
+fp32 expressions, the space-to-depth split bit for bit, the SpatialRescaler, the padded direct conv, the row softmax and
+the nearest-code search against fp64.  Inside a CUDA-graph capture the shadow only runs each launch and lists it in
+``captured``: a capture records work for later replays, so nothing may be copied, synchronised or read there.
+
 Bounds are those of the single-kernel GPU tests, measured on an H100 with synthetic operands; each names its source.
 A launch whose output goes beyond its bound is a finding, not a bound to raise.
 """
@@ -61,9 +67,17 @@ OUTPUTS = {
     "layernorm_split": ("out_f32", "out_hi", "out_lo"), "layernorm_bwd": ("dx", "dgamma", "dbeta", "workspace"),
     "geglu_split": ("out_f32", "out_hi", "out_lo"), "geglu_bwd": ("du",),
     "adam_multi": ("exp_avg", "exp_avg_sq", "ema_shadow"), "ema_multi": ("shadow",),
+    # the capturable Adam step also increments its device step counter
+    "adam_multi_dev": ("exp_avg", "exp_avg_sq", "ema_shadow", "step"),
+    # sampling: the bridge update, the SpatialRescaler condition, the uint8 output path
+    "p_sample": ("x_out", "x0_out"), "p_sample_dev": ("x_out", "x0_out"), "spatial_rescale": ("out",),
+    "denorm_to_uint8": ("out",),
+    # VQGAN ends (and the UNet's tensor-core Downsample operand)
+    "s2d_split": ("out_hi", "out_lo"), "conv_direct_pad": ("out",), "softmax_rows_split": ("out_hi", "out_lo"),
+    "vq_nearest": ("z_q", "indices"),
 }
 # launches that read (and adam_multi writes) the parameters of a TensorTable instead of tensor arguments
-TABLE_LAUNCHES = ("adam_multi", "ema_multi")
+TABLE_LAUNCHES = ("adam_multi", "adam_multi_dev", "ema_multi")
 
 # a split-bf16 pair carries 16 bits: 2^-17 = 7.6e-6 of the element (test_gpu_winograd.py::test_wino_input_production_layouts)
 PAIR = 8e-6
@@ -126,6 +140,11 @@ BOUNDS = {
     "adam_dp": 1e-5,
     "adam_moments": 1e-6,
     "ema": 1e-6,
+    # sampling and VQGAN ends
+    "conv_direct_pad": 2e-6,    # test_gpu_vqgan.py::test_conv_direct_pad
+    "softmax": 2e-5,            # test_gpu_vqgan.py::test_softmax_rows_split
+    "vq_distance": 1e-5,        # test_gpu_vqgan.py::test_vq_nearest (chosen vs minimum distance; the top-2 gap)
+    "spatial_rescale": 1e-6,    # test_gpu_kernels.py::test_spatial_rescale
 }
 
 # Winograd matrices, interpolation points 0, +-1, +-2 (F(4,3)) and 0, +-1, +-2, +-1/2 (F(6,3))
@@ -287,6 +306,27 @@ def up_phase_reference(w):
     return out
 
 
+def space_to_depth(x):
+    """NHWC [n, H, W, C] -> [n, H/2, W/2, 4C]: channel (a*2 + b)*C + c of pixel (i, j) is pixel (2i + a, 2j + b)."""
+    n, H, W, C = x.shape
+    return x.reshape(n, H // 2, 2, W // 2, 2, C).permute(0, 1, 3, 2, 4, 5).reshape(n, H // 2, W // 2, 4 * C)
+
+
+def s2d_tap_reference(w, origin):
+    """fp64 2x2 taps [4, Cout, 4*Cin] of a 3x3 stride-2 conv w on the space-to-depth operand, from the definition:
+    output pixel i reads input row 2i + k - pad_lo (pad_lo 1 for padding 1, 0 for the VQGAN's (0, 1) padding), which
+    is phase a of operand row i + o for 2o + a = k - pad_lo; tap r = o - origin of the window at origin."""
+    w = w.to(F64)
+    co, ci = w.shape[0], w.shape[1]
+    out = torch.zeros(4, co, 4, ci, dtype=F64, device=w.device)
+    pad_lo = -origin            # origin -1: padding (1, 1), the UNet Downsample; origin 0: padding (0, 1)
+    for ky in range(3):
+        for kx in range(3):
+            (oy, a), (ox, b) = divmod(ky - pad_lo, 2), divmod(kx - pad_lo, 2)
+            out[(oy - origin) * 2 + (ox - origin), :, a * 2 + b] = w[:, :, ky, kx]
+    return out.reshape(4, co, 4 * ci)
+
+
 def attention_ref(qkv, heads, order, sl_img):
     """fp64 softmax attention of images sl_img of qkv [B, T, 3C] (fp64), head by head -> [n, T, C]."""
     B, T, C3 = qkv.shape
@@ -304,6 +344,10 @@ def attention_ref(qkv, heads, order, sl_img):
     return out
 
 
+def _capturing():
+    return torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
+
+
 # ------------------------------------------------------------------------------------------------ the shadow
 Check = collections.namedtuple("Check", "launch method form what dev bound shapes")
 
@@ -314,6 +358,7 @@ class Shadow:
         self.be = be
         self.bounds = dict(BOUNDS, **(bounds or {}))
         self.checks, self.launches = [], []
+        self.captured = []                # methods launched inside a CUDA-graph capture: run, not checked
         self.mutate = {}                  # launch index -> fn(bound arguments): perturbs an output after the launch
         self._wino_in, self._wino_m = {}, {}
         self._weights = {}                # U planes' data_ptr -> (module weight [Cout, Cin, 3, 3], up2_phases, name)
@@ -324,20 +369,29 @@ class Shadow:
     def register_engine(self, eng):
         """Map every Winograd cache entry's U planes to the module weight they were packed from (plain convs, tile 4 and
         6, and the phase-stacked '#up6' entries of the up-ResBlock conv1s), and check the up-phase tap stacks against the
-        module weights."""
+        module weights, and the stride-2 convs' 2x2 tap stacks (space-to-depth operand) likewise.  The UNet executor
+        keeps its modules on eng.unet, the VQGAN executor on eng.vq."""
+        root = eng.vq if hasattr(eng, "vq") else eng.unet
         for name, ent in eng._w.items():
             if not isinstance(ent, dict):
                 continue
             mod = name[:-len("#up6")] if name.endswith("#up6") else name
             if "u_hi" in ent:
-                w = eng.unet.get_submodule(mod).weight.detach()
+                w = root.get_submodule(mod).weight.detach()
                 self._weights[ent["u_hi"].data_ptr()] = (w, name.endswith("#up6"), name)
                 self._packed.pop(ent["u_hi"].data_ptr(), None)
             if "up_hi" in ent:
-                w = eng.unet.get_submodule(mod).weight.detach()
+                w = root.get_submodule(mod).weight.detach()
                 d = image_devs(planes(ent["up_hi"], ent["up_lo"])[None], up_phase_reference(w)[None])
                 self._record(-1, "pack_weight_split_taps", "up-phase stack", "phase taps vs module weight", d,
                              self.bounds["up_phase"], [tuple(ent["up_hi"].shape)])
+            for key, origin in (("s2_hi", -1), ("ds_hi", 0)):     # UNet Downsample / VQGAN Downsample
+                if key in ent:
+                    w = root.get_submodule(mod).weight.detach()
+                    got = planes(ent[key], ent[key[:2] + "_lo"])
+                    d = image_devs(got[None], s2d_tap_reference(w, origin)[None])
+                    self._record(-1, "pack_weight_split_taps", f"s2d stack origin {origin}",
+                                 "s2d taps vs module weight", d, PAIR, [tuple(got.shape)])
 
     def _record(self, idx, method, form, what, devs, bound, shapes):
         dev = float(devs.max()) if isinstance(devs, torch.Tensor) and devs.numel() else float(devs)
@@ -362,6 +416,9 @@ class Shadow:
         lines = [f"{title}: {len(self.launches)} launches, {len(self.checks)} checks",
                  "  launches per method: " + ", ".join(f"{m} {n}" for m, n in
                                                        sorted(collections.Counter(m for m, _ in self.launches).items()))]
+        if self.captured:
+            lines.append("  captured, not checked: " + ", ".join(f"{m} {n}" for m, n in
+                                                                 sorted(collections.Counter(self.captured).items())))
         for (m, what), (n, worst, bound) in sorted(self.families().items()):
             lines.append(f"  {m:22s} {what:34s} {n:5d}  worst {worst:.2e}  bound {bound:.1e}")
         return "\n".join(lines)
@@ -379,6 +436,11 @@ class Shadow:
         sig = inspect.signature(attr)
 
         def launch(*args, **kwargs):
+            if _capturing():
+                # a stream capture records the launch for later replays: no copy, synchronisation or fault-word read
+                # may run inside it, and its outputs do not exist yet
+                self.captured.append(name)
+                return attr(*args, **kwargs)
             bound = sig.bind(*args, **kwargs)
             bound.apply_defaults()
             a = dict(bound.arguments)
@@ -399,9 +461,9 @@ class Shadow:
                 torch.cuda.synchronize(dev)
             self.be.check_fault()
             idx = len(self.launches)
+            form = self._form(name, a)
             if idx in self.mutate:
                 self.mutate[idx](a)
-            form = self._form(name, a)
             self.launches.append((name, form))
             shapes = [tuple(v.shape) for v in a.values() if isinstance(v, torch.Tensor)]
             for k, v in ins.items():
@@ -409,9 +471,10 @@ class Shadow:
                     same = fingerprint(v) == prints[k] if k in big else bits_equal(v, clones[k])
                     self._record(idx, name, form, "inputs unchanged", 0.0 if same else math.inf, 0.0,
                                  [(k, tuple(v.shape))])
-            if tab is not None:         # adam_multi reads the gradients, ema_multi the parameters
-                read = [p.grad for p in tab.tensors] if name == "adam_multi" else [p.detach() for p in tab.tensors]
-                want = pre["grads"] if name == "adam_multi" else pre["params"]
+            if tab is not None:         # adam_multi(_dev) reads the gradients, ema_multi the parameters
+                adam = name != "ema_multi"
+                read = [p.grad for p in tab.tensors] if adam else [p.detach() for p in tab.tensors]
+                want = pre["grads"] if adam else pre["params"]
                 same = all((g is None) == (w is None) and (g is None or bits_equal(g, w)) for g, w in zip(read, want))
                 self._record(idx, name, form, "inputs unchanged", 0.0 if same else math.inf, 0.0,
                              [("tab", len(tab.tensors))])
@@ -430,6 +493,8 @@ class Shadow:
             if a["weights_per_image"]:
                 return "position GEMMs"
             f.append(f"taps {a['taps']}")
+            if a.get("window_origin", 0):
+                f.append(f"origin {a['window_origin']}")
             if a["w_hi"].data_ptr() in self._dgrad_w:        # a training data gradient (each plane set is read once)
                 self._dgrad_w.discard(a["w_hi"].data_ptr())
                 f.append("dgrad")
@@ -438,6 +503,8 @@ class Shadow:
                                   ("stats", a["stats_partial"] is not None)) if on]
             if a["res_mode"]:
                 f.append(f"res {a['res_mode']}")
+            if a["Cin"] >= 4096:           # the VQGAN AttnBlock's O = P V: K = T = 4096 positive products
+                f.append("long K")
         elif name in ("wino_input", "wino_output", "wino_pack_weight"):
             f.append(f"F({a.get('tile', 4)},3)")
             if name == "wino_pack_weight" and a["dgrad"]:
@@ -459,6 +526,8 @@ class Shadow:
             f += [t for t, on in (("planes", a["hi"] is not None), ("colsum", a["colsum"] is not None)) if on]
         elif name == "conv_wgrad":
             f.append(f"taps {a['taps']}")
+            if a["taps"] == 4:
+                f.append(f"origin {a.get('window_origin', 0)}")
         elif name == "conv_wgrad_direct":
             f.append(f"taps {a['k'] ** 2}")
             if a["x"].shape[3] * a["dy"].shape[3] > 1024:
@@ -467,10 +536,23 @@ class Shadow:
             f += [t for t, on in (("film", a["fscale"] is not None), ("no act", not a["silu"])) if on]
         elif name == "attention_bwd":
             f.append(f"order {a['order']}")
-        elif name == "adam_multi":
-            f.append(f"step {a['step']}")
+        elif name in ("adam_multi", "adam_multi_dev"):
+            # adam_multi_dev increments its step counter first: the form names the step it takes, as adam_multi's
+            f.append(f"step {a['step'] if name == 'adam_multi' else int(a['step'].item())}")
             if a["ema_shadow"] is not None:
                 f.append("ema")
+        elif name in ("p_sample", "p_sample_dev"):
+            f += [t for t, on in (("last" if a["is_last"] else "not last", True), ("clip", a["clip"])) if on]
+        elif name == "conv_direct_pad":
+            f.append(f"k {a['k']} stride {a['stride']} pad ({a['pad_lo']}, {a['pad_hi']})")
+        elif name == "softmax_rows_split":
+            f.append(f"{a['src'].shape[-1]} columns")
+        elif name == "spatial_rescale":
+            f.append(f"{a['n_stages']} stages")
+            if a["weight"] is not None:
+                f.append("1x1 map")
+        elif name == "denorm_to_uint8" and a["to_normal"]:
+            f.append("to_normal")
         return " ".join(f)
 
     # -- references: layout / dense ----------------------------------------------------------------------------
@@ -636,8 +718,9 @@ class Shadow:
                                 for pa in range(2) for pb in range(2)]
         elif taps == 9:
             tap_of = lambda w: [[(ky, kx, w[3 * ky + kx]) for ky in range(3) for kx in range(3)]]
-        elif taps == 4:     # 2x2 window at rows / columns 0..1, zero padding bottom / right
-            tap_of = lambda w: [[(1 + r, 1 + s, w[2 * r + s]) for r in range(2) for s in range(2)]]
+        elif taps == 4:     # 2x2 window at rows / columns o..o+1 (window_origin o = 0 or -1), zero padding outside
+            o0 = 1 + c.get("window_origin", 0)
+            tap_of = lambda w: [[(o0 + r, o0 + s, w[2 * r + s]) for r in range(2) for s in range(2)]]
         else:
             assert taps == 1
             tap_of = lambda w: [[(1, 1, w[0])]]
@@ -909,11 +992,14 @@ class Shadow:
 
     # -- training: weight gradients ------------------------------------------------------------------------------
     @staticmethod
-    def _wgrad64(act, grad_rows, k):
-        """fp64 weight gradient [Cout, Cin, k, k] of a stride-1 'same' conv: act [B, H, W, Cin] (any dtype), grad_rows
-        fn(slice of images) -> [Cout, n*H*W] fp64, summed over image chunks."""
+    def _wgrad64(act, grad_rows, k, origin=None):
+        """fp64 weight gradient [Cout, Cin, k, k] of a stride-1 conv whose window starts at offset origin (default
+        -(k // 2), the 'same' conv): dw[:, :, ky, kx] = sum over pixels p of dY[p] act[p + origin + (ky, kx)]^T, zero
+        outside the map.  act [B, H, W, Cin] (any dtype), grad_rows fn(slice of images) -> [Cout, n*H*W] fp64, summed
+        over image chunks."""
         B, H, W, Cin = act.shape
-        p = k // 2
+        o = -(k // 2) if origin is None else origin
+        p = max(-o, k - 1 + o)
         dw = None
         for sl in chunks(B, (H + 2 * p) * (W + 2 * p) * Cin * 8 * 2, act.device):
             ap = F.pad(act[sl].to(F64), (0, 0, p, p, p, p))
@@ -922,7 +1008,8 @@ class Shadow:
                 dw = torch.zeros(g.shape[0], Cin, k, k, dtype=F64, device=act.device)
             for ky in range(k):
                 for kx in range(k):
-                    dw[:, :, ky, kx] += g @ ap[:, ky:ky + H, kx:kx + W].reshape(-1, Cin)
+                    y0, x0 = p + o + ky, p + o + kx
+                    dw[:, :, ky, kx] += g @ ap[:, y0:y0 + H, x0:x0 + W].reshape(-1, Cin)
         return dw
 
     def _ref_conv_wgrad(self, idx, form, shapes, c, a, pre):
@@ -930,7 +1017,10 @@ class Shadow:
         act = planes(c["a_hi"], c["a_lo"]).reshape(B, H, W, Cin)
         gh, gl = c["g_hi_t"].reshape(Cout, -1), c["g_lo_t"].reshape(Cout, -1)
         rows = lambda sl: planes(gh[:, sl.start * H * W:sl.stop * H * W], gl[:, sl.start * H * W:sl.stop * H * W])
-        want = self._wgrad64(act, rows, 3 if taps == 9 else 1)
+        if taps == 4:       # the 2x2 window at rows / columns o..o+1, o = window_origin
+            want = self._wgrad64(act, rows, 2, c.get("window_origin", 0))
+        else:
+            want = self._wgrad64(act, rows, 3 if taps == 9 else 1)
         self._record(idx, "conv_wgrad", form, "dW", image_devs(a["dw"][None], want[None]), self.bounds["conv_wgrad"],
                      shapes)
 
@@ -1113,6 +1203,17 @@ class Shadow:
 
     # -- optimizer -----------------------------------------------------------------------------------------------
     def _ref_adam_multi(self, idx, form, shapes, c, a, pre):
+        self._adam(idx, "adam_multi", form, shapes, c, a, pre, c["lr"], c["step"])
+
+    def _ref_adam_multi_dev(self, idx, form, shapes, c, a, pre):
+        """The capturable step: lr and the step counter are device scalars, read here as they stood before the launch;
+        the launch takes step + 1 and leaves exactly that in the counter."""
+        s0 = float(pre["step"].item())
+        self._record(idx, "adam_multi_dev", form, "step counter + 1", 0.0 if float(a["step"].item()) == s0 + 1 else
+                     math.inf, 0.0, shapes)
+        self._adam(idx, "adam_multi_dev", form, shapes, c, a, pre, float(c["lr"].item()), int(s0) + 1)
+
+    def _adam(self, idx, method, form, shapes, c, a, pre, lr, step):
         """Per parameter tensor: one fp64 torch.optim.Adam step from the pre-launch parameter, gradient and moments
         (state step = step - 1).
 
@@ -1130,9 +1231,9 @@ class Shadow:
             p0 = pre["params"][i]
             q = torch.nn.Parameter(p0.to(F64))
             q.grad = g.to(F64)
-            ref = torch.optim.Adam([q], lr=c["lr"], betas=(c["beta1"], c["beta2"]), eps=c["eps"],
+            ref = torch.optim.Adam([q], lr=lr, betas=(c["beta1"], c["beta2"]), eps=c["eps"],
                                    weight_decay=c["weight_decay"], foreach=False)
-            ref.state[q] = {"step": torch.tensor(float(c["step"] - 1)),
+            ref.state[q] = {"step": torch.tensor(float(step - 1)),
                             "exp_avg": pre["exp_avg"][o:o + n].view(p.shape).to(F64),
                             "exp_avg_sq": pre["exp_avg_sq"][o:o + n].view(p.shape).to(F64)}
             ref.step()
@@ -1149,11 +1250,10 @@ class Shadow:
                 s0 = pre["ema_shadow"][o:o + n].to(F64)
                 w = (1.0 - c["ema_decay"]) * p1.reshape(-1).to(F64) + c["ema_decay"] * s0
                 ema.append(image_devs(a["ema_shadow"][o:o + n][None], w[None]))
-        self._record(idx, "adam_multi", form, "dp beyond fp32 resolution", torch.cat(dp), self.bounds["adam_dp"],
-                     shapes)
-        self._record(idx, "adam_multi", form, "exp_avg, exp_avg_sq", torch.cat(mo), self.bounds["adam_moments"], shapes)
+        self._record(idx, method, form, "dp beyond fp32 resolution", torch.cat(dp), self.bounds["adam_dp"], shapes)
+        self._record(idx, method, form, "exp_avg, exp_avg_sq", torch.cat(mo), self.bounds["adam_moments"], shapes)
         if ema:
-            self._record(idx, "adam_multi", form, "EMA shadow", torch.cat(ema), self.bounds["ema"], shapes)
+            self._record(idx, method, form, "EMA shadow", torch.cat(ema), self.bounds["ema"], shapes)
 
     def _ref_ema_multi(self, idx, form, shapes, c, a, pre):
         tab = a["tab"]
@@ -1165,6 +1265,117 @@ class Shadow:
                 w = (1.0 - c["decay"]) * w + c["decay"] * pre["shadow"][o:o + n].to(F64)
             devs.append(image_devs(a["shadow"][o:o + n][None], w[None]))
         self._record(idx, "ema_multi", form, "EMA shadow", torch.cat(devs), self.bounds["ema"], shapes)
+
+    # -- sampling: bridge update, condition, output path ---------------------------------------------------------
+    def _p_sample(self, idx, method, form, shapes, c, a, coef):
+        """The reference's update (oracle.p_sample_update, BrownianBridgeModel.py:174-201) evaluated with fp32 torch
+        ops on the CPU from the launch's seven step coefficients (schedule.step_coefficients), as
+        test_gpu_kernels.py::test_p_sample_update_bit_exact holds the kernel to it: bit for bit."""
+        m_t, om_t, sq, m_nt, om_nt, c_xt, sigma = (torch.tensor(float(v), dtype=torch.float32) for v in coef)
+        x_t, y, eps = (c[k].cpu().float() for k in ("x_t", "y", "eps"))
+        x0 = {"grad": lambda: x_t - eps, "noise": lambda: (x_t - m_t * y - sq * eps) / om_t,
+              "ysubx": lambda: y - eps}[c["objective"]]()
+        if c["clip"]:
+            x0 = x0.clamp(-1.0, 1.0)
+        if c["is_last"]:
+            x1 = x0
+        else:
+            x1 = om_nt * x0 + m_nt * y + c_xt * (x_t - om_t * x0 - m_t * y) + sigma * c["noise"].cpu().float()
+        outs = [("x_{t-1}", a["x_out"], x1)] + ([("x0", a["x0_out"], x0)] if a["x0_out"] is not None else [])
+        for what, got, want in outs:
+            self._record(idx, method, form, what, image_equal(got.cpu(), want), 0.0, shapes)
+
+    def _ref_p_sample(self, idx, form, shapes, c, a, pre):
+        self._p_sample(idx, "p_sample", form, shapes, c, a, c["coef"])
+
+    def _ref_p_sample_dev(self, idx, form, shapes, c, a, pre):
+        self._p_sample(idx, "p_sample_dev", form, shapes, c, a, c["coef_dev"].cpu().tolist())   # pre-launch clone
+
+    def _ref_spatial_rescale(self, idx, form, shapes, c, a, pre):
+        """n_stages bilinear x0.5 interpolations (align_corners False: the mean of each 2x2 block, an odd last row /
+        column dropped), then the optional 1x1 map, in fp64."""
+        x = c["src"].to(F64)
+        for _ in range(c["n_stages"]):
+            H, W = x.shape[2] // 2 * 2, x.shape[3] // 2 * 2
+            x = x[:, :, :H, :W].reshape(x.shape[0], x.shape[1], H // 2, 2, W // 2, 2).mean((3, 5))
+        if c["weight"] is not None:
+            x = torch.einsum("oc,bchw->bohw", c["weight"].to(F64), x)
+            if c["bias"] is not None:
+                x = x + c["bias"].to(F64).view(1, -1, 1, 1)
+        self._record(idx, "spatial_rescale", form, "out", image_devs(a["out"], x), self.bounds["spatial_rescale"],
+                     shapes)
+
+    def _ref_denorm_to_uint8(self, idx, form, shapes, c, a, pre):
+        """runners/utils.py:67-74 of the reference, on the CPU in fp32, as the byte-exact single-kernel test."""
+        x = c["images"].cpu().float()
+        if c["to_normal"]:
+            x = x.mul(0.5).add(0.5).clamp(0, 1.)
+        want = x.mul(255).add(0.5).clamp(0, 255).permute(0, 2, 3, 1).to(torch.uint8)
+        self._record(idx, "denorm_to_uint8", form, "bytes", image_equal(a["out"].cpu(), want), 0.0, shapes)
+
+    # -- VQGAN ends and the space-to-depth operand ---------------------------------------------------------------
+    def _ref_s2d_split(self, idx, form, shapes, c, a, pre):
+        h, l = split_bf16(space_to_depth(c["src"]))
+        self._record(idx, "s2d_split", form, "planes (bit-exact split)",
+                     torch.maximum(image_equal(a["out_hi"], h), image_equal(a["out_lo"], l)), 0.0, shapes)
+
+    def _ref_conv_direct_pad(self, idx, form, shapes, c, a, pre):
+        src, k, cout = c["src"], c["k"], c["cout"]
+        w = c["w_packed"].reshape(k, k, src.shape[3], cout).permute(3, 2, 0, 1).to(F64)
+        p = (c["pad_lo"], c["pad_hi"])
+        devs = []
+        for sl in chunks(src.shape[0], src[0].numel() * 8 * 4, src.device):
+            x = F.pad(src[sl].to(F64).permute(0, 3, 1, 2), p + p)
+            o = F.conv2d(x, w, None if c["bias"] is None else c["bias"].to(F64), stride=c["stride"]).permute(0, 2, 3, 1)
+            if c["residual"] is not None:
+                o = o + c["residual"][sl].to(F64)
+            devs.append(image_devs(a["out"][sl], o))
+        self._record(idx, "conv_direct_pad", form, "out", torch.cat(devs), self.bounds["conv_direct_pad"], shapes)
+
+    def _ref_softmax_rows_split(self, idx, form, shapes, c, a, pre):
+        """Per row: fp64 softmax(scale * s) against hi + lo, and hi, lo a split pair."""
+        s = c["src"]
+        n = s.shape[-1]
+        hi, lo = a["out_hi"].reshape(-1, n), a["out_lo"].reshape(-1, n)
+        want = torch.softmax(s.reshape(-1, n).to(F64) * c["scale"], dim=-1)
+        self._record(idx, "softmax_rows_split", form, "rows hi + lo", image_devs(planes(hi, lo), want),
+                     self.bounds["softmax"], shapes)
+        self._record(idx, "softmax_rows_split", form, "rows split", pair_well_formed(hi, lo), 0.0, shapes)
+
+    def _ref_vq_nearest(self, idx, form, shapes, c, a, pre):
+        """Per image: the chosen code's fp64 squared distance within fp32 noise of the fp64 minimum, the index equal to
+        the fp64 argmin wherever the top-2 gap is clear of that noise, and z_q = z + (e - z) (the reference's
+        straight-through expression) bit for bit.  Distances are in units of 1 + |z|^2 + |e|^2, the magnitude of the
+        terms an fp32 evaluation sums."""
+        z, cb = c["z"], c["codebook"]
+        B, D = z.shape[0], cb.shape[1]
+        zf = z.reshape(B, -1, D)
+        idx_got = a["indices"].reshape(B, -1)
+        cb64 = cb.to(F64)
+        gap_dev, idx_dev, zq_dev = [], [], []
+        for b in range(B):
+            for r0 in range(0, zf.shape[1], 4096):
+                zr = zf[b, r0:r0 + 4096].to(F64)
+                d = torch.cdist(zr, cb64) ** 2
+                top = d.topk(2, dim=1, largest=False)
+                chosen = a["indices"].reshape(B, -1)[b, r0:r0 + 4096]
+                ok_range = bool(((chosen >= 0) & (chosen < cb.shape[0])).all())
+                ci = chosen.clamp(0, cb.shape[0] - 1)
+                scale = 1.0 + (zr * zr).sum(1) + (cb64[ci] * cb64[ci]).sum(1)
+                excess = (d.gather(1, ci[:, None])[:, 0] - top.values[:, 0]) / scale
+                gap_dev.append(float(excess.max()) if ok_range else math.inf)
+                clear = (top.values[:, 1] - top.values[:, 0]) / scale > self.bounds["vq_distance"]
+                idx_dev.append(0.0 if ok_range and torch.equal(chosen[clear], top.indices[clear, 0]) else math.inf)
+                zr32 = zf[b, r0:r0 + 4096]
+                e = cb[ci]
+                want = zr32 + (e - zr32)
+                got = a["z_q"].reshape(B, -1, D)[b, r0:r0 + 4096]
+                zq_dev.append(0.0 if torch.equal(got, want) else math.inf)
+        per = lambda v: torch.tensor(v, dtype=F64).reshape(B, -1).amax(1)
+        self._record(idx, "vq_nearest", form, "chosen distance - minimum", per(gap_dev), self.bounds["vq_distance"],
+                     shapes)
+        self._record(idx, "vq_nearest", form, "index where the top-2 gap is clear", per(idx_dev), 0.0, shapes)
+        self._record(idx, "vq_nearest", form, "z_q = z + (e - z) (bit-exact)", per(zq_dev), 0.0, shapes)
 
 
 # ------------------------------------------------------------------------------------------------ coverage
