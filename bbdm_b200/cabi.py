@@ -17,7 +17,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BBDM_LIB selects another in-tree build of the same sources (A/B experiments, tools/); the product default is fixed
 LIB_PATH = os.environ.get("BBDM_LIB") or os.path.join(_HERE, "libbbdm_b200.so")
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 OBJ = {"grad": 0, "noise": 1, "ysubx": 2}
 RESAMPLE_NONE, RESAMPLE_UP2, RESAMPLE_DOWN2 = 0, 1, 2
 RES_NONE, RES_SAME, RES_UP2, RES_DOWN2 = 0, 1, 2, 3
@@ -169,7 +169,7 @@ def load():
     lib.bbdm_attention_tc.argtypes = [vp, vp, i, i, i, i, i, vp, vp, vp, vp]
     lib.bbdm_attention_bwd.argtypes = [vp, vp, vp, i, i, i, i, i, vp, vp, vp, vp]
     lib.bbdm_conv_direct_pad.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, i, i, i, i, i, vp]
-    lib.bbdm_softmax_rows_split.argtypes = [vp, i64, i64, C.c_float, vp, vp, vp]
+    lib.bbdm_softmax_rows_split.argtypes = [vp, i64, i64, i64, C.c_float, vp, vp, vp]
     lib.bbdm_vq_nearest.argtypes = [vp, vp, i64, i, i, vp, vp, vp]
     lib.bbdm_s2d_split.argtypes = [vp, i, i, i, i, vp, vp, vp]
     lib.bbdm_pack_weight_split_both.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp]
@@ -644,9 +644,11 @@ class CudaBackend:
                                             B, H, W, Cin, cout, k, stride, pad_lo, pad_hi, stream()))
         LAUNCHES["n"] += 1
 
-    def softmax_rows_split(self, src, scale, out_hi, out_lo):
+    def softmax_rows_split(self, src, scale, out_hi, out_lo, valid_cols=None):
+        """valid_cols: the columns of each row the softmax covers (None: all); the planes are zero in the rest."""
         rows, cols = src.numel() // src.shape[-1], src.shape[-1]
-        check(self.lib.bbdm_softmax_rows_split(ptr(_req(src)), rows, cols, float(scale), ptr(_req(out_hi, torch.bfloat16)),
+        check(self.lib.bbdm_softmax_rows_split(ptr(_req(src)), rows, cols, cols if valid_cols is None else int(valid_cols),
+                                               float(scale), ptr(_req(out_hi, torch.bfloat16)),
                                                ptr(_req(out_lo, torch.bfloat16)), stream()))
         LAUNCHES["n"] += 1
 

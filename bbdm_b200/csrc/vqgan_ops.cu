@@ -1,6 +1,6 @@
 // The two VQGAN-specific steps either side of the latent bridge loop :
-//   * row softmax of the single-head AttnBlock's T x T score matrix, written as split-bf16 planes
-//     (the A operand of the P.V tensor-core GEMM)                      model/VQGAN/model.py:140-192
+//   * row softmax of the single-head AttnBlock's T x Tp score matrix (Tp = T rounded up to 64, the padding columns
+//     masked), written as split-bf16 planes (the A operand of the P.V tensor-core GEMM)   model/VQGAN/model.py:140-192
 //   * VectorQuantizer2 nearest-codebook lookup                          model/VQGAN/quantize.py:271-312
 // Everything else of the autoencoder (ResnetBlocks, 1x1/3x3 convs, GroupNorm, resampling) runs on the
 // same kernels as the UNet.
@@ -26,31 +26,48 @@ __device__ __forceinline__ float block_reduce(float v, float* red, bool is_max) 
 // exp(scale*s - m) with the product rounded first, as the reference scales the scores before its softmax
 __device__ __forceinline__ float sexp(float s, float scale, float m) { return expf(__fsub_rn(__fmul_rn(s, scale), m)); }
 
-// one CTA per row: p = softmax(scale * s) -> hi/lo planes.  N % 4 == 0.
+// columns i+1..i+3 of a float4 at or past V take `fill` (column i < V is the caller's condition)
+__device__ __forceinline__ void mask_tail(float4& v, int64_t i, int64_t V, float fill) {
+  if (i + 1 >= V) v.y = fill;
+  if (i + 2 >= V) v.z = fill;
+  if (i + 3 >= V) v.w = fill;
+}
+
+// one CTA per row: p = softmax(scale * s) over the first V columns -> hi/lo planes, exact zeros in columns V..N-1
+// (the padding of a key axis rounded up to the GEMM's 64-column tile).  N % 4 == 0, 0 < V <= N; MASKED == (V < N).
+// Only the float4 that straddles V is masked, so the first V columns see the unmasked arithmetic and reduction order.
+template <bool MASKED>
 __global__ void __launch_bounds__(256)
-softmax_rows_split_kernel(const float* __restrict__ src, int64_t N, float scale, __nv_bfloat16* __restrict__ hi,
-                          __nv_bfloat16* __restrict__ lo) {
+softmax_rows_split_kernel(const float* __restrict__ src, int64_t N, int64_t V, float scale,
+                          __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
   __shared__ float red[8];
   const float* row = src + (int64_t)blockIdx.x * N;
   float mx = -INFINITY;
-  for (int64_t i = threadIdx.x * 4; i < N; i += 1024) {
-    const float4 v = ld_f4(row + i);
+  for (int64_t i = threadIdx.x * 4; i < V; i += 1024) {
+    float4 v = ld_f4(row + i);
+    if (MASKED && i + 4 > V) mask_tail(v, i, V, -INFINITY);
     mx = fmaxf(fmaxf(mx, fmaxf(v.x, v.y)), fmaxf(v.z, v.w));
   }
   // scale > 0: max(scale * s) = scale * max(s) exactly (monotone rounding)
   const float m = block_reduce(mx, red, true) * scale;
   float sum = 0.f;
-  for (int64_t i = threadIdx.x * 4; i < N; i += 1024) {
+  for (int64_t i = threadIdx.x * 4; i < V; i += 1024) {
     const float4 v = ld_f4(row + i);
-    sum += sexp(v.x, scale, m) + sexp(v.y, scale, m) + sexp(v.z, scale, m) + sexp(v.w, scale, m);
+    float4 e = make_float4(sexp(v.x, scale, m), sexp(v.y, scale, m), sexp(v.z, scale, m), sexp(v.w, scale, m));
+    if (MASKED && i + 4 > V) mask_tail(e, i, V, 0.f);
+    sum += e.x + e.y + e.z + e.w;
   }
   const float inv = 1.0f / block_reduce(sum, red, false);
   __nv_bfloat16* h = hi + (int64_t)blockIdx.x * N;
   __nv_bfloat16* l = lo + (int64_t)blockIdx.x * N;
   for (int64_t i = threadIdx.x * 4; i < N; i += 1024) {
-    const float4 v = ld_f4(row + i);
-    const float4 p = make_float4(sexp(v.x, scale, m) * inv, sexp(v.y, scale, m) * inv, sexp(v.z, scale, m) * inv,
-                                 sexp(v.w, scale, m) * inv);
+    float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (!MASKED || i < V) {
+      const float4 v = ld_f4(row + i);
+      p = make_float4(sexp(v.x, scale, m) * inv, sexp(v.y, scale, m) * inv, sexp(v.z, scale, m) * inv,
+                      sexp(v.w, scale, m) * inv);
+      if (MASKED && i + 4 > V) mask_tail(p, i, V, 0.f);
+    }
     uint2 ph, pl;
     split4(p, ph, pl);
     *reinterpret_cast<uint2*>(h + i) = ph;
@@ -144,13 +161,19 @@ extern "C" int bbdm_s2d_split(const float* src, int B, int H, int W, int C, void
   return BBDM_OK;
 }
 
-extern "C" int bbdm_softmax_rows_split(const float* src, int64_t rows, int64_t cols, float scale, void* out_hi,
-                                       void* out_lo, void* stream) {
+extern "C" int bbdm_softmax_rows_split(const float* src, int64_t rows, int64_t cols, int64_t valid_cols, float scale,
+                                       void* out_hi, void* out_lo, void* stream) {
   BBDM_REQUIRE(src && out_hi && out_lo, "softmax_rows_split: null pointer");
   BBDM_REQUIRE(rows > 0 && rows < (1ll << 31) && cols > 0 && cols % 4 == 0 && scale > 0.f,
                "softmax_rows_split: bad shape (cols must be a multiple of 4, scale > 0)");
-  softmax_rows_split_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(
-      src, cols, scale, (__nv_bfloat16*)out_hi, (__nv_bfloat16*)out_lo);
+  BBDM_REQUIRE(valid_cols > 0 && valid_cols <= cols, "softmax_rows_split: valid_cols %lld not in 1..cols = %lld",
+               (long long)valid_cols, (long long)cols);
+  if (valid_cols == cols)
+    softmax_rows_split_kernel<false><<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(
+        src, cols, cols, scale, (__nv_bfloat16*)out_hi, (__nv_bfloat16*)out_lo);
+  else
+    softmax_rows_split_kernel<true><<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(
+        src, cols, valid_cols, scale, (__nv_bfloat16*)out_hi, (__nv_bfloat16*)out_lo);
   BBDM_LAUNCH_CHECK();
   return BBDM_OK;
 }

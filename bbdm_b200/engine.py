@@ -38,6 +38,7 @@ class _Pool:
 
     def __init__(self, backend, device):
         self.be, self.device, self.free = backend, device, {}
+        self.padded = {}
         self.bytes = 0
         _Pool._serial += 1
         self.serial = _Pool._serial          # identity of this set of buffers (captured graphs key on it)
@@ -49,6 +50,16 @@ class _Pool:
             return lst.pop()
         t = self.be.empty(tuple(shape), dtype, self.device)
         self.bytes += t.numel() * t.element_size()
+        return t
+
+    def zero_padded(self, tag, shape, dtype=torch.float32):
+        """The buffer `tag` of this shape, zeroed once when allocated and never put on the free lists: for operands
+        whose users all write the same leading rows or columns and rely on the rest staying zero from call to call."""
+        key = (tag, tuple(shape), dtype)
+        t = self.padded.get(key)
+        if t is None:
+            t = self.padded[key] = self.be.empty(tuple(shape), dtype, self.device).zero_()
+            self.bytes += t.numel() * t.element_size()
         return t
 
     def put(self, *ts):

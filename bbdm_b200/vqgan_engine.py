@@ -9,7 +9,8 @@ container, exactly like the UNet) and issues the same kernels as the UNet execut
                                   GN eps 1e-6: the 1x1 nin_shortcut rides as extra K-blocks of conv2, the identity
                                   skip as its residual
   AttnBlock   (model.py:140-192)  single head of width C: C <= 64 -> the flash kernels; C >= 128 -> per image two
-                                  tensor-core GEMMs (S = Q K^T, O = P V) around bbdm_softmax_rows_split
+                                  tensor-core GEMMs (S = Q K^T, O = P V) around bbdm_softmax_rows_split, the key axis
+                                  zero-padded to a multiple of 64 and masked in the softmax at any other token count
   Downsample  (model.py:55-73)    zero-pad (0,1,0,1) + stride-2 conv = space-to-depth split + 2x2-tap wgmma conv
                                   (bbdm_conv_direct_pad for unaligned channel counts)
   Upsample    (model.py:38-53)    nearest-2x + conv3x3 = the fused 4-phase wgmma conv (no upsampled tensor)
@@ -108,9 +109,12 @@ class VQGANEngine(KernelExecutor):
             be.attention(qkv.view(B, T, 3 * Cc), 1, 1, None if o_f32 is None else o_f32.view(B, T, Cc),
                          None if o_hi is None else o_hi.view(B, T, Cc), None if o_lo is None else o_lo.view(B, T, Cc))
             pool.put(qkv)
+        elif not umma:
+            raise NotImplementedError(f"VQGAN AttnBlock with C={Cc} on a {H}x{W} map: the GEMM-composed attention "
+                                      f"needs C % 64 == 0 and a map at least 4 wide")
+        elif T % 64:
+            o_hi, o_lo = self._attn_padded(pool, name, a_hi, a_lo, x.shape)
         else:
-            if not (umma and T % 64 == 0):
-                raise NotImplementedError(f"VQGAN AttnBlock with C={Cc}, T={T}: needs C % 64 == 0 and T % 64 == 0")
             _, q_hi, q_lo = self._conv(pool, w[name + ".q"], a_hi=a_hi, a_lo=a_lo, shape=(B, H, W), out_split=True,
                                        want_f32=False)
             _, k_hi, k_lo = self._conv(pool, w[name + ".k"], a_hi=a_hi, a_lo=a_lo, shape=(B, H, W), out_split=True,
@@ -137,6 +141,39 @@ class VQGANEngine(KernelExecutor):
                                res_mode=cabi.RES_SAME, stats=True)
         pool.put(o_f32, o_hi, o_lo)
         return out
+
+    def _attn_padded(self, pool, name, a_hi, a_lo, shape):
+        """The GEMM-composed AttnBlock at a token count T that is not a multiple of 64: the key axis is padded to
+        Tp = T rounded up to 64.  Each image's k 1x1 conv writes the first T rows of [Tp][C] K planes and its V^T the
+        first T columns of [C][Tp] planes, both zero beyond; S = Q K^T then has Tp columns, the softmax covers the first
+        T of them and writes zeros past them, and O = P V runs over K = Tp.  Returns O's split planes."""
+        be, w = self.be, self._w
+        B, H, W, Cc = shape
+        T = H * W
+        Tp = -(-T // 64) * 64
+        bf16 = torch.bfloat16
+        ek = w[name + ".k"]
+        _, q_hi, q_lo = self._conv(pool, w[name + ".q"], a_hi=a_hi, a_lo=a_lo, shape=(B, H, W), out_split=True,
+                                   want_f32=False)
+        v, _, _ = self._conv(pool, w[name + ".v"], a_hi=a_hi, a_lo=a_lo, shape=(B, H, W))
+        k_pl = pool.zero_padded(("attention K", T), (2, Tp, Cc), bf16)
+        vt_pl = pool.zero_padded(("attention V^T", T), (2, Cc, Tp), bf16)
+        o_hi, o_lo = pool.get(shape, bf16), pool.get(shape, bf16)
+        s = pool.get((1, H, W, Tp))
+        p_hi, p_lo = pool.get((1, H, W, Tp), bf16), pool.get((1, H, W, Tp), bf16)
+        scale = float(int(Cc) ** (-0.5))
+        for b in range(B):
+            be.conv_umma(B=1, H=H, W=W, Cin=Cc, Cout=Cc, taps=1, a_hi=a_hi[b:b + 1], a_lo=a_lo[b:b + 1], w_hi=ek["hi"],
+                         w_lo=ek["lo"], bias=ek["bias"], out=None, out_hi=k_pl[0, :T].view(1, H, W, Cc),
+                         out_lo=k_pl[1, :T].view(1, H, W, Cc), passes=self.passes)
+            be.split_grad(v[b].view(T, Cc), None, None, vt_pl[0, :, :T], vt_pl[1, :, :T])
+            be.conv_umma(B=1, H=H, W=W, Cin=Cc, Cout=Tp, taps=1, a_hi=q_hi[b:b + 1], a_lo=q_lo[b:b + 1],
+                         w_hi=k_pl[0:1], w_lo=k_pl[1:2], out=s, passes=self.passes)
+            be.softmax_rows_split(s.view(T, Tp), scale, p_hi.view(T, Tp), p_lo.view(T, Tp), valid_cols=T)
+            be.conv_umma(B=1, H=H, W=W, Cin=Tp, Cout=Cc, taps=1, a_hi=p_hi, a_lo=p_lo, w_hi=vt_pl[0:1],
+                         w_lo=vt_pl[1:2], out=None, out_hi=o_hi[b:b + 1], out_lo=o_lo[b:b + 1], passes=self.passes)
+        pool.put(q_hi, q_lo, v, s, p_hi, p_lo)
+        return o_hi, o_lo
 
     def _downsample(self, pool, name, m, x):
         B, H, W, Cc = x.shape

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define BBDM_ABI_VERSION 7
+#define BBDM_ABI_VERSION 8
 
 enum {
   BBDM_OK = 0,
@@ -545,9 +545,11 @@ int bbdm_attention_bwd(const float* qkv, const float* out, const float* dout, in
 
 /* ---- VQGAN ends of the latent models ---------------------------------------
  * Row softmax of a [rows, cols] fp32 score matrix, p = softmax(scale * s), written as split-bf16 planes
- * (A operand of the P.V GEMM of the single-head AttnBlock, model/VQGAN/model.py:168-183). cols % 4 == 0. */
-int bbdm_softmax_rows_split(const float* src, int64_t rows, int64_t cols, float scale, void* out_hi,
-                            void* out_lo, void* stream);
+ * (A operand of the P.V GEMM of the single-head AttnBlock, model/VQGAN/model.py:168-183). cols % 4 == 0.
+ * Only the first valid_cols (1..cols) columns of a row enter its max and sum; the planes hold exact zeros in
+ * the rest (the padding of a token axis rounded up to the GEMM tile).  valid_cols == cols: the whole row. */
+int bbdm_softmax_rows_split(const float* src, int64_t rows, int64_t cols, int64_t valid_cols, float scale,
+                            void* out_hi, void* out_lo, void* stream);
 
 /* Space-to-depth by 2 with bf16 split: src [B,H,W,C] fp32 -> planes [B,H/2,W/2,4C], channel
  * (row parity*2 + col parity)*C + c.  With it the VQGAN Downsample (zero-pad (0,1,0,1) + 3x3 stride-2 conv,

@@ -2,9 +2,15 @@
 """VQGAN ends at the BASELINE configs[2] shape (LBBDM-f4: images [B,3,256,256] <-> latents [B,3,64,64], ch 128,
 mult (1,2,4), 8192 codes): VQGANEngine (split-bf16 x3, fp32-class) vs the same graph on the PyTorch library path
 (fp32 / TF32 / bf16 autocast).  One encode = what LatentBrownianBridgeModel.encode costs (twice per training
-sample, once per sampled batch); one decode = quantize + post_quant_conv + decoder."""
+sample, once per sampled batch); one decode = quantize + post_quant_conv + decoder.
+
+    python tools/bench_vqgan.py [B]                                  the f4 table above (B = 32)
+    python tools/bench_vqgan.py --size 224 --template f8 [--batch 4]  one template autoencoder at one image size:
+        native encode / decode against the module path the latent model otherwise takes (the same graph in stock
+        PyTorch with torch's default TF32 convolutions), with the card's name and power limit"""
 import json
 import os
+import subprocess
 import sys
 
 import torch
@@ -15,6 +21,12 @@ from bbdm_b200.vqgan import VQModel  # noqa: E402
 
 DD = dict(double_z=False, z_channels=3, resolution=256, in_channels=3, out_ch=3, ch=128, ch_mult=(1, 2, 4),
           num_res_blocks=2, attn_resolutions=[], dropout=0.0)
+# Template-LBBDM-f4 / f8 / f16 autoencoders: (ddconfig, n_embed, embed_dim)
+TEMPLATES = {
+    "f4": (DD, 8192, 3),
+    "f8": (dict(DD, z_channels=4, ch_mult=(1, 2, 2, 4), attn_resolutions=[32]), 16384, 4),
+    "f16": (dict(DD, z_channels=16, ch_mult=(1, 1, 2, 2, 4), attn_resolutions=[16]), 16384, 16),
+}
 
 
 # ---- stock-PyTorch forward of the same parameter tree (library baseline only) ------------------------------
@@ -46,8 +58,10 @@ def lib_encode(vq, x):
     e = vq.encoder
     h = e.conv_in(x)
     for i in range(e.num_resolutions):
-        for blk in e.down[i].block:
+        for j, blk in enumerate(e.down[i].block):
             h = resnet(blk, h)
+            if len(e.down[i].attn) > 0:
+                h = attn(e.down[i].attn[j], h)
         if i != e.num_resolutions - 1:
             h = e.down[i].downsample.conv(F.pad(h, (0, 1, 0, 1)))
     return vq.quant_conv(e.conv_out(F.silu(gn(e.norm_out, mid(e.mid, h)))))
@@ -65,8 +79,10 @@ def lib_decode(vq, z, idx=None, return_idx=False):
     dcd = vq.decoder
     h = mid(dcd.mid, dcd.conv_in(vq.post_quant_conv(zq)))
     for i in reversed(range(dcd.num_resolutions)):
-        for blk in dcd.up[i].block:
+        for j, blk in enumerate(dcd.up[i].block):
             h = resnet(blk, h)
+            if len(dcd.up[i].attn) > 0:
+                h = attn(dcd.up[i].attn[j], h)
         if i != 0:
             h = dcd.up[i].upsample.conv(F.interpolate(h, scale_factor=2.0, mode="nearest"))
     return dcd.conv_out(F.silu(gn(dcd.norm_out, h)))
@@ -85,15 +101,52 @@ def timeit(fn, steps=5, warmup=2):
     return e0.elapsed_time(e1) / steps
 
 
-def main():
-    B = int(sys.argv[1]) if len(sys.argv) > 1 and sys.argv[1].isdigit() else 32
+def make_vq(template):
+    dd, n_embed, embed_dim = TEMPLATES[template]
     torch.manual_seed(0)
-    vq = VQModel(ddconfig=DD, n_embed=8192, embed_dim=3).eval().cuda()
+    vq = VQModel(ddconfig=dd, n_embed=n_embed, embed_dim=embed_dim).eval().cuda()
     with torch.no_grad():
         for n, p in vq.named_parameters():
             if p.dim() >= 2:
                 p.normal_(0, 0.02)
         vq.quantize.embedding.weight.normal_(0, 0.5)
+    return vq
+
+
+def _arg(name, default):
+    return type(default)(sys.argv[sys.argv.index(name) + 1]) if name in sys.argv else default
+
+
+def size_mode():
+    """One template autoencoder at one image size: native encode / decode vs the module path at torch's defaults."""
+    size, template, B = _arg("--size", 256), _arg("--template", "f8"), _arg("--batch", 4)
+    steps, warmup = _arg("--steps", 10), _arg("--warmup", 3)
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                         text=True).stdout.strip()
+    vq = make_vq(template)
+    f = 2 ** (len(TEMPLATES[template][0]["ch_mult"]) - 1)
+    x = (0.5 * torch.randn(B, 3, size, size, device="cuda")).clamp_(-1, 1)
+    with torch.no_grad():
+        eng = vq.engine()
+        z = eng.encode(x)
+        lat = z + 0.2 * torch.randn_like(z)
+        native = {"encode_ms": timeit(lambda: eng.encode(x), steps, warmup),
+                  "decode_ms": timeit(lambda: eng.decode(lat), steps, warmup)}
+        module = {"encode_ms": timeit(lambda: lib_encode(vq, x), steps, warmup),
+                  "decode_ms": timeit(lambda: lib_decode(vq, lat), steps, warmup)}
+        dev = lambda a, b: float((a - b).abs().max() / b.abs().max())
+        z_mod = lib_encode(vq, x)
+    print(json.dumps({"what": f"VQGAN-{template} ends, images [{B},3,{size},{size}], attention map {size // f}^2 "
+                              f"(T = {(size // f) ** 2})", "gpu": smi, "native split3": native,
+                      "module path (torch defaults: cudnn.allow_tf32=%s)" % torch.backends.cudnn.allow_tf32: module,
+                      "encode_rel_dev_native_vs_module": dev(z, z_mod)}))
+
+
+def main():
+    if "--size" in sys.argv:
+        return size_mode()
+    B = int(sys.argv[1]) if len(sys.argv) > 1 and sys.argv[1].isdigit() else 32
+    vq = make_vq("f4")
     x = (0.5 * torch.randn(B, 3, 256, 256, device="cuda")).clamp_(-1, 1)
     rows = []
     torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False     # true-fp32 reference values
