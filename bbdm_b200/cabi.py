@@ -17,7 +17,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BBDM_LIB selects another in-tree build of the same sources (A/B experiments, tools/); the product default is fixed
 LIB_PATH = os.environ.get("BBDM_LIB") or os.path.join(_HERE, "libbbdm_b200.so")
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 OBJ = {"grad": 0, "noise": 1, "ysubx": 2}
 RESAMPLE_NONE, RESAMPLE_UP2, RESAMPLE_DOWN2 = 0, 1, 2
 RES_NONE, RES_SAME, RES_UP2, RES_DOWN2 = 0, 1, 2, 3
@@ -285,6 +285,8 @@ class CudaBackend:
     # conv_umma / conv_wgrad take window_origin: the 2x2 window of taps = 4 at rows/cols -1..0 as well as 0..1 (the
     # UNet's stride-2 conv on a space-to-depth operand and the adjoints of it and of the nearest-2x conv)
     window_origin = True
+    # conv_umma / conv_wgrad take channel counts that are multiples of 32 (a backend without this attribute: 64)
+    conv_channel_multiple = 32
 
     def __init__(self):
         self.lib = load()

@@ -27,12 +27,19 @@ WINO_MIN_C = int(os.environ.get("BBDM_WINO_MIN_C", "256"))
 WINO_MIN_TILES = int(os.environ.get("BBDM_WINO_MIN_TILES", "512"))
 
 
-def tensor_core_ok(cin, cout, w):
+def channel_multiple(be):
+    """The channel multiple the backend's tensor-core convolutions take (its conv_channel_multiple; 64 when it does not
+    declare one)."""
+    return getattr(be, "conv_channel_multiple", 64)
+
+
+def tensor_core_ok(cin, cout, w, multiple=64):
     """Convolutions the tensor-core kernels take, in sampling (bbdm_conv_umma) and in training (its data gradient and
-    bbdm_conv_wgrad): channel counts that are multiples of 64 and a map at least 4 pixels wide.  Any height and batch:
-    the forward covers ragged map edges with zero-filled tile boxes, the weight gradient reads its 64-pixel K blocks in
-    TMA im2col mode wherever they wrap across rows and images."""
-    return cin % 64 == 0 and cout % 64 == 0 and w >= 4
+    bbdm_conv_wgrad): channel counts that are multiples of ``multiple`` (channel_multiple of the backend: 32 for
+    CudaBackend) and a map at least 4 pixels wide.  Any height and batch: the forward covers ragged map edges with
+    zero-filled tile boxes, the weight gradient reads its 64-pixel K blocks in TMA im2col mode wherever they wrap across
+    rows and images."""
+    return cin % multiple == 0 and cout % multiple == 0 and w >= 4
 
 
 def wino_channels_ok(cin, cout, min_c, tile=4):
@@ -150,12 +157,13 @@ class WeightPacker:
     swapped in and out, and every address a captured CUDA graph holds stays valid.
 
     An entry has cout, cin, k, bias, f32 [k*k][Cin][Cout], and split-bf16 hi/lo [k*k][Cout][Cin] when both channel
-    counts are multiples of 64.  The caller decides which convs also get a zero-padded head (padded_head), Winograd
+    counts are multiples of ``multiple`` (the executor's tensor-core channel multiple).  The caller decides which convs also get a zero-padded head (padded_head), Winograd
     planes (winograd), the fused nearest-2x phase planes (up_phase) or the space-to-depth planes of a stride-2 conv
     (stride2)."""
 
-    def __init__(self, be, device, old=None):
+    def __init__(self, be, device, old=None, multiple=64):
         self.be, self.device, self.old, self.w = be, device, old or {}, {}
+        self.multiple = multiple
 
     def _buf(self, name, field, shape, dtype):
         ent = self.old.get(name)
@@ -173,11 +181,12 @@ class WeightPacker:
         wt = wt.contiguous()
         cout, cin, k = wt.shape[0], wt.shape[1], wt.shape[2]
         ent = {"cout": cout, "cin": cin, "k": k, "bias": None if bias is None else bias.detach()}
-        if cin % 64 == 0 and cout % 64 == 0 and k in (1, 3):
+        m = self.multiple
+        if cin % m == 0 and cout % m == 0 and k in (1, 3):
             ent["hi"] = self._buf(name, "hi", (k * k, cout, cin), torch.bfloat16)
             ent["lo"] = self._buf(name, "lo", (k * k, cout, cin), torch.bfloat16)
             be.pack_weight_split(wt, ent["hi"], ent["lo"])
-        elif padded_head and cin % 64 == 0 and cout < 64 and k == 3:
+        elif padded_head and cin % m == 0 and cout < 64 and k == 3:
             prev = self.old[name].get("hi_pad") if isinstance(self.old.get(name), dict) else None
             hi = self._buf(name, "hi_pad", (k * k, 64, cin), torch.bfloat16)
             lo = self._buf(name, "lo_pad", (k * k, 64, cin), torch.bfloat16)

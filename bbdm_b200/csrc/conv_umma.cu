@@ -5,6 +5,10 @@
 //
 //   * M tile = 128 output pixels = a (TW x TH x TB) box of the NHWC tensor; N tile = BN couts (64 or 128);
 //     K block = 64 input channels of one filter tap.
+//   * Channel counts are multiples of 32.  A K block that runs past Cin (Cin2) reads zeros: the TMA zero-fills the
+//     activation and weight boxes past the end of their channel dimension.  The last N block may run 32 or 96 couts
+//     past Cout; an epilogue slice (BN / 4 columns: 16 or 32) then lies wholly inside or wholly past Cout, and the
+//     slices past it are skipped.
 //   * Operands are split planes (hi, lo) in bf16 or fp16.  passes=3 issues A_lo.W_hi + A_hi.W_lo + A_hi.W_hi
 //     into the same accumulator (fp32-class accuracy); passes=1 issues A_hi.W_hi only.
 //   * TMA (cp.async.bulk.tensor, 4-D tiled map, SWIZZLE_128B) stages the shifted pixel box of a
@@ -40,9 +44,9 @@ constexpr int UM_SLICES = 4;     // epilogue slices per tile, each BN / 32 colum
 struct ConvParams {
   int B, H, W, Cout;
   int TW, TH, TB, tiles_w, tiles_h, tiles_b, n_tiles;
-  int kb_per_tap;   // Cin / 64
-  int K1;           // taps * Cin/64
-  int K2;           // Cin2 / 64
+  int kb_per_tap;   // ceil(Cin / 64)
+  int K1;           // taps * kb_per_tap
+  int K2;           // ceil(Cin2 / 64)
   int taps;
   int up2;           // 1: fused nearest-2x upsample (4 output phases x 2x2 taps on the low-res input)
   int origin;        // taps == 4: first row / column of the 2x2 window (0 or -1)
@@ -118,6 +122,7 @@ template <int BN>
 __device__ __forceinline__ void epi_slice(const ConvParams& p, const float* racc, EpiTile e, int s, int warp,
                                           int lane, float (*stats_s)[BN][2]) {
   constexpr int JS = BN / 8 / UM_SLICES;
+  if (e.nb * BN + s * (BN / UM_SLICES) >= p.Cout) return;   // past the last cout (warp-uniform)
   // opaque tile coordinates: otherwise the compiler hoists every slice's address arithmetic out of the K loop the
   // slice runs in, and those addresses would occupy registers (and spill) for the whole loop
   asm volatile("" : "+r"(e.nb), "+r"(e.bb[0]), "+r"(e.bb[1]), "+r"(e.hh[0]), "+r"(e.hh[1]), "+r"(e.ww[0]),
@@ -232,6 +237,7 @@ __device__ __forceinline__ void epi_stats_out(const ConvParams& p, const EpiTile
   asm volatile("" : "+r"(i0));   // keeps this loop's per-thread indices from being held across the tile loop
   for (int i = i0; i < 4 * BN; i += 256) {
     const int q = i / BN, c = i % BN;
+    if (e.nb * BN + c >= p.Cout) continue;
     const float s = stats_s[2 * q][c][0] + stats_s[2 * q + 1][c][0];
     const float sq = stats_s[2 * q][c][1] + stats_s[2 * q + 1][c][1];
     *reinterpret_cast<float2*>(p.stats + ((tile_lin + q) * p.Cout + e.nb * BN + c) * 2) = make_float2(s, sq);
@@ -283,7 +289,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
   }
   __syncthreads();
 
-  const int n_blocks = p.Cout / BN;
+  const int n_blocks = (p.Cout + BN - 1) / BN;
   const int total_tiles = p.n_tiles * n_blocks * (p.up2 ? 4 : 1);
   const int KB = p.K1 + p.K2;
 
@@ -495,9 +501,9 @@ extern "C" int bbdm_conv_umma(const BbdmConvArgs* a, void* stream) {
   BBDM_REQUIRE(a->B > 0 && a->H > 0 && a->W > 0, "conv_umma: bad spatial shape");
   BBDM_REQUIRE(a->taps == 1 || a->taps == 9 || a->taps == 4, "conv_umma: taps must be 1, 4 or 9 (got %d)", a->taps);
   BBDM_REQUIRE(!a->upsample2x || (a->taps == 4 && a->Cin2 == 0), "conv_umma: upsample2x needs the 16 phase taps and no fused 1x1");
-  BBDM_REQUIRE(a->Cin > 0 && a->Cin % 64 == 0, "conv_umma: Cin %% 64 != 0 (Cin=%d)", a->Cin);
-  BBDM_REQUIRE(a->Cout > 0 && a->Cout % 64 == 0, "conv_umma: Cout %% 64 != 0 (Cout=%d)", a->Cout);
-  BBDM_REQUIRE(a->Cin2 >= 0 && a->Cin2 % 64 == 0, "conv_umma: Cin2 %% 64 != 0 (Cin2=%d)", a->Cin2);
+  BBDM_REQUIRE(a->Cin > 0 && a->Cin % 32 == 0, "conv_umma: Cin %% 32 != 0 (Cin=%d)", a->Cin);
+  BBDM_REQUIRE(a->Cout > 0 && a->Cout % 32 == 0, "conv_umma: Cout %% 32 != 0 (Cout=%d)", a->Cout);
+  BBDM_REQUIRE(a->Cin2 >= 0 && a->Cin2 % 32 == 0, "conv_umma: Cin2 %% 32 != 0 (Cin2=%d)", a->Cin2);
   BBDM_REQUIRE(a->passes == 1 || a->passes == 3, "conv_umma: passes must be 1 or 3");
   BBDM_REQUIRE(a->a_hi && a->w_hi && (a->passes == 1 || (a->a_lo && a->w_lo)), "conv_umma: missing operand plane");
   if (a->Cin2) BBDM_REQUIRE(a->a2_hi && a->w2_hi && (a->passes == 1 || (a->a2_lo && a->w2_lo)), "conv_umma: missing 1x1 operand plane");
@@ -512,6 +518,7 @@ extern "C" int bbdm_conv_umma(const BbdmConvArgs* a, void* stream) {
                "conv_umma: window_origin -1 needs taps == 4 and no upsample2x");
   const bool wpi = a->weights_per_image != 0, f16 = a->operand_f16 != 0;
   if (wpi) BBDM_REQUIRE(a->taps == 1 && a->Cin2 == 0 && !a->upsample2x, "conv_umma: weights_per_image needs taps == 1 and no fused operand");
+  if (wpi) BBDM_REQUIRE(a->Cin % 64 == 0 && a->Cout % 64 == 0, "conv_umma: weights_per_image needs Cin, Cout %% 64 == 0");
 
   ConvParams p;
   p.B = a->B; p.H = a->H; p.W = a->W; p.Cout = a->Cout;
@@ -520,17 +527,20 @@ extern "C" int bbdm_conv_umma(const BbdmConvArgs* a, void* stream) {
   p.tiles_h = (a->H + p.TH - 1) / p.TH;
   p.tiles_b = (a->B + p.TB - 1) / p.TB;
   p.n_tiles = p.tiles_w * p.tiles_h * p.tiles_b;
-  // N tile: 128 couts where Cout allows (64 accumulator + 64 promotion registers per thread) -- unless that leaves
-  // most SMs without a tile (small spatial extents / batches): then 64-wide tiles (more CTAs) finish sooner.
-  int BN = (a->Cout % 128 == 0) ? 128 : 64;
+  // N tile: 128 couts where 128-wide blocks cover Cout with no more padding columns than 64-wide ones (64 accumulator +
+  // 64 promotion registers per thread; each A box is then loaded once per 128 couts): Cout % 128 in {0, 96}.  At
+  // Cout % 128 in {32, 64} the last 128-wide block would compute 96 or 64 zero columns, so 64-wide ones pad at most
+  // 32.  Either way 64-wide tiles when 128-wide ones leave most SMs without a tile (small spatial extents / batches):
+  // more CTAs finish sooner.
+  int BN = (a->Cout + 127) / 128 * 128 == (a->Cout + 63) / 64 * 64 ? 128 : 64;
   {
     const int64_t m_tiles = (int64_t)p.n_tiles * (a->upsample2x ? 4 : 1);
     const int64_t want = (int64_t)(0.7 * num_sms());
-    if (BN > 64 && m_tiles * (a->Cout / BN) < want) BN = 64;
+    if (BN > 64 && m_tiles * ((a->Cout + BN - 1) / BN) < want) BN = 64;
   }
-  p.kb_per_tap = a->Cin / UM_BK;
+  p.kb_per_tap = (a->Cin + UM_BK - 1) / UM_BK;
   p.K1 = a->taps * p.kb_per_tap;
-  p.K2 = a->Cin2 / UM_BK;
+  p.K2 = (a->Cin2 + UM_BK - 1) / UM_BK;
   p.taps = a->taps;
   p.up2 = a->upsample2x ? 1 : 0;
   p.origin = a->window_origin;
@@ -570,7 +580,7 @@ extern "C" int bbdm_conv_umma(const BbdmConvArgs* a, void* stream) {
   } else {
     maps[4] = maps[0]; maps[5] = maps[1]; maps[6] = maps[2]; maps[7] = maps[3];
   }
-  const int64_t total = (int64_t)p.n_tiles * (a->Cout / BN) * (p.up2 ? 4 : 1);
+  const int64_t total = (int64_t)p.n_tiles * ((a->Cout + BN - 1) / BN) * (p.up2 ? 4 : 1);
   BBDM_REQUIRE(total < (1ll << 30), "conv_umma: too many tiles");
   const int grid = (int)(total < num_sms() ? total : num_sms());
   cudaStream_t s = (cudaStream_t)stream;

@@ -16,6 +16,9 @@
 //     atoms side by side, LBO = one atom (8 KiB).
 //   * two consumer warpgroups (couts 0-63 / 64-127 of the tile) + one TMA producer warp; split-bf16 x3
 //     products, chunked wgmma -> fp32-register promotion (as conv_umma.cu).
+//   * Cin and Cout are multiples of 32.  The last Cin tile may run past Cin: a channel past the end only reaches the
+//     accumulator column of that channel, and columns past Cin are not stored, so the result does not depend on what
+//     the im2col load puts there.  Likewise rows past Cout of the last Cout tile (the dY^T map zero-fills them).
 //   * K is split across CTAs (the pixel range); every CTA writes its partial [split][tap][Cout][Cin]
 //     tile, bbdm's reduce kernel sums the splits in a fixed order (deterministic) into OIHW.
 #include "tc_common.cuh"
@@ -38,8 +41,9 @@ struct WgradParams {
   unsigned long long* fault;
 };
 
-// N tile along Cin: 128 where Cin allows (64 accumulator + 64 promotion registers per thread)
-static inline int wgrad_bn(int Cin) { return Cin % 128 == 0 ? 128 : 64; }
+// N tile along Cin: 128 where 128-wide tiles cover Cin with no more padding channels than 64-wide ones (64 accumulator
+// + 64 promotion registers per thread), i.e. Cin % 128 in {0, 96}
+static inline int wgrad_bn(int Cin) { return (Cin + 127) / 128 * 128 == (Cin + 63) / 64 * 64 ? 128 : 64; }
 
 template <int BN>
 __global__ void __launch_bounds__(WG_THREADS, 1)
@@ -171,7 +175,8 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_g_hi, const __grid_con
         float* op = p.partial + (((int64_t)split * p.taps + tap) * p.Cout + co) * p.Cin + ci_t * BN + 2 * (lane & 3);
 #pragma unroll
         for (int jj = 0; jj < BN / 8; ++jj)
-          *reinterpret_cast<float2*>(op + 8 * jj) = make_float2(racc[4 * jj + 2 * ri], racc[4 * jj + 2 * ri + 1]);
+          if (ci_t * BN + 8 * jj < p.Cin)     // Cin % 32 == 0: a block of 8 columns lies wholly inside or past Cin
+            *reinterpret_cast<float2*>(op + 8 * jj) = make_float2(racc[4 * jj + 2 * ri], racc[4 * jj + 2 * ri + 1]);
       }
     }
   }
@@ -332,12 +337,12 @@ int bbdm_split_grad(const float* src, int64_t P, int C, void* hi, void* lo, void
 }
 
 int bbdm_conv_wgrad_workspace(int B, int H, int W, int Cin, int Cout, int taps, int* splits, int64_t* floats) {
-  BBDM_REQUIRE(B > 0 && H > 0 && W > 0 && Cin % 64 == 0 && Cout % 64 == 0 && (taps == 1 || taps == 4 || taps == 9),
-               "wgrad_workspace: bad shape");
+  BBDM_REQUIRE(B > 0 && H > 0 && W > 0 && Cin > 0 && Cin % 32 == 0 && Cout > 0 && Cout % 32 == 0 &&
+               (taps == 1 || taps == 4 || taps == 9), "wgrad_workspace: bad shape");
   const int64_t P = (int64_t)B * H * W;
   const int64_t kblocks = (P + 63) / 64;
   const int BN = wgrad_bn(Cin);
-  const int64_t tiles = (int64_t)taps * ((Cout + 127) / 128) * (Cin / BN);
+  const int64_t tiles = (int64_t)taps * ((Cout + 127) / 128) * ((Cin + BN - 1) / BN);
   int64_t sp = (3 * (int64_t)num_sms() + tiles - 1) / tiles;
   if (sp > kblocks / 8) sp = kblocks / 8;
   if (sp < 1) sp = 1;
@@ -351,7 +356,7 @@ int bbdm_conv_wgrad(const void* g_hi_t, const void* g_lo_t, int64_t ld_g, const 
                     int H, int W, int Cin, int Cout, int taps, int window_origin, float* dw, float* workspace,
                     void* stream) {
   BBDM_REQUIRE(g_hi_t && g_lo_t && a_hi && a_lo && dw && workspace, "conv_wgrad: null pointer");
-  BBDM_REQUIRE(Cin % 64 == 0 && Cout % 64 == 0 && (taps == 1 || taps == 4 || taps == 9) && W >= 4,
+  BBDM_REQUIRE(Cin > 0 && Cin % 32 == 0 && Cout > 0 && Cout % 32 == 0 && (taps == 1 || taps == 4 || taps == 9) && W >= 4,
                "conv_wgrad: unsupported shape");
   BBDM_REQUIRE(window_origin == 0 || (taps == 4 && window_origin == -1),
                "conv_wgrad: window_origin -1 needs taps == 4 (got origin %d, taps %d)", window_origin, taps);
@@ -377,7 +382,7 @@ int bbdm_conv_wgrad(const void* g_hi_t, const void* g_lo_t, int64_t ld_g, const 
   BBDM_REQUIRE(p.fault != nullptr, "conv_wgrad: device fault word unavailable");
   const int BN = wgrad_bn(Cin);
   p.n_co = (Cout + WG_BM - 1) / WG_BM;
-  p.n_ci = Cin / BN;
+  p.n_ci = (Cin + BN - 1) / BN;
   CUtensorMap maps[4];
   if ((rc = make_gt_map(&maps[0], g_hi_t, Cout, P, ld_g))) return rc;
   if ((rc = make_gt_map(&maps[1], g_lo_t, Cout, P, ld_g))) return rc;

@@ -272,7 +272,7 @@ class KernelExecutor:
         umma2 = self._umma_ok(cout, cout, W)
         # a 1x1 skip conv rides as extra K-blocks of conv2 (or, before a Winograd conv2, as its own GEMM) on the raw
         # input's split planes; any other skip that is not plain src1 needs the raw (resampled / concatenated) input
-        fuse_skip = es is not None and umma2 and es["k"] == 1 and cin % 64 == 0
+        fuse_skip = es is not None and umma1 and umma2 and es["k"] == 1
         need_raw_f32 = (es is not None and not fuse_skip) or \
                        (es is None and (src2 is not None or (resample != cabi.RESAMPLE_NONE and not umma2)))
         r_f32 = r_hi = r_lo = None
@@ -413,12 +413,17 @@ class KernelExecutor:
 class UNetEngine(KernelExecutor):
     def __init__(self, unet: UNetModel, backend=None, precision: str = "split3"):
         super().__init__(backend, precision)
+        # channel multiple of the tensor-core convs and GEMMs (32 on CudaBackend); Winograd keeps 64 (convs.wino_*)
+        self.conv_multiple = convs.channel_multiple(self.be)
         self.unet = unet
         self._wkey = None
         self._w = {}
         self._table = None
         self.num_timesteps = 1000
         self.generation = 0          # bumps whenever cache/parameter ADDRESSES change (graphs key on it)
+
+    def _umma_ok(self, cin, cout, w):
+        return convs.tensor_core_ok(cin, cout, w, self.conv_multiple)
 
     # ------------------------------------------------------------------------------ weights
     def _params_key(self):
@@ -444,8 +449,9 @@ class UNetEngine(KernelExecutor):
         old = self._w or {}
         if self._ptrs(key) != self._ptrs(self._wkey) or not self._w:
             self.generation += 1
-        packer = convs.WeightPacker(be, dev, old)
+        packer = convs.WeightPacker(be, dev, old, multiple=self.conv_multiple)
         w = packer.w
+        mult = self.conv_multiple
 
         film_w, film_b, off = [], [], 0
         for name, m in u.named_modules():
@@ -493,17 +499,18 @@ class UNetEngine(KernelExecutor):
                     if not direct and self._wino_ready(w[cname], tile):
                         packer.winograd(cname, conv.weight, tile)
         for name, m in u.named_modules():
-            if isinstance(m, ResBlock) and m.up and m.channels % 64 == 0 and m.out_channels % 64 == 0:
+            if isinstance(m, ResBlock) and m.up and m.channels % mult == 0 and m.out_channels % mult == 0:
                 # up-ResBlock in_layers conv: 16 phase taps of the fused nearest-2x + 3x3 conv; on a low-res map that
                 # takes F(6,3) also its phase-stacked F(6,3) planes (4*Cout outputs: 2.1x fewer tensor-core MACs
-                # than the 16 phase taps at 64x64 and 128x128, edge tiles included)
+                # than the 16 phase taps at 64x64 and 128x128, edge tiles included; Winograd needs multiples of 64)
                 packer.up_phase(name + ".in_layers.2", m.in_layers[2].weight)
                 low = sizes[name] // 2
-                if self.wino and 6 in getattr(be, "wino_tiles", (4,)) and convs.wino_tile(low, low) == 6:
+                if self.wino and 6 in getattr(be, "wino_tiles", (4,)) and convs.wino_tile(low, low) == 6 \
+                        and m.channels % 64 == 0 and m.out_channels % 64 == 0:
                     packer.up_phase_winograd(name + ".in_layers.2", m.in_layers[2].weight)
         if getattr(be, "window_origin", False):
             for name, m in u.named_modules():
-                if isinstance(m, Downsample) and m.use_conv and m.channels % 64 == 0 and m.out_channels % 64 == 0:
+                if isinstance(m, Downsample) and m.use_conv and m.channels % mult == 0 and m.out_channels % mult == 0:
                     # Downsample conv: 2x2 taps on the space-to-depth operand instead of the fp32 stride-2 kernel
                     packer.stride2(name + ".op", m.op.weight)
         if old and old.get("film_n") == off and old["film_w"].device == dev:
@@ -619,8 +626,9 @@ class UNetEngine(KernelExecutor):
         if not cabi.attn_head_dim_ok(d):
             raise NotImplementedError(f"SpatialTransformer head_dim {d}: the sm_90a attention kernels take "
                                       f"{cabi.ATTN_HEAD_DIM_RULE}")
-        if not (self._umma_ok(Cc, inner, W) and inner % 64 == 0):
-            raise NotImplementedError("SpatialTransformer: channel counts must be multiples of 64 (tensor-core GEMMs)")
+        if not self._umma_ok(Cc, inner, W):
+            raise NotImplementedError(f"SpatialTransformer: channel counts must be multiples of {self.conv_multiple} "
+                                      "(tensor-core GEMMs)")
         bf = torch.bfloat16
         tok = (B, H, W, inner)
         _, a_hi, a_lo = self._gn_act(pool, x, m.norm, True, silu=False, eps=m.norm.eps)

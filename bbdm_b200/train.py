@@ -143,10 +143,11 @@ def _on_device(x: torch.Tensor) -> bool:
 
 def _tc_ok(x: torch.Tensor, cin: int, cout: int) -> bool:
     """Operands the tensor-core fwd/dgrad/wgrad kernels take: fp32 [B, C, H, W] on the device and the shapes of
-    convs.tensor_core_ok (any map size and batch)."""
+    convs.tensor_core_ok at the backend's channel multiple (any map size and batch).  The backend is consulted only for
+    an operand on the device: a CPU call never loads the library."""
     if not _on_device(x) or x.dtype != torch.float32 or x.dim() != 4:
         return False
-    return convs.tensor_core_ok(cin, cout, x.shape[3])
+    return convs.tensor_core_ok(cin, cout, x.shape[3], convs.channel_multiple(backend()))
 
 
 def native_ok(conv: torch.nn.Conv2d, x: torch.Tensor) -> bool:
@@ -416,22 +417,24 @@ def _resample_ok(x, cin, cout):
 
 def downsample_conv(conv: torch.nn.Conv2d, x: torch.Tensor, enabled: bool = True):
     """The Downsample's 3x3 stride-2 padding-1 conv on Stride2Conv2dFn, or None where the kernels do not take the
-    shape (Cin, Cout multiples of 64, H and W even, and a half-resolution grid at least 4 wide)."""
+    shape (Cin, Cout multiples of the backend's channel multiple, H and W even, and a half-resolution grid at least 4
+    wide)."""
     if not (enabled and _resample_ok(x, conv.in_channels, conv.out_channels)):
         return None
     B, Cin, H, W = x.shape
-    if Cin % 64 or H % 2 or W % 2 or not convs.tensor_core_ok(4 * Cin, conv.out_channels, W // 2):
+    mult = convs.channel_multiple(backend())
+    if Cin % mult or H % 2 or W % 2 or not convs.tensor_core_ok(4 * Cin, conv.out_channels, W // 2, mult):
         return None
     return Stride2Conv2dFn.apply(x, conv.weight, conv.bias)
 
 
 def upsample_conv(conv: torch.nn.Conv2d, x: torch.Tensor, enabled: bool = True):
     """conv(nearest-2x(x)) of the Upsample on Up2Conv2dFn, or None where the kernels do not take the shape (Cin, Cout
-    multiples of 64 and a low-res grid at least 4 wide)."""
+    multiples of the backend's channel multiple and a low-res grid at least 4 wide)."""
     if not (enabled and _resample_ok(x, conv.in_channels, conv.out_channels)):
         return None
     B, Cin, H, W = x.shape
-    if not convs.tensor_core_ok(Cin, conv.out_channels, W):
+    if not convs.tensor_core_ok(Cin, conv.out_channels, W, convs.channel_multiple(backend())):
         return None
     return Up2Conv2dFn.apply(x, conv.weight, conv.bias)
 

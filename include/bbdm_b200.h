@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define BBDM_ABI_VERSION 8
+#define BBDM_ABI_VERSION 9
 
 enum {
   BBDM_OK = 0,
@@ -188,9 +188,10 @@ enum { BBDM_RES_NONE = 0, BBDM_RES_SAME = 1, BBDM_RES_UP2 = 2, BBDM_RES_DOWN2 = 
  * TMA (4-D tiled maps, OOB zero fill = the conv padding), accumulate in wgmma register fragments (fp32).
  * passes = 3: A_hi.W_hi + A_lo.W_hi + A_hi.W_lo  (fp32-class accuracy, the parity mode)
  * passes = 1: A_hi.W_hi                           (plain bf16)
- * Requirements: Cin % 64 == 0, Cin2 % 64 == 0, Cout % 64 == 0, taps in {1, 9}, or 4 (2x2 window at rows/cols
+ * Requirements: Cin % 32 == 0, Cin2 % 32 == 0, Cout % 32 == 0 (K blocks of 64 channels past Cin / Cin2 read TMA
+ * zero fill; N tiles past Cout are not stored), taps in {1, 9}, or 4 (2x2 window at rows/cols
  * window_origin..window_origin+1 -- the stride-2 conv on a space-to-depth operand, bbdm_s2d_split; with upsample2x the
- * 4 taps are per output phase), W >= 4.
+ * 4 taps are per output phase), W >= 4.  weights_per_image needs Cin % 64 == 0 and Cout % 64 == 0.
  * Replaces nn.Conv2d 3x3 / 1x1 in ResBlock (openaimodel.py:207,233,244), the qkv / proj_out
  * nn.Conv1d of AttentionBlock (:307,315) and the residual adds (:278,327). */
 typedef struct {
@@ -377,7 +378,7 @@ int bbdm_conv_direct_pad(const float* src, const float* w_packed, const float* b
 int bbdm_split_grad(const float* src, int64_t P, int C, void* hi, void* lo, void* hi_t, void* lo_t, int64_t ld_t,
                     float* colsum, float* workspace, void* stream);
 
-/* split-K factor and workspace size (floats) bbdm_conv_wgrad needs for this problem. */
+/* split-K factor and workspace size (floats) bbdm_conv_wgrad needs for this problem (Cin, Cout % 32 == 0). */
 int bbdm_conv_wgrad_workspace(int B, int H, int W, int Cin, int Cout, int taps, int* splits,
                               int64_t* floats);
 
@@ -385,7 +386,7 @@ int bbdm_conv_wgrad_workspace(int B, int H, int W, int Cin, int Cout, int taps, 
  * g_hi_t/g_lo_t = dY^T planes [Cout][P] from bbdm_split_grad, rows ld_g elements apart (ld_g >= P, a multiple of 8),
  * a_hi/a_lo = the forward conv's operand planes [B,H,W,Cin].  M = Cout, N = Cin, K = pixels in blocks of 64 consecutive
  * pixels of the flattened (b, h, w) index (any map size and batch; the last block is zero-filled past P); split-bf16
- * x3; split-K partials reduced in a fixed order.  Requirements: Cin, Cout % 64 == 0, W >= 4, taps in {1, 9}
+ * x3; split-K partials reduced in a fixed order.  Requirements: Cin, Cout % 32 == 0, W >= 4, taps in {1, 9}
  * (window_origin 0), or 4 (2x2 window at rows/cols window_origin..window_origin+1, window_origin 0 or -1, as in
  * BbdmConvArgs; dw is then [Cout][Cin][2][2]). */
 int bbdm_conv_wgrad(const void* g_hi_t, const void* g_lo_t, int64_t ld_g, const void* a_hi, const void* a_lo,
