@@ -33,6 +33,13 @@ def attn_head_dim_ok(d):
     return d % 8 == 0 and 8 <= d <= 128
 
 
+def attn_head_dims(be):
+    """The attention head sizes backend ``be`` runs natively, as (ok, rule): ok(d) is True for the multiples of 8 up to
+    its attn_max_head_dim (128 when it declares none; 256 for CudaBackend) and rule names them for error messages."""
+    top = getattr(be, "attn_max_head_dim", 128)
+    return (lambda d: d % 8 == 0 and 8 <= d <= top), f"multiples of 8 up to {top}"
+
+
 @contextlib.contextmanager
 def collector_paused():
     """Collect the dead reference cycles now and keep Python's cycle collector off until the block ends; wraps every
@@ -287,6 +294,9 @@ class CudaBackend:
     window_origin = True
     # conv_umma / conv_wgrad take channel counts that are multiples of 32 (a backend without this attribute: 64)
     conv_channel_multiple = 32
+    # attention / _split / _cross / _bwd / _cross_bwd take head sizes that are multiples of 8 up to this (a backend
+    # without this attribute: 128); attention_tc takes 64 and 128 only
+    attn_max_head_dim = 256
 
     def __init__(self):
         self.lib = load()

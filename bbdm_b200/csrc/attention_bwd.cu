@@ -17,79 +17,9 @@
 // A head_dim D that is not a multiple of 16 is staged at DP = D rounded up to 16 columns, zero past D, so that the
 // 16 column threads of dQ / dK / dV hold DP / 16 columns each; only the columns < D are stored.  With D == DP the
 // padding tests are compile-time constants.
-#include "common.cuh"
+#include "attention_bwd.cuh"
 
 namespace bbdm {
-
-constexpr int AB_T = 64;           // tile edge (queries and keys)
-constexpr int AB_LD = AB_T + 4;    // row stride of the P / dS tiles (float4-aligned, conflict-free)
-template <int D>
-constexpr int ab_dp() { return (D + 15) / 16 * 16; }   // head_dim padded to the 16 column threads
-
-// Queries come from q [B, Tq, ldq], keys and values from kv [B, Tkv, ldkv] (the same tensor for self-attention);
-// head h reads columns q_base + h*q_hstride (q), k_base / v_base + h*kv_hstride (k, v) and its gradients go to the
-// same columns of dq / dkv, whose row strides equal ldq / ldkv.
-struct AttnBwdParams {
-  const float* q; const float* kv; const float* o; const float* dout; float* dq; float* dkv;
-  float* lse; float* delta;        // [B*heads, Tq]
-  int Tq, Tkv, C, heads;
-  int64_t ldq, ldkv;
-  int q_base, k_base, v_base, q_hstride, kv_hstride;
-  float scale2, scale_log2;
-};
-
-__device__ __forceinline__ void head_offsets(const AttnBwdParams& p, int head, int& qoff, int& koff, int& voff) {
-  qoff = p.q_base + head * p.q_hstride;
-  koff = p.k_base + head * p.kv_hstride;
-  voff = p.v_base + head * p.kv_hstride;
-}
-
-// 64 rows x D columns of a [*, ld] fp32 matrix -> transposed tile dst_t[DP][64] (and row-major dst_r[64][DP]),
-// zero past row T and past column D
-template <int D>
-__device__ __forceinline__ void load_tile(const float* __restrict__ src, int64_t ld, int t0, int T, float* dst_t, float* dst_r) {
-  constexpr int DP = ab_dp<D>();
-  for (int i = threadIdx.x; i < AB_T * (DP / 4); i += 256) {
-    const int row = i % AB_T, ch = i / AB_T;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (t0 + row < T && (D == DP || ch * 4 < D)) v = ld_f4(src + (int64_t)(t0 + row) * ld + ch * 4);
-    dst_t[(ch * 4 + 0) * AB_T + row] = v.x;
-    dst_t[(ch * 4 + 1) * AB_T + row] = v.y;
-    dst_t[(ch * 4 + 2) * AB_T + row] = v.z;
-    dst_t[(ch * 4 + 3) * AB_T + row] = v.w;
-    if (dst_r) *reinterpret_cast<float4*>(dst_r + row * DP + ch * 4) = v;
-  }
-}
-
-// acc[i][j] = sum_d At[d][ty*4+i] * Bt[d][tx*4+j]
-template <int D>
-__device__ __forceinline__ void mm_tt(const float* At, const float* Bt, int ty, int tx, float (&acc)[4][4]) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-#pragma unroll 8
-  for (int d = 0; d < D; ++d) {
-    const float4 a = *reinterpret_cast<const float4*>(At + d * AB_T + ty * 4);
-    const float4 b = *reinterpret_cast<const float4*>(Bt + d * AB_T + tx * 4);
-    const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
-  }
-}
-
-__device__ __forceinline__ float group16_max(float v) {
-#pragma unroll
-  for (int o = 1; o < 16; o <<= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-__device__ __forceinline__ float group16_sum(float v) {
-#pragma unroll
-  for (int o = 1; o < 16; o <<= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 
 // ---------------------------------------------------------------------------------------------
 // kernel 1: per 64-query tile -- delta, log-sum-exp, dQ
@@ -348,13 +278,13 @@ static int attention_bwd_launch(const char* what, AttnBwdParams p, int B, void* 
   p.scale2 = (float)(scale * scale);
   p.scale_log2 = (float)(scale * scale * 1.4426950408889634);
   cudaStream_t s = (cudaStream_t)stream;
-  // at D = 128 kernel 2 takes 231,936 B of the 232,448 B opt-in shared memory; DP <= 128 takes no more
+  // at D = 128 kernel 2 takes 231,936 B of the 232,448 B opt-in shared memory; DP <= 128 takes no more.  Wider heads
+  // run on the kernels of attention_bwd_wide.cu.
 #define BBDM_AB(DD) \
   case DD: return launch_bwd<DD>(p, B, s);
   switch (D) {
     BBDM_FOR_ATTN_HEAD_DIMS(BBDM_AB)
-    default:
-      BBDM_REQUIRE(false, "%s: head_dim %d not supported (a multiple of 8 up to 128)", what, D);
+    default: return launch_attention_bwd_wide(what, p, D, B, s);
   }
 #undef BBDM_AB
   return BBDM_OK;

@@ -1,5 +1,6 @@
 // Entry points of the mma.sync attention core (attention_split.cuh): head sizes 16, 32, 64 and 128 are instantiated
-// here, the other multiples of 8 up to 128 in attention_split_padded.cu.
+// here, the other multiples of 8 up to 128 in attention_split_padded.cu and the multiples of 8 from 136 to 256 in
+// attention_split_wide.cu.
 #include "attention_split.cuh"
 
 using namespace bbdm;

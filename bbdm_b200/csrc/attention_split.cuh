@@ -439,4 +439,10 @@ template <bool F32IN>
 int launch_attention_padded(const char* who, int D, const AttnOperands& ops, dim3 grid, int T, int C, int heads,
                             float scale, float* out_f32, __nv_bfloat16* out_hi, __nv_bfloat16* out_lo, cudaStream_t s);
 
+// Head sizes 136 to 256 (attention_split_wide.cu): 64-query CTAs over 32-key tiles, so that the stages and the output
+// fragment fit.  Any other head_dim fails here with BBDM_E_UNSUPPORTED.
+template <bool F32IN>
+int launch_attention_wide(const char* who, int D, const AttnOperands& ops, dim3 grid, int T, int C, int heads,
+                          float scale, float* out_f32, __nv_bfloat16* out_hi, __nv_bfloat16* out_lo, cudaStream_t s);
+
 }  // namespace bbdm

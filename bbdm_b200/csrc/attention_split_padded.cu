@@ -11,9 +11,7 @@ int launch_attention_padded(const char* who, int D, const AttnOperands& ops, dim
   case DD: return launch_attention_d<DD, F32IN>(ops, grid, T, C, heads, scale, out_f32, out_hi, out_lo, s);
   switch (D) {
     BBDM_ATTN_PADDED_HEAD_DIMS(BBDM_AL)
-    default:
-      set_error("%s: head_dim %d not supported (a multiple of 8 up to 128)", who, D);
-      return BBDM_E_UNSUPPORTED;
+    default: return launch_attention_wide<F32IN>(who, D, ops, grid, T, C, heads, scale, out_f32, out_hi, out_lo, s);
   }
 #undef BBDM_AL
 }

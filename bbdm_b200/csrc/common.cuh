@@ -33,11 +33,14 @@ unsigned long long* device_fault_ptr();
 
 // Head dims of the mma.sync attention forward (attention_split.cuh) and the flash backward (attention_bwd.cu): every
 // multiple of 8 up to 128.  A multiple of 8 keeps each head's columns 16-byte aligned in the bf16 planes, as the
-// 16-byte cp.async chunks need; past 128 the backward's tiles do not fit in shared memory.  The forward instantiates
+// 16-byte cp.async chunks need; past 128 these kernels' tiles do not fit in shared memory.  The forward instantiates
 // the multiples of 16 in attention_split.cu and the padded sizes in attention_split_padded.cu.
 #define BBDM_ATTN_POW2_HEAD_DIMS(X) X(16) X(32) X(64) X(128)
 #define BBDM_ATTN_PADDED_HEAD_DIMS(X) X(8) X(24) X(40) X(48) X(56) X(72) X(80) X(88) X(96) X(104) X(112) X(120)
 #define BBDM_FOR_ATTN_HEAD_DIMS(X) BBDM_ATTN_POW2_HEAD_DIMS(X) BBDM_ATTN_PADDED_HEAD_DIMS(X)
+// Head dims 136 to 256 (multiples of 8) run on kernels of their own (attention_split_wide.cu, attention_bwd_wide.cu),
+// instantiated per padded width: D runs at the next multiple of 32, zero past D.
+#define BBDM_ATTN_WIDE_PADDED_DIMS(X) X(160) X(192) X(224) X(256)
 
 // Everything cached on the host is cached PER DEVICE (the reference's single-GPU launcher puts the
 // model on cuda:N without cudaSetDevice-ing the process default; cabi.py guards the device per call).

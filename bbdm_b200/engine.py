@@ -574,8 +574,9 @@ class UNetEngine(KernelExecutor):
         eq, ep = w[name + ".qkv"], w[name + ".proj_out"]
         heads = m.num_heads
         hd = Cc // heads
-        if not cabi.attn_head_dim_ok(hd):
-            raise NotImplementedError(f"attention head_dim {hd}: the sm_90a kernels take {cabi.ATTN_HEAD_DIM_RULE}")
+        head_dim_ok, rule = cabi.attn_head_dims(be)
+        if not head_dim_ok(hd):
+            raise NotImplementedError(f"attention head_dim {hd}: the sm_90a kernels take {rule}")
         umma = self._umma_ok(Cc, Cc, W)
         a_f32, a_hi, a_lo = self._gn_act(pool, x, m.norm, umma, silu=False)
         # qkv 1x1: on the tensor-core path its epilogue writes the split planes the attention core reads
@@ -586,7 +587,8 @@ class UNetEngine(KernelExecutor):
         order = 1 if m.new_order else 0
         if umma:
             o_hi, o_lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
-            # head_dim 64 (all templates) or 128: warp-specialised wgmma kernel; any other size: the mma.sync one
+            # head_dim 64 (all templates) or 128: warp-specialised wgmma kernel; any other size (up to 256): the
+            # mma.sync one
             attn = be.attention_tc if hd in cabi.ATTN_TC_HEAD_DIMS else be.attention_split
             attn(q_hi.view(B, T, 3 * Cc), q_lo.view(B, T, 3 * Cc), heads, order,
                  None, o_hi.view(B, T, Cc), o_lo.view(B, T, Cc))
@@ -623,9 +625,9 @@ class UNetEngine(KernelExecutor):
         B, H, W, Cc = x.shape
         T, heads, d = H * W, m.n_heads, m.d_head
         inner = heads * d
-        if not cabi.attn_head_dim_ok(d):
-            raise NotImplementedError(f"SpatialTransformer head_dim {d}: the sm_90a attention kernels take "
-                                      f"{cabi.ATTN_HEAD_DIM_RULE}")
+        head_dim_ok, rule = cabi.attn_head_dims(be)
+        if not head_dim_ok(d):
+            raise NotImplementedError(f"SpatialTransformer head_dim {d}: the sm_90a attention kernels take {rule}")
         if not self._umma_ok(Cc, inner, W):
             raise NotImplementedError(f"SpatialTransformer: channel counts must be multiples of {self.conv_multiple} "
                                       "(tensor-core GEMMs)")

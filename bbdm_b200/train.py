@@ -637,7 +637,8 @@ def conv1x1(conv1d: torch.nn.Conv1d, x4: torch.Tensor, enabled: bool = True):
 class AttentionCoreFn(torch.autograd.Function):
     """softmax((q s)(k s)^T) v per head (QKVAttentionLegacy / QKVAttention, openaimodel.py:350-413) on a
     [B,3C,H,W] qkv tensor -> [B,C,H,W].  Forward: the sampling path's attention kernels (wgmma for
-    head_dim 64 and 128, the fp32-qkv mma.sync kernel for the other multiples of 8 up to 128); backward:
+    head_dim 64 and 128, the fp32-qkv mma.sync kernel for the other multiples of 8 up to the backend's
+    attn_max_head_dim, 256 on CudaBackend); backward:
     bbdm_attention_bwd (flash-style recompute, exact fp32) -- the T x T matrix is never stored, which also replaces
     the reference's checkpoint() around the block (openaimodel.py:318)."""
 
@@ -680,8 +681,8 @@ def attention_core(qkv4: torch.Tensor, heads: int, new_order: bool, enabled: boo
     """[B,3C,H,W] -> [B,C,H,W] or None when the native kernels do not take the shape."""
     B, C3, H, W = qkv4.shape
     hd = C3 // 3 // heads
-    if not (enabled and _on_device(qkv4) and qkv4.dtype == torch.float32 and cabi.attn_head_dim_ok(hd) and (C3 // 3) % 4 == 0
-            and B * heads <= 65535):
+    if not (enabled and _on_device(qkv4) and qkv4.dtype == torch.float32 and cabi.attn_head_dims(backend())[0](hd)
+            and (C3 // 3) % 4 == 0 and B * heads <= 65535):
         return None
     return AttentionCoreFn.apply(qkv4, heads, 1 if new_order else 0)
 

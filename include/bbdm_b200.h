@@ -433,7 +433,7 @@ int bbdm_geglu_split(const float* u, int64_t rows, int N, float* out_f32, void* 
 
 /* Cross-attention core (CrossAttention.forward, attention.py:166-192): queries q [B,Tq,C] and keys|values
  * kv [B,Tkv,2C] (k = columns [0,C), v = [C,2C)), both as split-bf16 planes, head h = columns h*D..(h+1)*D of each;
- * out[b,i,:] = softmax_j(q_i.k_j * D^-1/2) v_j per head, flash-style (no Tq x Tkv buffer).  D: a multiple of 8 up to 128. */
+ * out[b,i,:] = softmax_j(q_i.k_j * D^-1/2) v_j per head, flash-style (no Tq x Tkv buffer).  D: a multiple of 8 up to 256. */
 int bbdm_attention_cross(const void* q_hi, const void* q_lo, const void* kv_hi, const void* kv_lo, int B, int Tq,
                          int Tkv, int C, int heads, float* out_f32, void* out_hi, void* out_lo, void* stream);
 
@@ -443,7 +443,7 @@ int bbdm_attention_cross(const void* q_hi, const void* q_lo, const void* kv_hi, 
  * bbdm_geglu_bwd: u [rows][2N] (the forward's input), dy [rows][N] -> du [rows][2N] = [dy*gelu(g) | dy*a*gelu'(g)].
  * bbdm_attention_cross_bwd: fp32 q [B,Tq,C], kv [B,Tkv,2C] and out [B,Tq,C] of bbdm_attention_cross, dout [B,Tq,C] ->
  *   dq [B,Tq,C], dkv [B,Tkv,2C]; the probabilities are recomputed tile by tile (no Tq x Tkv buffer), exact fp32.
- *   lse / delta: [B*heads*Tq] fp32 workspaces.  D: a multiple of 8 up to 128; the same kernels as bbdm_attention_bwd. */
+ *   lse / delta: [B*heads*Tq] fp32 workspaces.  D: a multiple of 8 up to 256; the same kernels as bbdm_attention_bwd. */
 int bbdm_layernorm_bwd(const float* x, const float* dy, int64_t rows, int C, const float* gamma, float eps, float* dx,
                        float* dgamma, float* dbeta, float* workspace, void* stream);
 int bbdm_geglu_bwd(const float* u, const float* dy, int64_t rows, int N, float* du, void* stream);
@@ -517,14 +517,15 @@ int bbdm_ema_multi(const void* const* params, const int64_t* numel, const int64_
  * out: fp32 [B,T,C] and/or split bf16 (A operand of the proj_out GEMM).
  * Split-bf16 tensor-core products with fp32 accumulation: q and k are scaled by s, then split; expf softmax.
  * Runs on the mma.sync kernel of bbdm_attention_split, which copies the fp32 K/V tiles with cp.async and splits
- * them in shared memory.  head_dim: a multiple of 8 up to 128. */
+ * them in shared memory.  head_dim: a multiple of 8 up to 256. */
 int bbdm_attention(const float* qkv, int B, int T, int C, int heads, int order,
                    float* out_f32, void* out_hi, void* out_lo, void* stream);
 
 /* Same attention core on PRE-SPLIT bf16 planes qkv_hi/qkv_lo [B,T,3C] (written by the qkv
  * conv's epilogue, BbdmConvArgs.out_hi/out_lo): no conversion or re-splitting of K/V per query
- * tile; cp.async double-buffered KV tiles, ldmatrix fragments, 128 queries per CTA; S is scaled by D^-1/2 after the
- * products and the softmax runs on ex2.approx.  head_dim: a multiple of 8 up to 128. */
+ * tile; cp.async double-buffered KV tiles, ldmatrix fragments, 128 queries per CTA over 64-key tiles (head_dim
+ * above 128: 64 queries over 32-key tiles); S is scaled by D^-1/2 after the products and the softmax runs on
+ * ex2.approx.  head_dim: a multiple of 8 up to 256. */
 int bbdm_attention_split(const void* qkv_hi, const void* qkv_lo, int B, int T, int C, int heads,
                          int order, float* out_f32, void* out_hi, void* out_lo, void* stream);
 
@@ -540,7 +541,8 @@ int bbdm_attention_tc(const void* qkv_hi, const void* qkv_lo, int B, int T, int 
  * QKVAttentionLegacy / QKVAttention, openaimodel.py:318,350-413, util.py:119-148): given qkv [B,T,3C],
  * out = attention(qkv) [B,T,C] and dout [B,T,C] (all fp32), writes dqkv [B,T,3C].  FlashAttention-style
  * recompute in exact fp32 -- no T x T tensor.  lse, delta: fp32 workspaces of B*heads*T elements each.
- * head_dim: a multiple of 8 up to 128; deterministic. */
+ * head_dim: a multiple of 8 up to 256 (above 128 the streamed operands share one shared-memory tile);
+ * deterministic. */
 int bbdm_attention_bwd(const float* qkv, const float* out, const float* dout, int B, int T, int C, int heads,
                        int order, float* dqkv, float* lse, float* delta, void* stream);
 

@@ -71,8 +71,9 @@ def main():
         a.B, a.T, a.C = a.shape[:3]
         a.head_dims = [a.shape[2] // a.shape[3]]
     for d in a.head_dims:
-        if not cabi.attn_head_dim_ok(d):
-            ap.error(f"head_dim {d}: the kernels take {cabi.ATTN_HEAD_DIM_RULE}")
+        head_dim_ok, rule = cabi.attn_head_dims(cabi.CudaBackend)
+        if not head_dim_ok(d):
+            ap.error(f"head_dim {d}: the kernels take {rule}")
         if "attention_tc" in a.kernels and d not in cabi.ATTN_TC_HEAD_DIMS:
             ap.error(f"attention_tc takes head_dim {cabi.ATTN_TC_HEAD_DIMS}, not {d}")
     assert torch.cuda.is_available(), "time_attention.py needs a GPU"
