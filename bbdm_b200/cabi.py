@@ -17,7 +17,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BBDM_LIB selects another in-tree build of the same sources (A/B experiments, tools/); the product default is fixed
 LIB_PATH = os.environ.get("BBDM_LIB") or os.path.join(_HERE, "libbbdm_b200.so")
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 OBJ = {"grad": 0, "noise": 1, "ysubx": 2}
 RESAMPLE_NONE, RESAMPLE_UP2, RESAMPLE_DOWN2 = 0, 1, 2
 RES_NONE, RES_SAME, RES_UP2, RES_DOWN2 = 0, 1, 2, 3
@@ -38,6 +38,18 @@ def attn_head_dims(be):
     its attn_max_head_dim (128 when it declares none; 256 for CudaBackend) and rule names them for error messages."""
     top = getattr(be, "attn_max_head_dim", 128)
     return (lambda d: d % 8 == 0 and 8 <= d <= top), f"multiples of 8 up to {top}"
+
+
+def attn_gemm_route(be, d):
+    """True when backend ``be`` runs attention heads of width d as GEMMs around a materialised row softmax (one image
+    and head at a time): d is above its attn_max_head_dim and it declares attn_gemm_route."""
+    return bool(getattr(be, "attn_gemm_route", False)) and d > getattr(be, "attn_max_head_dim", 128)
+
+
+def gemm_heads_pad(d):
+    """Width of a head's zero-padded q/k/v/o slices on the GEMM route: d rounded up to 32 (the channel multiple of the
+    tensor-core GEMMs)."""
+    return -(-d // 32) * 32
 
 
 @contextlib.contextmanager
@@ -68,7 +80,7 @@ SYMBOLS = [
     "bbdm_pack_weight_f32", "bbdm_conv_umma", "bbdm_conv_direct",
     "bbdm_attention", "bbdm_attention_split", "bbdm_attention_tc", "bbdm_conv_umma_geometry", "bbdm_gn_finalize_partials",
     "bbdm_split_grad", "bbdm_conv_wgrad_workspace", "bbdm_conv_wgrad", "bbdm_gn_bwd_reduce", "bbdm_gn_bwd_apply",
-    "bbdm_conv_wgrad_direct", "bbdm_attention_bwd", "bbdm_conv_direct_pad", "bbdm_softmax_rows_split", "bbdm_vq_nearest", "bbdm_s2d_split", "bbdm_pack_weight_split_both",
+    "bbdm_conv_wgrad_direct", "bbdm_attention_bwd", "bbdm_conv_direct_pad", "bbdm_softmax_rows_split", "bbdm_softmax_rows_bwd", "bbdm_vq_nearest", "bbdm_s2d_split", "bbdm_pack_weight_split_both",
     "bbdm_wino_geometry", "bbdm_wino_input", "bbdm_wino_output", "bbdm_wino_pack_weight",
     "bbdm_wino6_geometry", "bbdm_wino6_input", "bbdm_wino6_output", "bbdm_wino6_pack_weight",
     "bbdm_optim_chunk_elems", "bbdm_adam_multi", "bbdm_adam_multi_dev", "bbdm_ema_multi", "bbdm_denorm_to_uint8",
@@ -177,6 +189,7 @@ def load():
     lib.bbdm_attention_bwd.argtypes = [vp, vp, vp, i, i, i, i, i, vp, vp, vp, vp]
     lib.bbdm_conv_direct_pad.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, i, i, i, i, i, vp]
     lib.bbdm_softmax_rows_split.argtypes = [vp, i64, i64, i64, C.c_float, vp, vp, vp]
+    lib.bbdm_softmax_rows_bwd.argtypes = [vp, vp, i64, i64, i64, C.c_float, vp, vp, vp]
     lib.bbdm_vq_nearest.argtypes = [vp, vp, i64, i, i, vp, vp, vp]
     lib.bbdm_s2d_split.argtypes = [vp, i, i, i, i, vp, vp, vp]
     lib.bbdm_pack_weight_split_both.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp]
@@ -297,6 +310,9 @@ class CudaBackend:
     # attention / _split / _cross / _bwd / _cross_bwd take head sizes that are multiples of 8 up to this (a backend
     # without this attribute: 128); attention_tc takes 64 and 128 only
     attn_max_head_dim = 256
+    # heads wider than attn_max_head_dim run as two conv_umma GEMMs per (image, head) around softmax_rows_split, and
+    # train through softmax_rows_split(grad=...), conv_umma and conv_wgrad (a backend without this attribute: not at all)
+    attn_gemm_route = True
 
     def __init__(self):
         self.lib = load()
@@ -656,12 +672,21 @@ class CudaBackend:
                                             B, H, W, Cin, cout, k, stride, pad_lo, pad_hi, stream()))
         LAUNCHES["n"] += 1
 
-    def softmax_rows_split(self, src, scale, out_hi, out_lo, valid_cols=None):
-        """valid_cols: the columns of each row the softmax covers (None: all); the planes are zero in the rest."""
+    def softmax_rows_split(self, src, scale, out_hi, out_lo, valid_cols=None, grad=None):
+        """The planes of p = softmax(scale * src) per row.  valid_cols: the columns of each row the softmax covers (None:
+        all); the planes are zero in the rest.  grad: dL/dp of the same shape -- the planes then hold the backward's
+        score gradient scale * p * (grad - sum_j p_j grad_j) instead of p (bbdm_softmax_rows_bwd)."""
         rows, cols = src.numel() // src.shape[-1], src.shape[-1]
-        check(self.lib.bbdm_softmax_rows_split(ptr(_req(src)), rows, cols, cols if valid_cols is None else int(valid_cols),
-                                               float(scale), ptr(_req(out_hi, torch.bfloat16)),
-                                               ptr(_req(out_lo, torch.bfloat16)), stream()))
+        v = cols if valid_cols is None else int(valid_cols)
+        if grad is not None:
+            assert grad.shape == src.shape, (grad.shape, src.shape)
+            check(self.lib.bbdm_softmax_rows_bwd(ptr(_req(src)), ptr(_req(grad)), rows, cols, v, float(scale),
+                                                 ptr(_req(out_hi, torch.bfloat16)), ptr(_req(out_lo, torch.bfloat16)),
+                                                 stream()))
+        else:
+            check(self.lib.bbdm_softmax_rows_split(ptr(_req(src)), rows, cols, v, float(scale),
+                                                   ptr(_req(out_hi, torch.bfloat16)), ptr(_req(out_lo, torch.bfloat16)),
+                                                   stream()))
         LAUNCHES["n"] += 1
 
     def s2d_split(self, src, out_hi, out_lo):

@@ -1,6 +1,7 @@
 // The two VQGAN-specific steps either side of the latent bridge loop :
 //   * row softmax of the single-head AttnBlock's T x Tp score matrix (Tp = T rounded up to 64, the padding columns
-//     masked), written as split-bf16 planes (the A operand of the P.V tensor-core GEMM)   model/VQGAN/model.py:140-192
+//     masked), written as split-bf16 planes (the A operand of the P.V tensor-core GEMM)   model/VQGAN/model.py:140-192,
+//     and its backward (the dS planes of the GEMM-composed attention's training route for heads wider than 256)
 //   * VectorQuantizer2 nearest-codebook lookup                          model/VQGAN/quantize.py:271-312
 // Everything else of the autoencoder (ResnetBlocks, 1x1/3x3 convs, GroupNorm, resampling) runs on the
 // same kernels as the UNet.
@@ -72,6 +73,64 @@ softmax_rows_split_kernel(const float* __restrict__ src, int64_t N, int64_t V, f
     split4(p, ph, pl);
     *reinterpret_cast<uint2*>(h + i) = ph;
     *reinterpret_cast<uint2*>(l + i) = pl;
+  }
+}
+
+// Backward of the row softmax above, one CTA per row: recomputes p = softmax(scale * s) over the first V columns with
+// the forward's loops, reductions and expressions (the same p the forward split), then writes the score gradient
+// ds = scale * p * (dp - sum_j p_j dp_j) as split-bf16 planes (the A operand of dQ = dS K and of the dK weight
+// gradient), exact zeros in columns V..N-1.  The row (N <= a few thousand floats of s and of dp) is re-read from L1/L2
+// by the later loops, not from HBM.
+template <bool MASKED>
+__global__ void __launch_bounds__(256)
+softmax_rows_bwd_kernel(const float* __restrict__ s_in, const float* __restrict__ dp_in, int64_t N, int64_t V,
+                        float scale, __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
+  __shared__ float red[8];
+  const float* row = s_in + (int64_t)blockIdx.x * N;
+  const float* drow = dp_in + (int64_t)blockIdx.x * N;
+  float mx = -INFINITY;
+  for (int64_t i = threadIdx.x * 4; i < V; i += 1024) {
+    float4 v = ld_f4(row + i);
+    if (MASKED && i + 4 > V) mask_tail(v, i, V, -INFINITY);
+    mx = fmaxf(fmaxf(mx, fmaxf(v.x, v.y)), fmaxf(v.z, v.w));
+  }
+  const float m = block_reduce(mx, red, true) * scale;
+  float sum = 0.f;
+  for (int64_t i = threadIdx.x * 4; i < V; i += 1024) {
+    const float4 v = ld_f4(row + i);
+    float4 e = make_float4(sexp(v.x, scale, m), sexp(v.y, scale, m), sexp(v.z, scale, m), sexp(v.w, scale, m));
+    if (MASKED && i + 4 > V) mask_tail(e, i, V, 0.f);
+    sum += e.x + e.y + e.z + e.w;
+  }
+  const float inv = 1.0f / block_reduce(sum, red, false);
+  // sum_j p_j dp_j over the valid columns, in the same per-thread order and fixed cross-warp order
+  float dot = 0.f;
+  for (int64_t i = threadIdx.x * 4; i < V; i += 1024) {
+    const float4 v = ld_f4(row + i);
+    float4 p = make_float4(sexp(v.x, scale, m) * inv, sexp(v.y, scale, m) * inv, sexp(v.z, scale, m) * inv,
+                           sexp(v.w, scale, m) * inv);
+    float4 g = ld_f4(drow + i);
+    if (MASKED && i + 4 > V) { mask_tail(p, i, V, 0.f); mask_tail(g, i, V, 0.f); }
+    dot += p.x * g.x + p.y * g.y + p.z * g.z + p.w * g.w;
+  }
+  dot = block_reduce(dot, red, false);
+  __nv_bfloat16* h = hi + (int64_t)blockIdx.x * N;
+  __nv_bfloat16* l = lo + (int64_t)blockIdx.x * N;
+  for (int64_t i = threadIdx.x * 4; i < N; i += 1024) {
+    float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (!MASKED || i < V) {
+      const float4 v = ld_f4(row + i);
+      const float4 g = ld_f4(drow + i);
+      const float4 p = make_float4(sexp(v.x, scale, m) * inv, sexp(v.y, scale, m) * inv, sexp(v.z, scale, m) * inv,
+                                   sexp(v.w, scale, m) * inv);
+      d = make_float4(scale * p.x * (g.x - dot), scale * p.y * (g.y - dot), scale * p.z * (g.z - dot),
+                      scale * p.w * (g.w - dot));
+      if (MASKED && i + 4 > V) mask_tail(d, i, V, 0.f);
+    }
+    uint2 dh, dl;
+    split4(d, dh, dl);
+    *reinterpret_cast<uint2*>(h + i) = dh;
+    *reinterpret_cast<uint2*>(l + i) = dl;
   }
 }
 
@@ -174,6 +233,23 @@ extern "C" int bbdm_softmax_rows_split(const float* src, int64_t rows, int64_t c
   else
     softmax_rows_split_kernel<true><<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(
         src, cols, valid_cols, scale, (__nv_bfloat16*)out_hi, (__nv_bfloat16*)out_lo);
+  BBDM_LAUNCH_CHECK();
+  return BBDM_OK;
+}
+
+extern "C" int bbdm_softmax_rows_bwd(const float* s, const float* dp, int64_t rows, int64_t cols, int64_t valid_cols,
+                                     float scale, void* ds_hi, void* ds_lo, void* stream) {
+  BBDM_REQUIRE(s && dp && ds_hi && ds_lo, "softmax_rows_bwd: null pointer");
+  BBDM_REQUIRE(rows > 0 && rows < (1ll << 31) && cols > 0 && cols % 4 == 0 && scale > 0.f,
+               "softmax_rows_bwd: bad shape (cols must be a multiple of 4, scale > 0)");
+  BBDM_REQUIRE(valid_cols > 0 && valid_cols <= cols, "softmax_rows_bwd: valid_cols %lld not in 1..cols = %lld",
+               (long long)valid_cols, (long long)cols);
+  if (valid_cols == cols)
+    softmax_rows_bwd_kernel<false><<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(
+        s, dp, cols, cols, scale, (__nv_bfloat16*)ds_hi, (__nv_bfloat16*)ds_lo);
+  else
+    softmax_rows_bwd_kernel<true><<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(
+        s, dp, cols, valid_cols, scale, (__nv_bfloat16*)ds_hi, (__nv_bfloat16*)ds_lo);
   BBDM_LAUNCH_CHECK();
   return BBDM_OK;
 }

@@ -366,6 +366,30 @@ class KernelExecutor:
         pool.put(r_f32, r_hi, r_lo, skip_out)
         return out
 
+    def _attention_gemm(self, q, k, vt, v, shape, tkv, scale, s, p, out_f32=None, out_hi=None, out_lo=None,
+                        write_k=None):
+        """softmax(scale Q K^T) V of one image and one head as two tensor-core GEMMs around the row softmax; the key axis
+        is padded to Tkvp, a multiple of 64, and the softmax covers its first tkv columns.
+          q         (hi, lo) [1, H, W, d] query planes, shape = (H, W): T = H * W queries; d a multiple of 32
+          k         (hi, lo) [1, Tkvp, d] key planes, zero in rows tkv..Tkvp-1 (the weights of S = Q K^T); write_k, if
+                    given, writes their first tkv rows first
+          vt, v     (hi, lo) [1, d, Tkvp] planes that receive V^T from the fp32 values v [tkv, d] (split_grad), zero
+                    in columns tkv..Tkvp-1
+          s, p      scratch: fp32 [1, H, W, Tkvp] scores and the (hi, lo) planes of P
+          out_*     O = P V [1, H, W, d] as fp32 and / or split planes"""
+        be = self.be
+        H, W = shape
+        T, tkvp, d = H * W, k[0].shape[1], k[0].shape[2]
+        if write_k is not None:
+            write_k()
+        be.split_grad(v, None, None, vt[0][0, :, :tkv], vt[1][0, :, :tkv])
+        be.conv_umma(B=1, H=H, W=W, Cin=d, Cout=tkvp, taps=1, a_hi=q[0], a_lo=q[1], w_hi=k[0], w_lo=k[1], out=s,
+                     passes=self.passes)
+        masked = {} if tkv == tkvp else dict(valid_cols=tkv)
+        be.softmax_rows_split(s.view(T, tkvp), scale, p[0].view(T, tkvp), p[1].view(T, tkvp), **masked)
+        be.conv_umma(B=1, H=H, W=W, Cin=tkvp, Cout=d, taps=1, a_hi=p[0], a_lo=p[1], w_hi=vt[0], w_lo=vt[1],
+                     out=out_f32, out_hi=out_hi, out_lo=out_lo, passes=self.passes)
+
     def _geom(self, H, W):
         key = (H, W)
         r = self._geom_cache.get(key)
@@ -485,6 +509,24 @@ class UNetEngine(KernelExecutor):
                     packer.conv(pre + ".attn2.to_out.0", a2.to_out[0].weight, a2.to_out[0].bias)
                     packer.conv(pre + ".ff.net.0.proj", blk.ff.net[0].proj.weight, blk.ff.net[0].proj.bias)
                     packer.conv(pre + ".ff.net.2", blk.ff.net[2].weight, blk.ff.net[2].bias)
+                    if cabi.attn_gemm_route(be, m.d_head):
+                        for a in ("attn1", "attn2"):
+                            at = getattr(blk, a)
+                            self._pack_gemm_heads(packer, f"{pre}.{a}", m.n_heads, m.d_head, at.to_q.weight,
+                                                  at.to_k.weight, at.to_v.weight, None, None, None,
+                                                  at.to_out[0].weight, at.to_out[0].bias)
+            if isinstance(m, AttentionBlock) and cabi.attn_gemm_route(be, m.channels // m.num_heads):
+                C, heads = m.channels, m.num_heads
+                d = C // heads
+                wq, bq = m.qkv.weight.detach()[:, :, 0], m.qkv.bias.detach()
+                if m.new_order:          # q, k, v of head h at channels h*d, C + h*d, 2C + h*d
+                    rows = lambda j: torch.cat([torch.arange(j * C + h * d, j * C + (h + 1) * d) for h in range(heads)])
+                else:                    # legacy: head h's q, k, v at 3hd, 3hd + d, 3hd + 2d
+                    rows = lambda j: torch.cat([torch.arange(3 * h * d + j * d, 3 * h * d + (j + 1) * d)
+                                                for h in range(heads)])
+                r = [rows(j).to(wq.device) for j in range(3)]
+                self._pack_gemm_heads(packer, name, heads, d, wq[r[0]], wq[r[1]], wq[r[2]], bq[r[0]], bq[r[1]],
+                                      bq[r[2]], m.proj_out.weight.detach()[:, :, 0], m.proj_out.bias)
         sizes = self._resblock_sizes()
         for name, m in u.named_modules():
             # Winograd planes for the stride-1 3x3 convs of the scale-shift ResBlocks: F(6x6,3x3) for the convs that
@@ -523,6 +565,32 @@ class UNetEngine(KernelExecutor):
         w["film_n"] = off
         self._w = w
         self._wkey = key
+
+    @staticmethod
+    def _pack_gemm_heads(packer, pre, heads, d, wq, wk, wv, bq, bk, bv, wo, bo):
+        """Per-head 1x1 conv entries of an attention whose heads run on the GEMM route: pre.q{h} / .k{h} / .v{h} from
+        rows h*d.. of wq / wk / wv ([heads*d, Cin]) and biases, their outputs zero-padded to d32 = d rounded up to 32
+        (zero weights and zero bias); pre.o{h} from columns h*d.. of the output projection wo ([Cout, heads*d]), zero
+        columns past d, with the bias bo on head 0 only (the later heads add to head 0's result)."""
+        d32 = cabi.gemm_heads_pad(d)
+
+        def padded(name, field, shape, src, into):
+            t = packer._buf(name, field, shape, torch.float32)     # reused across refreshes: the bias keeps its address
+            t.zero_()
+            into(t).copy_(src)
+            return t
+
+        for h in range(heads):
+            sl = slice(h * d, (h + 1) * d)
+            for j, (wt, bt) in enumerate(((wq, bq), (wk, bk), (wv, bv))):
+                name = f"{pre}.{'qkv'[j]}{h}"
+                w = padded(name, "w_src", (d32, wt.shape[1]), wt.detach()[sl], lambda t: t[:d])
+                b = None if bt is None else padded(name, "b_src", (d32,), bt.detach()[sl], lambda t: t[:d])
+                ent = packer.conv(name, w, b)
+                ent["w_src"], ent["b_src"] = w, b
+            name = f"{pre}.o{h}"
+            w = padded(name, "w_src", (wo.shape[0], d32), wo.detach()[:, sl], lambda t: t[:, :d])
+            packer.conv(name, w, None if h else bo)["w_src"] = w
 
     def _resblock_sizes(self):
         """{ResBlock name: side of the map its convs write} at the UNet's nominal image_size (the input side)."""
@@ -575,9 +643,14 @@ class UNetEngine(KernelExecutor):
         heads = m.num_heads
         hd = Cc // heads
         head_dim_ok, rule = cabi.attn_head_dims(be)
+        umma = self._umma_ok(Cc, Cc, W)
+        if cabi.attn_gemm_route(be, hd) and umma:
+            _, a_hi, a_lo = self._gn_act(pool, x, m.norm, True, silu=False)
+            out = self._attention_heads_gemm(pool, name, heads, hd, (a_hi, a_lo), None, (B, H, W), x)
+            pool.put(a_hi, a_lo)
+            return out
         if not head_dim_ok(hd):
             raise NotImplementedError(f"attention head_dim {hd}: the sm_90a kernels take {rule}")
-        umma = self._umma_ok(Cc, Cc, W)
         a_f32, a_hi, a_lo = self._gn_act(pool, x, m.norm, umma, silu=False)
         # qkv 1x1: on the tensor-core path its epilogue writes the split planes the attention core reads
         qkv, q_hi, q_lo = self._conv(pool, eq, a_f32=a_f32, a_hi=a_hi, a_lo=a_lo, shape=(B, H, W),
@@ -599,6 +672,60 @@ class UNetEngine(KernelExecutor):
         out, _, _ = self._conv(pool, ep, a_f32=o_f32, a_hi=o_hi, a_lo=o_lo, shape=(B, H, W),
                                residual=x, res_mode=cabi.RES_SAME, stats=True)
         pool.put(o_f32, o_hi, o_lo)
+        return out
+
+    def _attention_heads_gemm(self, pool, pre, heads, d, a, ctx, shape, residual, stats=True):
+        """Multi-head attention whose heads are wider than the flash kernels take, and its output projection: per head
+        the q/k/v 1x1 convs of its padded slices (pre.q{h}, .k{h}, .v{h}: d32 = d rounded up to 32 outputs), per image
+        the GEMM-composed core (_attention_gemm), then the head's slice of the output projection (pre.o{h}) added to the
+        running result.  a: (hi, lo) [B, H, W, Cin] planes the projections read; ctx: fp32 [B, Hc, Wc, Cc] context the k
+        and v projections read instead (fp32 direct conv: few channels), or None; residual: fp32 [B, H, W, Cout] the
+        first head's projection adds.  Scratch is one image-head's [T, Tkvp] scores and P planes.  Returns the fp32
+        output, with the GroupNorm partial sums of its last conv if stats."""
+        be, w = self.be, self._w
+        B, H, W = shape
+        T = H * W
+        bf = torch.bfloat16
+        d32 = cabi.gemm_heads_pad(d)
+        kv_shape = shape if ctx is None else tuple(ctx.shape[:3])
+        tkv = kv_shape[1] * kv_shape[2]
+        tkvp = -(-tkv // 64) * 64
+        k_pl = pool.zero_padded(("gemm heads K", tkv), (2, tkvp, d32), bf)
+        vt_pl = pool.zero_padded(("gemm heads V^T", tkv), (2, d32, tkvp), bf)
+        s = pool.get((1, H, W, tkvp))
+        p = pool.get((1, H, W, tkvp), bf), pool.get((1, H, W, tkvp), bf)
+        scale = float(d ** -0.5)
+        out = residual
+        for h in range(heads):
+            eq, ek, ev = w[f"{pre}.q{h}"], w[f"{pre}.k{h}"], w[f"{pre}.v{h}"]
+            _, q_hi, q_lo = self._conv(pool, eq, a_hi=a[0], a_lo=a[1], shape=shape, out_split=True, want_f32=False)
+            k = None
+            if ctx is None:
+                v, _, _ = self._conv(pool, ev, a_hi=a[0], a_lo=a[1], shape=shape)
+            else:
+                k, _, _ = self._conv(pool, ek, a_f32=ctx, shape=kv_shape)
+                v, _, _ = self._conv(pool, ev, a_f32=ctx, shape=kv_shape)
+            o_hi, o_lo = pool.get((B, H, W, d32), bf), pool.get((B, H, W, d32), bf)
+            k_rows = (k_pl[0, :tkv].view(1, *kv_shape[1:], d32), k_pl[1, :tkv].view(1, *kv_shape[1:], d32))
+            for b in range(B):
+                if ctx is None:      # K of this image straight into the padded planes (its k 1x1 conv's epilogue)
+                    write_k = lambda b=b: be.conv_umma(
+                        B=1, H=H, W=W, Cin=ek["cin"], Cout=d32, taps=1, a_hi=a[0][b:b + 1], a_lo=a[1][b:b + 1],
+                        w_hi=ek["hi"], w_lo=ek["lo"], bias=ek["bias"], out=None, out_hi=k_rows[0], out_lo=k_rows[1],
+                        passes=self.passes)
+                else:
+                    write_k = lambda b=b: be.prep(k[b:b + 1], None, raw_hi=k_rows[0], raw_lo=k_rows[1])
+                self._attention_gemm((q_hi[b:b + 1], q_lo[b:b + 1]), (k_pl[0:1], k_pl[1:2]), (vt_pl[0:1], vt_pl[1:2]),
+                                     v[b].view(tkv, d32), (H, W), tkv, scale, s, p, out_hi=o_hi[b:b + 1],
+                                     out_lo=o_lo[b:b + 1], write_k=write_k)
+            pool.put(q_hi, q_lo, k, v)
+            new, _, _ = self._conv(pool, w[f"{pre}.o{h}"], a_hi=o_hi, a_lo=o_lo, shape=shape, residual=out,
+                                   res_mode=cabi.RES_SAME, stats=stats and h == heads - 1)
+            pool.put(o_hi, o_lo)
+            if out is not residual:
+                pool.put(out)
+            out = new
+        pool.put(s, *p)
         return out
 
     def _stem(self, pool, ent, x):
@@ -626,7 +753,8 @@ class UNetEngine(KernelExecutor):
         T, heads, d = H * W, m.n_heads, m.d_head
         inner = heads * d
         head_dim_ok, rule = cabi.attn_head_dims(be)
-        if not head_dim_ok(d):
+        gemm = cabi.attn_gemm_route(be, d)
+        if not (head_dim_ok(d) or gemm):
             raise NotImplementedError(f"SpatialTransformer head_dim {d}: the sm_90a attention kernels take {rule}")
         if not self._umma_ok(Cc, inner, W):
             raise NotImplementedError(f"SpatialTransformer: channel counts must be multiples of {self.conv_multiple} "
@@ -647,10 +775,34 @@ class UNetEngine(KernelExecutor):
             pool.put(o_hi, o_lo, res)
             return new
 
+        def feed_forward(pre, blk, h):
+            # ---- GEGLU feed-forward -----------------------------------------------------------------------------------
+            if not blk.ff.glu:
+                raise NotImplementedError("SpatialTransformer feed-forward without GEGLU")
+            n_hi, n_lo = layernorm(blk.norm3, h)
+            uu, _, _ = self._conv(pool, w[pre + ".ff.net.0.proj"], a_hi=n_hi, a_lo=n_lo, shape=(B, H, W))
+            pool.put(n_hi, n_lo)
+            ffi = uu.shape[3] // 2
+            g_hi, g_lo = pool.get((B, H, W, ffi), bf), pool.get((B, H, W, ffi), bf)
+            be.geglu_split(uu, out_hi=g_hi, out_lo=g_lo)
+            pool.put(uu)
+            return project_out(w[pre + ".ff.net.2"], g_hi, g_lo, h)
+
         for j, blk in enumerate(m.transformer_blocks):
             pre = f"{name}.transformer_blocks.{j}"
             # ---- self-attention ----------------------------------------------------------------------------------
             n_hi, n_lo = layernorm(blk.norm1, h)
+            if gemm:
+                # heads wider than the flash kernels take: per head GEMMs around the row softmax, to_out per head
+                new = self._attention_heads_gemm(pool, pre + ".attn1", heads, d, (n_hi, n_lo), None, (B, H, W), h,
+                                                 stats=False)
+                pool.put(n_hi, n_lo, h)
+                n_hi, n_lo = layernorm(blk.norm2, new)
+                h = self._attention_heads_gemm(pool, pre + ".attn2", heads, d, (n_hi, n_lo), ctx, (B, H, W), new,
+                                               stats=False)
+                pool.put(n_hi, n_lo, new)
+                h = feed_forward(pre, blk, h)
+                continue
             _, q_hi, q_lo = self._conv(pool, w[pre + ".attn1.qkv"], a_hi=n_hi, a_lo=n_lo, shape=(B, H, W), out_split=True,
                                        want_f32=False)
             pool.put(n_hi, n_lo)
@@ -681,17 +833,7 @@ class UNetEngine(KernelExecutor):
                                kv_lo.view(B, Tc, 2 * inner), heads, None, o_hi.view(B, T, inner), o_lo.view(B, T, inner))
             pool.put(q_hi, q_lo, kv_hi, kv_lo)
             h = project_out(w[pre + ".attn2.to_out.0"], o_hi, o_lo, h)
-            # ---- GEGLU feed-forward -----------------------------------------------------------------------------------
-            if not blk.ff.glu:
-                raise NotImplementedError("SpatialTransformer feed-forward without GEGLU")
-            n_hi, n_lo = layernorm(blk.norm3, h)
-            uu, _, _ = self._conv(pool, w[pre + ".ff.net.0.proj"], a_hi=n_hi, a_lo=n_lo, shape=(B, H, W))
-            pool.put(n_hi, n_lo)
-            ffi = uu.shape[3] // 2
-            g_hi, g_lo = pool.get((B, H, W, ffi), bf), pool.get((B, H, W, ffi), bf)
-            be.geglu_split(uu, out_hi=g_hi, out_lo=g_lo)
-            pool.put(uu)
-            h = project_out(w[pre + ".ff.net.2"], g_hi, g_lo, h)
+            h = feed_forward(pre, blk, h)
         r_hi, r_lo = pool.get(tok, bf), pool.get(tok, bf)
         be.prep(h, None, resample=cabi.RESAMPLE_NONE, raw_hi=r_hi, raw_lo=r_lo)
         pool.put(h)

@@ -634,6 +634,89 @@ def conv1x1(conv1d: torch.nn.Conv1d, x4: torch.Tensor, enabled: bool = True):
     return Conv2dFn.apply(x4, conv1d.weight.unsqueeze(-1), conv1d.bias)
 
 
+def _gemm_heads(be, q, k, v, grid, dout=None, grads=None):
+    """Attention heads wider than the flash kernels take, one (image, head) at a time as tensor-core GEMMs around the
+    materialised row softmax (UNetEngine's route in sampling).  q [B, T, heads, d], k / v [B, Tkv, heads, d]: fp32 views
+    of the saved inputs; grid = (H, W) of the queries (T = H * W).  Each head's slices are copied into zero-padded
+    [T, d32] / [Tkvp, d32] tensors (d32 = d rounded up to 32, Tkvp = Tkv rounded up to 64), and the scratch covers one
+    image-head: no [B * heads, T, Tkv] tensor exists.
+      forward (dout None): out [B, T, heads, d] = softmax(Q K^T d^-1/2) V, through KernelExecutor._attention_gemm.
+      backward: writes dq, dk, dv into grads (views of q's, k's and v's shapes) for dout [B, T, heads, d].  S = Q K^T
+      and dP = dO V^T are recomputed (conv_umma); softmax_rows_split gives the planes of P and, with grad=dP, of dS;
+      dQ = dS K (conv_umma); dK^T = Q^T dS and dV^T = dO^T P are weight gradients over the query pixels (conv_wgrad,
+      taps 1), so only Q and dO need transposed planes, never a [Tkv, T] matrix."""
+    from .engine import KernelExecutor
+    B, T, heads, d = q.shape
+    tkv = k.shape[1]
+    H, W = grid
+    dev = q.device
+    d32, tkvp = cabi.gemm_heads_pad(d), -(-tkv // 64) * 64
+    scale = float(d ** -0.5)
+    bf = torch.bfloat16
+    zeros = lambda *shape: torch.zeros(shape, dtype=torch.float32, device=dev)
+    planes = lambda *shape: torch.empty((2,) + shape, dtype=bf, device=dev)
+    qp, kp, vp = zeros(1, H, W, d32), zeros(tkvp, d32), zeros(tkvp, d32)
+    q_pl, k_pl, kt_pl = planes(1, H, W, d32), planes(1, tkvp, d32), planes(1, d32, tkvp)
+    s = torch.empty((1, H, W, tkvp), dtype=torch.float32, device=dev)
+    ex = KernelExecutor(be)
+    out = None
+    if dout is None:
+        out = torch.empty((B, T, heads, d), dtype=torch.float32, device=dev)
+        vt_pl = torch.zeros((2, 1, d32, tkvp), dtype=bf, device=dev)
+        p_pl, o = planes(1, H, W, tkvp), torch.empty((1, H, W, d32), dtype=torch.float32, device=dev)
+    else:
+        dq, dk, dv = grads
+        v_pl, vt_pl = planes(1, tkvp, d32), planes(1, d32, tkvp)
+        dop, do_pl = zeros(1, H, W, d32), planes(1, H, W, d32)
+        qt_pl, dot_pl = _transposed_planes(d32, T, dev), _transposed_planes(d32, T, dev)
+        dp = torch.empty_like(s)
+        p_pl, ds_pl = planes(1, H, W, tkvp), planes(1, H, W, tkvp)
+        dqo = torch.empty((1, H, W, d32), dtype=torch.float32, device=dev)
+        dkw, dvw = (torch.empty((d32, tkvp, 1, 1), dtype=torch.float32, device=dev) for _ in range(2))
+        ws = torch.empty((be.wgrad_workspace(1, H, W, tkvp, d32, 1)[1],), dtype=torch.float32, device=dev)
+    masked = {} if tkv == tkvp else dict(valid_cols=tkv)
+    for b in range(B):
+        for h in range(heads):
+            qp[..., :d].copy_(q[b, :, h].view(H, W, d))
+            kp[:tkv, :d].copy_(k[b, :, h])
+            vp[:tkv, :d].copy_(v[b, :, h])
+            be.split_grad(kp, k_pl[0], k_pl[1], kt_pl[0, 0], kt_pl[1, 0])
+            if dout is None:
+                be.prep(qp, None, raw_hi=q_pl[0], raw_lo=q_pl[1])
+                ex._attention_gemm((q_pl[0], q_pl[1]), (k_pl[0], k_pl[1]), (vt_pl[0], vt_pl[1]), vp[:tkv], grid, tkv,
+                                   scale, s, (p_pl[0], p_pl[1]), out_f32=o)
+                out[b, :, h].copy_(o.view(T, d32)[:, :d])
+                continue
+            be.split_grad(qp.view(T, d32), q_pl[0].view(T, d32), q_pl[1].view(T, d32), *qt_pl)
+            be.split_grad(vp, v_pl[0], v_pl[1], vt_pl[0, 0], vt_pl[1, 0])
+            dop[..., :d].copy_(dout[b, :, h].view(H, W, d))
+            be.split_grad(dop.view(T, d32), do_pl[0].view(T, d32), do_pl[1].view(T, d32), *dot_pl)
+            be.conv_umma(B=1, H=H, W=W, Cin=d32, Cout=tkvp, taps=1, a_hi=q_pl[0], a_lo=q_pl[1], w_hi=k_pl[0],
+                         w_lo=k_pl[1], out=s, passes=3)
+            be.conv_umma(B=1, H=H, W=W, Cin=d32, Cout=tkvp, taps=1, a_hi=do_pl[0], a_lo=do_pl[1], w_hi=v_pl[0],
+                         w_lo=v_pl[1], out=dp, passes=3)
+            s2, dp2 = s.view(T, tkvp), dp.view(T, tkvp)
+            be.softmax_rows_split(s2, scale, p_pl[0].view(T, tkvp), p_pl[1].view(T, tkvp), **masked)
+            be.softmax_rows_split(s2, scale, ds_pl[0].view(T, tkvp), ds_pl[1].view(T, tkvp), grad=dp2, **masked)
+            be.conv_umma(B=1, H=H, W=W, Cin=tkvp, Cout=d32, taps=1, a_hi=ds_pl[0], a_lo=ds_pl[1], w_hi=kt_pl[0],
+                         w_lo=kt_pl[1], out=dqo, passes=3)
+            be.conv_wgrad(*qt_pl, ds_pl[0], ds_pl[1], 1, H, W, tkvp, d32, 1, dkw, ws)
+            be.conv_wgrad(*dot_pl, p_pl[0], p_pl[1], 1, H, W, tkvp, d32, 1, dvw, ws)
+            dq[b, :, h].copy_(dqo.view(T, d32)[:, :d])
+            dk[b, :, h].copy_(dkw.view(d32, tkvp)[:d, :tkv].t())
+            dv[b, :, h].copy_(dvw.view(d32, tkvp)[:d, :tkv].t())
+    return out
+
+
+def _qkv_heads(t, heads, order):
+    """q, k, v views [B, T, heads, d] of an NHWC qkv tensor [B, H, W, 3C]: order 1 puts head h's q, k, v at channels
+    h*d, C + h*d, 2C + h*d; order 0 (legacy) at 3hd, 3hd + d, 3hd + 2d."""
+    B, H, W, C3 = t.shape
+    d = C3 // 3 // heads
+    v = t.view(B, H * W, 3, heads, d) if order else t.view(B, H * W, heads, 3, d).transpose(2, 3)
+    return v[:, :, 0], v[:, :, 1], v[:, :, 2]
+
+
 class AttentionCoreFn(torch.autograd.Function):
     """softmax((q s)(k s)^T) v per head (QKVAttentionLegacy / QKVAttention, openaimodel.py:350-413) on a
     [B,3C,H,W] qkv tensor -> [B,C,H,W].  Forward: the sampling path's attention kernels (wgmma for
@@ -649,13 +732,16 @@ class AttentionCoreFn(torch.autograd.Function):
         Cc, T = C3 // 3, H * W
         dev = qkv.device
         qn = _nhwc(qkv.detach()).contiguous()
-        out = torch.empty((B, T, Cc), dtype=torch.float32, device=dev)
-        if Cc // heads in cabi.ATTN_TC_HEAD_DIMS:
+        if cabi.attn_gemm_route(be, Cc // heads):
+            out = _gemm_heads(be, *_qkv_heads(qn, heads, order), (H, W)).view(B, T, Cc)
+        elif Cc // heads in cabi.ATTN_TC_HEAD_DIMS:
+            out = torch.empty((B, T, Cc), dtype=torch.float32, device=dev)
             q_hi = torch.empty((B, H, W, C3), dtype=torch.bfloat16, device=dev)
             q_lo = torch.empty_like(q_hi)
             be.prep(qn, None, raw_hi=q_hi, raw_lo=q_lo)
             be.attention_tc(q_hi.view(B, T, C3), q_lo.view(B, T, C3), heads, order, out, None, None)
         else:
+            out = torch.empty((B, T, Cc), dtype=torch.float32, device=dev)
             be.attention(qn.view(B, T, C3), heads, order, out, None, None)
         ctx.save_for_backward(qn, out)
         ctx.heads, ctx.order = heads, order
@@ -670,6 +756,10 @@ class AttentionCoreFn(torch.autograd.Function):
         dev = dout.device
         don = _nhwc(dout).contiguous()
         dqkv = torch.empty_like(qn)
+        if cabi.attn_gemm_route(be, C3 // 3 // ctx.heads):
+            _gemm_heads(be, *_qkv_heads(qn, ctx.heads, ctx.order), (H, W), dout=don.view(B, T, ctx.heads, -1),
+                        grads=_qkv_heads(dqkv, ctx.heads, ctx.order))
+            return dqkv.permute(0, 3, 1, 2), None, None
         lse = torch.empty((B * ctx.heads * T,), dtype=torch.float32, device=dev)
         delta = torch.empty_like(lse)
         be.attention_bwd(qn.view(B, T, C3), out, don.view(B, T, C3 // 3), ctx.heads, ctx.order,
@@ -681,7 +771,8 @@ def attention_core(qkv4: torch.Tensor, heads: int, new_order: bool, enabled: boo
     """[B,3C,H,W] -> [B,C,H,W] or None when the native kernels do not take the shape."""
     B, C3, H, W = qkv4.shape
     hd = C3 // 3 // heads
-    if not (enabled and _on_device(qkv4) and qkv4.dtype == torch.float32 and cabi.attn_head_dims(backend())[0](hd)
+    if not (enabled and _on_device(qkv4) and qkv4.dtype == torch.float32
+            and (cabi.attn_head_dims(backend())[0](hd) or (cabi.attn_gemm_route(backend(), hd) and W >= 4))
             and (C3 // 3) % 4 == 0 and B * heads <= 65535):
         return None
     return AttentionCoreFn.apply(qkv4, heads, 1 if new_order else 0)
@@ -776,6 +867,12 @@ class CrossAttentionCoreFn(torch.autograd.Function):
         Tq, Tkv = H * W, kv.shape[2] * kv.shape[3]
         dev = q.device
         qn, kvn = _nhwc(q.detach()).contiguous(), _nhwc(kv.detach()).contiguous()
+        ctx.heads = heads
+        if cabi.attn_gemm_route(be, Cc // heads):
+            kv5 = kvn.view(B, Tkv, 2, heads, -1)
+            out = _gemm_heads(be, qn.view(B, Tq, heads, -1), kv5[:, :, 0], kv5[:, :, 1], (H, W)).view(B, Tq, Cc)
+            ctx.save_for_backward(qn, kvn, out)
+            return out.view(B, H, W, Cc).permute(0, 3, 1, 2)
         planes = []
         for t in (qn, kvn):
             hi = torch.empty(t.shape, dtype=torch.bfloat16, device=dev)
@@ -799,6 +896,12 @@ class CrossAttentionCoreFn(torch.autograd.Function):
         dev = dout.device
         don = _nhwc(dout).contiguous()
         dq, dkv = torch.empty_like(qn), torch.empty_like(kvn)
+        if cabi.attn_gemm_route(be, Cc // ctx.heads):
+            kv5, dkv5 = kvn.view(B, Tkv, 2, ctx.heads, -1), dkv.view(B, Tkv, 2, ctx.heads, -1)
+            _gemm_heads(be, qn.view(B, Tq, ctx.heads, -1), kv5[:, :, 0], kv5[:, :, 1], (H, W),
+                        dout=don.view(B, Tq, ctx.heads, -1), grads=(dq.view(B, Tq, ctx.heads, -1), dkv5[:, :, 0],
+                                                                    dkv5[:, :, 1]))
+            return dq.permute(0, 3, 1, 2), dkv.permute(0, 3, 1, 2), None
         lse = torch.empty((B * ctx.heads * Tq,), dtype=torch.float32, device=dev)
         delta = torch.empty_like(lse)
         be.attention_cross_bwd(qn.view(B, Tq, Cc), kvn.view(B, Tkv, 2 * Cc), out, don.view(B, Tq, Cc), ctx.heads,

@@ -126,15 +126,11 @@ class VQGANEngine(KernelExecutor):
             p_hi, p_lo = pool.get((1, H, W, T), torch.bfloat16), pool.get((1, H, W, T), torch.bfloat16)
             scale = float(int(Cc) ** (-0.5))
             for b in range(B):
-                # V^T planes [C][T] = the K-major B operand of O = P V (same kernel as the wgrad operand split)
-                be.split_grad(v[b].view(T, Cc), None, None, vt_hi[b], vt_lo[b])
-                # S[t, s] = sum_c q[t, c] k[s, c]: the K planes of this image ARE a [Cout=T][Cin=C] weight
-                be.conv_umma(B=1, H=H, W=W, Cin=Cc, Cout=T, taps=1, a_hi=q_hi[b:b + 1], a_lo=q_lo[b:b + 1],
-                             w_hi=k_hi[b].view(1, T, Cc), w_lo=k_lo[b].view(1, T, Cc), out=s, passes=self.passes)
-                be.softmax_rows_split(s.view(T, T), scale, p_hi.view(T, T), p_lo.view(T, T))
-                be.conv_umma(B=1, H=H, W=W, Cin=T, Cout=Cc, taps=1, a_hi=p_hi, a_lo=p_lo,
-                             w_hi=vt_hi[b].view(1, Cc, T), w_lo=vt_lo[b].view(1, Cc, T), out=None,
-                             out_hi=o_hi[b:b + 1], out_lo=o_lo[b:b + 1], passes=self.passes)
+                # S[t, s] = sum_c q[t, c] k[s, c]: the K planes of this image ARE a [Cout=T][Cin=C] weight; V^T planes
+                # [C][T] are the K-major B operand of O = P V
+                self._attention_gemm((q_hi[b:b + 1], q_lo[b:b + 1]), (k_hi[b].view(1, T, Cc), k_lo[b].view(1, T, Cc)),
+                                     (vt_hi[b].view(1, Cc, T), vt_lo[b].view(1, Cc, T)), v[b].view(T, Cc), (H, W), T,
+                                     scale, s, (p_hi, p_lo), out_hi=o_hi[b:b + 1], out_lo=o_lo[b:b + 1])
             pool.put(q_hi, q_lo, k_hi, k_lo, v, vt_hi, vt_lo, s, p_hi, p_lo)
         pool.put(a_f32, a_hi, a_lo)
         out, _, _ = self._conv(pool, ep, a_f32=o_f32, a_hi=o_hi, a_lo=o_lo, shape=(B, H, W), residual=x,
@@ -163,15 +159,13 @@ class VQGANEngine(KernelExecutor):
         p_hi, p_lo = pool.get((1, H, W, Tp), bf16), pool.get((1, H, W, Tp), bf16)
         scale = float(int(Cc) ** (-0.5))
         for b in range(B):
-            be.conv_umma(B=1, H=H, W=W, Cin=Cc, Cout=Cc, taps=1, a_hi=a_hi[b:b + 1], a_lo=a_lo[b:b + 1], w_hi=ek["hi"],
-                         w_lo=ek["lo"], bias=ek["bias"], out=None, out_hi=k_pl[0, :T].view(1, H, W, Cc),
-                         out_lo=k_pl[1, :T].view(1, H, W, Cc), passes=self.passes)
-            be.split_grad(v[b].view(T, Cc), None, None, vt_pl[0, :, :T], vt_pl[1, :, :T])
-            be.conv_umma(B=1, H=H, W=W, Cin=Cc, Cout=Tp, taps=1, a_hi=q_hi[b:b + 1], a_lo=q_lo[b:b + 1],
-                         w_hi=k_pl[0:1], w_lo=k_pl[1:2], out=s, passes=self.passes)
-            be.softmax_rows_split(s.view(T, Tp), scale, p_hi.view(T, Tp), p_lo.view(T, Tp), valid_cols=T)
-            be.conv_umma(B=1, H=H, W=W, Cin=Tp, Cout=Cc, taps=1, a_hi=p_hi, a_lo=p_lo, w_hi=vt_pl[0:1],
-                         w_lo=vt_pl[1:2], out=None, out_hi=o_hi[b:b + 1], out_lo=o_lo[b:b + 1], passes=self.passes)
+            write_k = lambda b=b: be.conv_umma(
+                B=1, H=H, W=W, Cin=Cc, Cout=Cc, taps=1, a_hi=a_hi[b:b + 1], a_lo=a_lo[b:b + 1], w_hi=ek["hi"],
+                w_lo=ek["lo"], bias=ek["bias"], out=None, out_hi=k_pl[0, :T].view(1, H, W, Cc),
+                out_lo=k_pl[1, :T].view(1, H, W, Cc), passes=self.passes)
+            self._attention_gemm((q_hi[b:b + 1], q_lo[b:b + 1]), (k_pl[0:1], k_pl[1:2]), (vt_pl[0:1], vt_pl[1:2]),
+                                 v[b].view(T, Cc), (H, W), T, scale, s, (p_hi, p_lo), out_hi=o_hi[b:b + 1],
+                                 out_lo=o_lo[b:b + 1], write_k=write_k)
         pool.put(q_hi, q_lo, v, s, p_hi, p_lo)
         return o_hi, o_lo
 

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define BBDM_ABI_VERSION 9
+#define BBDM_ABI_VERSION 10
 
 enum {
   BBDM_OK = 0,
@@ -553,6 +553,14 @@ int bbdm_attention_bwd(const float* qkv, const float* out, const float* dout, in
  * the rest (the padding of a token axis rounded up to the GEMM tile).  valid_cols == cols: the whole row. */
 int bbdm_softmax_rows_split(const float* src, int64_t rows, int64_t cols, int64_t valid_cols, float scale,
                             void* out_hi, void* out_lo, void* stream);
+
+/* Backward of that row softmax, for attention run as two GEMMs around it (heads wider than the flash kernels take):
+ * from the scores s and dp = dL/dp ([rows, cols] fp32, row-major), recomputes p = softmax(scale * s) over the first
+ * valid_cols columns with bbdm_softmax_rows_split's max, sum and expf order, and writes the score gradient
+ * ds = scale * p * (dp - sum_j p_j dp_j) as split-bf16 planes (exact zeros past valid_cols).  cols % 4 == 0.
+ * Deterministic (fixed reduction order). */
+int bbdm_softmax_rows_bwd(const float* s, const float* dp, int64_t rows, int64_t cols, int64_t valid_cols, float scale,
+                          void* ds_hi, void* ds_lo, void* stream);
 
 /* Space-to-depth by 2 with bf16 split: src [B,H,W,C] fp32 -> planes [B,H/2,W/2,4C], channel
  * (row parity*2 + col parity)*C + c.  With it the VQGAN Downsample (zero-pad (0,1,0,1) + 3x3 stride-2 conv,
