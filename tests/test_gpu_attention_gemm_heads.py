@@ -11,6 +11,7 @@ import pytest
 import torch
 
 from _gemm_heads import GEMM_HEAD_CONFIGS
+from _launch_guard import canaried, tail_untouched
 from _launch_shadow import Shadow, pair_well_formed
 from _launch_shadow_gemm_heads import GemmHeadsShadow
 from _recipe import UNET_CONFIGS, fill_state_dict, rel_dev, synth_images
@@ -20,8 +21,6 @@ from test_gpu_attention_head_dims import _Recorder, _same, _step, build, load, r
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 TOL_PSAMPLE = 1e-4
-CANARY = 1234.5
-CANARY_N = 4096
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -37,19 +36,6 @@ def be():
     b = cabi.CudaBackend()
     yield b
     b.check_fault()
-
-
-def canaried(shape, dtype=torch.float32):
-    n = 1
-    for s in shape:
-        n *= s
-    buf = torch.full((n + CANARY_N,), float("nan"), dtype=dtype, device=DEV)
-    buf[n:] = CANARY
-    return buf[:n].view(shape), buf
-
-
-def tail_untouched(buf):
-    return bool((buf[-CANARY_N:] == torch.tensor(CANARY, dtype=buf.dtype)).all())
 
 
 # ------------------------------------------------------------------------------------ softmax backward kernel

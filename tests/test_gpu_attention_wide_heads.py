@@ -8,6 +8,7 @@ import gc
 import pytest
 import torch
 
+from _launch_guard import canaried, tail_untouched
 from _launch_shadow import Shadow
 from _recipe import fill_state_dict, rel_dev, synth_images
 from _wide_heads import WIDE_HEAD_CONFIGS
@@ -19,8 +20,6 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda"
 TOL_PSAMPLE = 1e-4
 WIDE_DIMS = [136, 160, 192, 200, 256]
-CANARY = 1234.5
-CANARY_N = 4096
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -36,20 +35,6 @@ def be():
     b = cabi.CudaBackend()
     yield b
     b.check_fault()
-
-
-def canaried(shape, dtype=torch.float32):
-    """(view of shape pre-filled with NaN, whole buffer): CANARY_N canary elements sit right behind the view."""
-    n = 1
-    for s in shape:
-        n *= s
-    buf = torch.full((n + CANARY_N,), float("nan"), dtype=dtype, device=DEV)
-    buf[n:] = CANARY
-    return buf[:n].view(shape), buf
-
-
-def tail_untouched(buf):
-    return bool((buf[-CANARY_N:] == torch.tensor(CANARY, dtype=buf.dtype)).all())
 
 
 def outputs(B, T, C):

@@ -13,6 +13,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from _launch_guard import CANARY, canaried as _canaried, tail_untouched
 from _launch_shadow import Shadow
 from _recipe import bb_namespace, fill_state_dict, rel_dev, synth_images
 from _widths import WIDTH_CONFIGS
@@ -22,8 +23,6 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda"
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 TOL_PSAMPLE = 1e-4
-CANARY = 1234.5
-CANARY_N = 4096
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -52,14 +51,8 @@ def split(x):
 
 
 def canaried(shape, dtype=torch.float32):
-    """(view of shape, whole buffer): a tail of CANARY_N canary elements sits right behind the view."""
-    n = int(np.prod(shape))
-    buf = torch.full((n + CANARY_N,), CANARY, dtype=dtype, device=DEV)
-    return buf[:n].view(shape), buf
-
-
-def tail_untouched(buf):
-    return bool((buf[-CANARY_N:] == torch.tensor(CANARY, dtype=buf.dtype)).all())
+    """(view of shape, whole buffer): the view and the tail of CANARY_N elements behind it hold CANARY."""
+    return _canaried(shape, dtype, DEV, fill=CANARY)
 
 
 # ------------------------------------------------------------------------------------------ conv_umma
