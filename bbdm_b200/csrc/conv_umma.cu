@@ -419,6 +419,218 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
   }
 }
 
+// ---- Winograd position GEMMs (weights_per_image, fp32 NHWC store + optional bias) ---------------------------------
+// Same tiles, ring, products, chunk boundaries and fold order as conv_umma_kernel, so the result is bit-identical; two
+// things differ.  A finished tile needs no epilogue state (no residual, statistics or split outputs): the consumers
+// store it straight from the fp32 sum and keep nothing across the next tile.  The registers that frees hold a second
+// chunk accumulator: chunk c + 1 is issued into one while chunk c, in the other, waits for its fold.  The fold runs
+// after chunk c + 1's first K block is committed and `wgmma_wait<1>` has retired chunk c, so the tensor core is never
+// drained at a chunk boundary; only a CTA's last tile ends in `wgmma_wait<0>`.
+
+template <int BN, bool F16>
+__device__ __forceinline__ void wino_mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+  if (F16) {
+    if (BN == 128) wgmma_n128_f16<0>(d, da, db, scale_d); else wgmma_n64_f16<0>(d, da, db, scale_d);
+  } else {
+    if (BN == 128) wgmma_n128_bf16<0>(d, da, db, scale_d); else wgmma_n64_bf16<0>(d, da, db, scale_d);
+  }
+}
+
+// One row block of a finished tile: out[pix, n] = racc (+ bias), columns nb * BN .. nb * BN + BN - 1 (BN divides
+// Cout on this route).
+template <int BN>
+__device__ __forceinline__ void wino_store(const ConvParams& p, const float* racc, int tile, int n_blocks, int warp,
+                                           int lane) {
+  const int nb = tile % n_blocks;
+  int mt = tile / n_blocks;
+  const int tw = mt % p.tiles_w; mt /= p.tiles_w;
+  const int th = mt % p.tiles_h;
+  const int tb = mt / p.tiles_h;                 // transform position (TB == 1: a tile lies inside one position)
+  const int n0 = nb * BN + 2 * (lane & 3);
+#pragma unroll
+  for (int ri = 0; ri < 2; ++ri) {
+    const int row = 16 * warp + (lane >> 2) + 8 * ri;
+    const int ws = tw * p.TW + row % p.TW, hs = th * p.TH + row / p.TW;
+    if (ws >= p.W || hs >= p.H) continue;
+    float* op = p.out + (((int64_t)tb * p.H + hs) * p.W + ws) * p.Cout + n0;
+#pragma unroll
+    for (int jj = 0; jj < BN / 8; ++jj) {
+      float2 v = make_float2(racc[4 * jj + 2 * ri], racc[4 * jj + 2 * ri + 1]);
+      if (p.bias) { const float2 b = *reinterpret_cast<const float2*>(p.bias + n0 + 8 * jj); v.x += b.x; v.y += b.y; }
+      *reinterpret_cast<float2*>(op + 8 * jj) = v;
+    }
+  }
+}
+
+// Consumer side of the position-GEMM kernel: where the chunk stream stands.  `tile`, `kb0`: the next chunk to issue;
+// the pending chunk (issued, not yet folded) belongs to `pend_tile` and starts (`pend_first`) or ends (`pend_last`)
+// that tile's K loop.
+struct WinoStream {
+  int tile, kb0, stage, prev, pend_tile;
+  uint32_t phase_bit;
+  bool pend, pend_first, pend_last;
+};
+
+// Folds the pending chunk's accumulator into racc (round-to-nearest, the order of conv_umma_kernel) and stores a
+// finished tile.  The caller has retired the chunk's wgmmas.
+template <int BN>
+__device__ __forceinline__ void wino_fold(const ConvParams& p, WinoStream& s, float* racc, float* acc, int n_blocks,
+                                          int warp, int lane) {
+  constexpr int NR = BN / 2;
+  reg_fence<NR>(acc);
+  if (s.pend_first) {
+#pragma unroll
+    for (int j = 0; j < NR; ++j) racc[j] = 0.f + acc[j];
+  } else {
+#pragma unroll
+    for (int j = 0; j < NR; ++j) racc[j] += acc[j];
+  }
+  if (s.pend_last) wino_store<BN>(p, racc, s.pend_tile, n_blocks, warp, lane);
+  s.pend = false;
+}
+
+// Issues the next chunk into `acc` and folds the pending one (in `other`) once the chunk's first K block is in
+// flight.  Returns false when the CTA has no chunk left (nothing issued; the pending chunk is still in `other`).
+template <int BN, int PASSES, bool F16, uint32_t STAGE_BYTES, int STAGES>
+__device__ __forceinline__ bool wino_chunk(const ConvParams& p, WinoStream& s, float* racc, float* acc, float* other,
+                                           uint32_t tiles_base, uint32_t bar_full, uint32_t bar_empty,
+                                           volatile int* abort_flag, int total_tiles, int n_blocks, int KB, int warp,
+                                           int lane) {
+  constexpr int NR = BN / 2;
+  constexpr uint32_t OFF_ALO = UmmaCfg<BN>::A_BYTES;
+  constexpr uint32_t OFF_WHI = PASSES == 3 ? 2 * UmmaCfg<BN>::A_BYTES : UmmaCfg<BN>::A_BYTES;
+  constexpr uint32_t OFF_WLO = OFF_WHI + UmmaCfg<BN>::W_BYTES;
+  if (s.tile >= total_tiles) return false;
+  const uint32_t a_off = (uint32_t)(warp >> 2) * 64 * 128;
+  const int kb1 = s.kb0 + p.kb_per_chunk < KB ? s.kb0 + p.kb_per_chunk : KB;
+  for (int kb = s.kb0; kb < kb1; ++kb) {
+    mbar_wait(bar_full + 8 * s.stage, s.phase_bit, abort_flag, p.fault, 0xF6000000ull | (unsigned)kb);
+    const uint32_t sbase = tiles_base + s.stage * STAGE_BYTES;
+    const uint64_t da_hi = make_sw128_desc(sbase + a_off);
+    const uint64_t da_lo = make_sw128_desc(sbase + OFF_ALO + a_off);
+    const uint64_t db_hi = make_sw128_desc(sbase + OFF_WHI);
+    const uint64_t db_lo = make_sw128_desc(sbase + OFF_WLO);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < UM_BK / 16; ++k) {
+      const uint64_t ko = (uint64_t)(k * 32 >> 4);
+      // the chunk's first product overwrites the accumulator (scale-d = 0): the chunk starts from zero without a
+      // register write that the tensor core would have to wait for
+      const uint32_t keep = (k == 0 && kb == s.kb0) ? 0u : 1u;
+      if (PASSES == 3) {
+        wino_mma<BN, F16>(acc, da_lo + ko, db_hi + ko, keep);
+        wino_mma<BN, F16>(acc, da_hi + ko, db_lo + ko, 1u);
+      }
+      wino_mma<BN, F16>(acc, da_hi + ko, db_hi + ko, PASSES == 3 ? 1u : keep);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();                         // everything before this K block has retired: free the previous slot
+    if (s.prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * s.prev);
+    s.prev = s.stage;
+    if (++s.stage == STAGES) { s.stage = 0; s.phase_bit ^= 1; }
+    if (s.pend) wino_fold<BN>(p, s, racc, other, n_blocks, warp, lane);
+  }
+  s.pend = true;
+  s.pend_tile = s.tile;
+  s.pend_first = s.kb0 == 0;
+  s.pend_last = kb1 == KB;
+  s.kb0 = kb1;
+  if (s.kb0 == KB) { s.kb0 = 0; s.tile += gridDim.x; }
+  return true;
+}
+
+template <int BN, int PASSES, bool F16>
+__device__ __forceinline__ void wino_drain(const ConvParams& p, WinoStream& s, float* racc, float* acc,
+                                           uint32_t bar_empty, int n_blocks, int warp, int lane) {
+  if (!s.pend) return;
+  wgmma_wait<0>();
+  if (lane == 0) mbar_arrive(bar_empty + 8 * s.prev);
+  wino_fold<BN>(p, s, racc, acc, n_blocks, warp, lane);
+}
+
+template <int BN, int PASSES, bool F16>
+__global__ void __launch_bounds__(UM_THREADS, 1)
+wino_gemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
+                 const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
+                 const ConvParams p) {
+  using Cfg = UmmaCfg<BN>;
+  constexpr int STAGES = PASSES == 3 ? Cfg::STAGES3 : Cfg::STAGES1;
+  constexpr uint32_t STAGE_BYTES = PASSES == 3 ? Cfg::STAGE3 : Cfg::STAGE1;
+  constexpr uint32_t OFF_ALO = Cfg::A_BYTES;
+  constexpr uint32_t OFF_WHI = PASSES == 3 ? 2 * Cfg::A_BYTES : Cfg::A_BYTES;
+  constexpr uint32_t OFF_WLO = OFF_WHI + Cfg::W_BYTES;
+  constexpr int NR = BN / 2;
+  static_assert(STAGES >= 2, "need at least a double buffer");
+
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t bars[2 * 8];
+  __shared__ int abort_s;
+
+  const uint32_t tiles_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t bar_full = smem_u32(&bars[0]);
+  const uint32_t bar_empty = smem_u32(&bars[8]);
+  volatile int* abort_flag = &abort_s;
+
+  if (threadIdx.x == 0) {
+    abort_s = 0;
+    for (int i = 0; i < STAGES; ++i) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, 8); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  const int n_blocks = p.Cout / BN;
+  const int total_tiles = p.n_tiles * n_blocks;
+  const int KB = p.K1;
+
+  if (warp >= 8) {
+    setmaxnreg_dec<UM_PRODUCER_REGS>();
+    if (warp == 8 && lane == 0) {
+      int stage = 0;
+      uint32_t phase_bit = 0;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int nb = tile % n_blocks;
+        int mt = tile / n_blocks;
+        const int tw = mt % p.tiles_w; mt /= p.tiles_w;
+        const int th = mt % p.tiles_h;
+        const int tb = mt / p.tiles_h;
+        const int w0 = tw * p.TW, h0 = th * p.TH, n0 = nb * BN;
+        for (int kb = 0; kb < KB; ++kb) {
+          mbar_wait(bar_empty + 8 * stage, phase_bit ^ 1, abort_flag, p.fault, 0xE6000000ull | (unsigned)kb);
+          const uint32_t sbase = tiles_base + stage * STAGE_BYTES;
+          const uint32_t full = bar_full + 8 * stage;
+          mbar_expect_tx(full, STAGE_BYTES);
+          tma_load_4d(sbase, &map_a_hi, full, kb * UM_BK, w0, h0, tb);
+          if (PASSES == 3) tma_load_4d(sbase + OFF_ALO, &map_a_lo, full, kb * UM_BK, w0, h0, tb);
+          tma_load_3d(sbase + OFF_WHI, &map_w_hi, full, kb * UM_BK, n0, tb);
+          if (PASSES == 3) tma_load_3d(sbase + OFF_WLO, &map_w_lo, full, kb * UM_BK, n0, tb);
+          if (++stage == STAGES) { stage = 0; phase_bit ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+
+  setmaxnreg_inc<UM_CONSUMER_REGS>();
+  float racc[NR], acc0[NR], acc1[NR];
+  WinoStream s;
+  s.tile = blockIdx.x; s.kb0 = 0; s.stage = 0; s.prev = -1; s.pend_tile = -1; s.phase_bit = 0;
+  s.pend = s.pend_first = s.pend_last = false;
+  // chunks alternate between the two accumulators; each call folds the chunk the other one holds
+  for (;;) {
+    if (!wino_chunk<BN, PASSES, F16, STAGE_BYTES, STAGES>(p, s, racc, acc0, acc1, tiles_base, bar_full, bar_empty,
+                                                          abort_flag, total_tiles, n_blocks, KB, warp, lane)) {
+      wino_drain<BN, PASSES, F16>(p, s, racc, acc1, bar_empty, n_blocks, warp, lane);
+      break;
+    }
+    if (!wino_chunk<BN, PASSES, F16, STAGE_BYTES, STAGES>(p, s, racc, acc1, acc0, tiles_base, bar_full, bar_empty,
+                                                          abort_flag, total_tiles, n_blocks, KB, warp, lane)) {
+      wino_drain<BN, PASSES, F16>(p, s, racc, acc0, bar_empty, n_blocks, warp, lane);
+      break;
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------- host side
 // bf16 NHWC activation [B,H,W,C] -> 4-D map (C, W, H, B), box (64, TW, TH, TB), SWIZZLE_128B
 static int make_act_map(CUtensorMap* m, const void* ptr, int B, int H, int W, int C, int TW, int TH, int TB,
@@ -469,6 +681,22 @@ static int launch_conv(const CUtensorMap* maps, const ConvParams& p, int grid, c
   }
   conv_umma_kernel<BN, PASSES, F16><<<grid, UM_THREADS, smem, s>>>(maps[0], maps[1], maps[2], maps[3], maps[4], maps[5],
                                                                   maps[6], maps[7], p);
+  BBDM_LAUNCH_CHECK();
+  return BBDM_OK;
+}
+
+template <int BN, int PASSES, bool F16>
+static int launch_wino(const CUtensorMap* maps, const ConvParams& p, int grid, cudaStream_t s) {
+  using Cfg = UmmaCfg<BN>;
+  constexpr int STAGES = PASSES == 3 ? Cfg::STAGES3 : Cfg::STAGES1;
+  constexpr uint32_t STAGE_BYTES = PASSES == 3 ? Cfg::STAGE3 : Cfg::STAGE1;
+  const size_t smem = (size_t)STAGES * STAGE_BYTES + 1024;
+  static DeviceOnce configured;
+  if (configured.need()) {
+    BBDM_CUDA_CHECK(cudaFuncSetAttribute(wino_gemm_kernel<BN, PASSES, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    configured.mark();
+  }
+  wino_gemm_kernel<BN, PASSES, F16><<<grid, UM_THREADS, smem, s>>>(maps[0], maps[1], maps[2], maps[3], p);
   BBDM_LAUNCH_CHECK();
   return BBDM_OK;
 }
@@ -585,6 +813,15 @@ extern "C" int bbdm_conv_umma(const BbdmConvArgs* a, void* stream) {
   const int grid = (int)(total < num_sms() ? total : num_sms());
   cudaStream_t s = (cudaStream_t)stream;
   const bool p3 = a->passes == 3;
+  // position GEMMs whose epilogue is a plain store (+ bias): the kernel without epilogue state (the Winograd route)
+  if (wpi && p.res_mode == BBDM_RES_NONE && !p.stats && !p.out_hi && !p.out_nchw_c && p.out) {
+    if (BN == 128) {
+      if (f16) return p3 ? launch_wino<128, 3, true>(maps, p, grid, s) : launch_wino<128, 1, true>(maps, p, grid, s);
+      return p3 ? launch_wino<128, 3, false>(maps, p, grid, s) : launch_wino<128, 1, false>(maps, p, grid, s);
+    }
+    if (f16) return p3 ? launch_wino<64, 3, true>(maps, p, grid, s) : launch_wino<64, 1, true>(maps, p, grid, s);
+    return p3 ? launch_wino<64, 3, false>(maps, p, grid, s) : launch_wino<64, 1, false>(maps, p, grid, s);
+  }
   if (BN == 128) {
     if (f16) return p3 ? launch_conv<128, 3, true>(maps, p, grid, s) : launch_conv<128, 1, true>(maps, p, grid, s);
     return p3 ? launch_conv<128, 3, false>(maps, p, grid, s) : launch_conv<128, 1, false>(maps, p, grid, s);
