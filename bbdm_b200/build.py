@@ -15,7 +15,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.environ.get("BBDM_LIB_OUT") or os.path.join(HERE, "libbbdm_b200.so")   # BBDM_LIB_OUT: experiment builds
-SOURCES = ["cabi.cu", "elementwise.cu", "groupnorm.cu", "conv_direct.cu", "conv_umma.cu", "attention_split.cu", "attention_split_padded.cu", "attention_split_wide.cu", "attention_tc.cu", "conv_wgrad.cu", "gn_backward.cu", "attention_bwd.cu", "attention_bwd_wide.cu", "vqgan_ops.cu", "winograd.cu", "optim.cu", "transformer_ops.cu"]
+SOURCES = ["cabi.cu", "elementwise.cu", "groupnorm.cu", "conv_direct.cu", "conv_umma.cu", "attention_split.cu", "attention_split_padded.cu", "attention_split_wide.cu", "attention_tc.cu", "conv_wgrad.cu", "gn_backward.cu", "attention_bwd.cu", "attention_bwd_wide.cu", "attention_pad.cu", "vqgan_ops.cu", "winograd.cu", "optim.cu", "transformer_ops.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]

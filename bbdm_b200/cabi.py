@@ -17,7 +17,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BBDM_LIB selects another in-tree build of the same sources (A/B experiments, tools/); the product default is fixed
 LIB_PATH = os.environ.get("BBDM_LIB") or os.path.join(_HERE, "libbbdm_b200.so")
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 OBJ = {"grad": 0, "noise": 1, "ysubx": 2}
 RESAMPLE_NONE, RESAMPLE_UP2, RESAMPLE_DOWN2 = 0, 1, 2
 RES_NONE, RES_SAME, RES_UP2, RES_DOWN2 = 0, 1, 2, 3
@@ -44,6 +44,24 @@ def attn_gemm_route(be, d):
     """True when backend ``be`` runs attention heads of width d as GEMMs around a materialised row softmax (one image
     and head at a time): d is above its attn_max_head_dim and it declares attn_gemm_route."""
     return bool(getattr(be, "attn_gemm_route", False)) and d > getattr(be, "attn_max_head_dim", 128)
+
+
+def attn_pad_route(be, d):
+    """True when backend ``be`` runs attention heads of width d on its attention kernels at d rounded up to 8 (the
+    heads repacked by prep(heads=...)): d is not a multiple of 8, at most its
+    attn_max_head_dim, and it declares attn_pad_heads."""
+    return bool(getattr(be, "attn_pad_heads", False)) and d % 8 != 0 and 0 < d <= getattr(be, "attn_max_head_dim", 128)
+
+
+def pad_heads_width(d):
+    """Width dp of a head of width d on the padded-head route: d rounded up to 8."""
+    return -(-d // 8) * 8
+
+
+def pad_heads_scale(d):
+    """(dp/d)^(1/4): the factor the padded-head route folds into q and k, so that the kernels' softmax scale dp^-1/2
+    (planes) or (dp^-1/4)^2 (fp32 qkv) becomes the reference's d^-1/2."""
+    return (pad_heads_width(d) / d) ** 0.25
 
 
 def gemm_heads_pad(d):
@@ -86,6 +104,7 @@ SYMBOLS = [
     "bbdm_optim_chunk_elems", "bbdm_adam_multi", "bbdm_adam_multi_dev", "bbdm_ema_multi", "bbdm_denorm_to_uint8",
     "bbdm_layernorm_split", "bbdm_geglu_split", "bbdm_attention_cross", "bbdm_conv_stem", "bbdm_spatial_rescale",
     "bbdm_layernorm_bwd", "bbdm_geglu_bwd", "bbdm_attention_cross_bwd",
+    "bbdm_attention_pad_heads", "bbdm_attention_unpad_heads",
 ]
 
 
@@ -209,6 +228,8 @@ def load():
     lib.bbdm_layernorm_bwd.argtypes = [vp, vp, i64, i, vp, f, vp, vp, vp, vp, vp]
     lib.bbdm_geglu_bwd.argtypes = [vp, vp, i64, i, vp, vp]
     lib.bbdm_attention_cross_bwd.argtypes = [vp, vp, vp, vp, i, i, i, i, i, vp, vp, vp, vp, vp]
+    lib.bbdm_attention_pad_heads.argtypes = [vp, i64, i, i, i, i, f, f, f, vp, vp, vp, vp]
+    lib.bbdm_attention_unpad_heads.argtypes = lib.bbdm_attention_pad_heads.argtypes
     lib.bbdm_optim_chunk_elems.argtypes = []
     lib.bbdm_adam_multi.argtypes = [vp, vp, vp, vp, vp, vp, i, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double,
                                      C.c_double, i64, vp, C.c_double, vp]
@@ -313,6 +334,9 @@ class CudaBackend:
     # heads wider than attn_max_head_dim run as two conv_umma GEMMs per (image, head) around softmax_rows_split, and
     # train through softmax_rows_split(grad=...), conv_umma and conv_wgrad (a backend without this attribute: not at all)
     attn_gemm_route = True
+    # heads up to attn_max_head_dim whose width is not a multiple of 8 run on the attention kernels at the width rounded
+    # up to 8, repacked by prep(heads=...) (a backend without this attribute: not at all)
+    attn_pad_heads = True
 
     def __init__(self):
         self.lib = load()
@@ -390,13 +414,39 @@ class CudaBackend:
 
     def prep(self, src1, src2, *, groups=32, mean=None, rstd=None, gamma=None, beta=None,
              film_scale=None, film_shift=None, film_stride=0, silu=True, resample=RESAMPLE_NONE,
-             act_f32=None, act_hi=None, act_lo=None, raw_f32=None, raw_hi=None, raw_lo=None):
+             act_f32=None, act_hi=None, act_lo=None, raw_f32=None, raw_hi=None, raw_lo=None, heads=None):
+        """heads: (n, scales, order) for the padded-head attention route -- the raw outputs then take src1's attention
+        heads re-laid to their own head width (bbdm_attention_pad_heads / _unpad_heads) instead of a plain copy.  src1
+        and the outputs hold len(scales) * n groups of columns, d wide on one side and d rounded up to 8 on the other;
+        columns past d are zero, and tensor t's groups are multiplied by scales[t] (order 0: the tensors of one head
+        together, the legacy qkv layout; order 1: all heads of one tensor together)."""
+        if heads is not None:
+            assert src2 is None and mean is None and act_f32 is None and act_hi is None and resample == RESAMPLE_NONE
+            self._repack_heads(src1, *heads, raw_f32, raw_hi, raw_lo)
+            return
         B, Hs, Ws, c1 = src1.shape
         a = PrepArgs(ptr(_req(src1)), c1, ptr(src2), 0 if src2 is None else src2.shape[3], B, Hs, Ws, groups,
                      ptr(mean), ptr(rstd), ptr(gamma), ptr(beta), ptr(film_scale), ptr(film_shift),
                      film_stride, int(silu), resample, ptr(act_f32), ptr(act_hi), ptr(act_lo),
                      ptr(raw_f32), ptr(raw_hi), ptr(raw_lo))
         check(self.lib.bbdm_prep_operand(C.byref(a), stream()))
+        LAUNCHES["n"] += 1
+
+    def _repack_heads(self, src, n, scales, order, out_f32, out_hi, out_lo):
+        tensors = len(scales)
+        out = out_f32 if out_f32 is not None else out_hi
+        ws, wo = src.shape[-1] // (tensors * n), out.shape[-1] // (tensors * n)
+        d, pad = min(ws, wo), wo >= ws
+        assert ws * tensors * n == src.shape[-1] and wo * tensors * n == out.shape[-1], (src.shape, out.shape, n, scales)
+        assert max(ws, wo) == pad_heads_width(d), (src.shape, out.shape)
+        rows = src.numel() // src.shape[-1]
+        for o, dt in ((out_f32, torch.float32), (out_hi, torch.bfloat16), (out_lo, torch.bfloat16)):
+            if o is not None:
+                assert o.numel() // o.shape[-1] == rows, (o.shape, src.shape)
+                _req(o, dt)
+        fn = self.lib.bbdm_attention_pad_heads if pad else self.lib.bbdm_attention_unpad_heads
+        s = [float(x) for x in scales] + [1.0] * (3 - tensors)
+        check(fn(ptr(_req(src)), rows, n, tensors, d, order, *s, ptr(out_f32), ptr(out_hi), ptr(out_lo), stream()))
         LAUNCHES["n"] += 1
 
     # -- convolutions --------------------------------------------------------------------------

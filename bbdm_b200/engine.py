@@ -390,6 +390,40 @@ class KernelExecutor:
         be.conv_umma(B=1, H=H, W=W, Cin=tkvp, Cout=d, taps=1, a_hi=p[0], a_lo=p[1], w_hi=vt[0], w_lo=vt[1],
                      out=out_f32, out_hi=out_hi, out_lo=out_lo, passes=self.passes)
 
+    def _attention_padded(self, pool, heads, d, srcs, order, planes, out_f32=None, out_hi=None, out_lo=None):
+        """Attention whose heads are d wide, d not a multiple of 8, on the kernels at dp = d rounded up to 8.  srcs:
+        (qkv,) fp32 [B, H, W, 3C] in the qkv order ``order``, or (q, kv) fp32 [B, H, W, C] and [B, Hc, Wc, 2C] for
+        cross-attention.  prep(heads=...) lays every head out dp wide (zeros past d) with (dp/d)^(1/4) folded into
+        q and k -- as split planes for the tensor-core kernels (planes) or fp32 for the fp32-qkv one -- the kernel runs
+        at dp, and prep(heads=...) writes the [B, H, W, C] output back d wide into out_f32 and/or out_hi / out_lo."""
+        be = self.be
+        B, H, W = srcs[0].shape[:3]
+        T, dp, c = H * W, cabi.pad_heads_width(d), cabi.pad_heads_scale(d)
+        cp = heads * dp
+        scales = ((c, c, 1.0),) if len(srcs) == 1 else ((c,), (c, 1.0))
+        bufs, ops = [], []            # the padded operands, and their [B, tokens, width] views the kernels take
+        for src, sc in zip(srcs, scales):
+            shape = src.shape[:3] + (len(sc) * cp,)
+            if planes:
+                t = pool.get(shape, torch.bfloat16), pool.get(shape, torch.bfloat16)
+                be.prep(src, None, raw_hi=t[0], raw_lo=t[1], heads=(heads, sc, order))
+            else:
+                t = (pool.get(shape),)
+                be.prep(src, None, raw_f32=t[0], heads=(heads, sc, order))
+            bufs += t
+            ops += [u.view(shape[0], -1, shape[3]) for u in t]
+        o = pool.get((B, H, W, cp))
+        if len(srcs) == 2:
+            be.attention_cross(*ops, heads, o.view(B, T, cp), None, None)
+        elif planes:
+            attn = be.attention_tc if dp in cabi.ATTN_TC_HEAD_DIMS else be.attention_split
+            attn(*ops, heads, order, o.view(B, T, cp), None, None)
+        else:
+            be.attention(*ops, heads, order, o.view(B, T, cp), None, None)
+        pool.put(*bufs)
+        be.prep(o, None, raw_f32=out_f32, raw_hi=out_hi, raw_lo=out_lo, heads=(heads, (1.0,), 0))
+        pool.put(o)
+
     def _geom(self, H, W):
         key = (H, W)
         r = self._geom_cache.get(key)
@@ -649,16 +683,24 @@ class UNetEngine(KernelExecutor):
             out = self._attention_heads_gemm(pool, name, heads, hd, (a_hi, a_lo), None, (B, H, W), x)
             pool.put(a_hi, a_lo)
             return out
-        if not head_dim_ok(hd):
+        pad = cabi.attn_pad_route(be, hd)
+        if not (head_dim_ok(hd) or pad):
             raise NotImplementedError(f"attention head_dim {hd}: the sm_90a kernels take {rule}")
         a_f32, a_hi, a_lo = self._gn_act(pool, x, m.norm, umma, silu=False)
-        # qkv 1x1: on the tensor-core path its epilogue writes the split planes the attention core reads
+        # qkv 1x1: on the tensor-core path its epilogue writes the split planes the attention core reads (fp32 for the
+        # padded-head route, which repacks it)
         qkv, q_hi, q_lo = self._conv(pool, eq, a_f32=a_f32, a_hi=a_hi, a_lo=a_lo, shape=(B, H, W),
-                                     out_split=umma, want_f32=not umma)
+                                     out_split=umma and not pad, want_f32=pad or not umma)
         pool.put(a_f32, a_hi, a_lo)
         o_f32 = o_hi = o_lo = None
         order = 1 if m.new_order else 0
-        if umma:
+        if pad:
+            if umma:
+                o_hi, o_lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
+            else:
+                o_f32 = pool.get(x.shape)
+            self._attention_padded(pool, heads, hd, (qkv,), order, umma, o_f32, o_hi, o_lo)
+        elif umma:
             o_hi, o_lo = pool.get(x.shape, torch.bfloat16), pool.get(x.shape, torch.bfloat16)
             # head_dim 64 (all templates) or 128: warp-specialised wgmma kernel; any other size (up to 256): the
             # mma.sync one
@@ -753,8 +795,8 @@ class UNetEngine(KernelExecutor):
         T, heads, d = H * W, m.n_heads, m.d_head
         inner = heads * d
         head_dim_ok, rule = cabi.attn_head_dims(be)
-        gemm = cabi.attn_gemm_route(be, d)
-        if not (head_dim_ok(d) or gemm):
+        gemm, pad = cabi.attn_gemm_route(be, d), cabi.attn_pad_route(be, d)
+        if not (head_dim_ok(d) or gemm or pad):
             raise NotImplementedError(f"SpatialTransformer head_dim {d}: the sm_90a attention kernels take {rule}")
         if not self._umma_ok(Cc, inner, W):
             raise NotImplementedError(f"SpatialTransformer: channel counts must be multiples of {self.conv_multiple} "
@@ -801,6 +843,28 @@ class UNetEngine(KernelExecutor):
                 h = self._attention_heads_gemm(pool, pre + ".attn2", heads, d, (n_hi, n_lo), ctx, (B, H, W), new,
                                                stats=False)
                 pool.put(n_hi, n_lo, new)
+                h = feed_forward(pre, blk, h)
+                continue
+            if pad:
+                # heads whose width is not a multiple of 8: the kernels at the width rounded up to 8, from fp32 q|k|v
+                qkv, _, _ = self._conv(pool, w[pre + ".attn1.qkv"], a_hi=n_hi, a_lo=n_lo, shape=(B, H, W))
+                pool.put(n_hi, n_lo)
+                o_hi, o_lo = pool.get(tok, bf), pool.get(tok, bf)
+                self._attention_padded(pool, heads, d, (qkv,), 1, True, out_hi=o_hi, out_lo=o_lo)
+                pool.put(qkv)
+                h = project_out(w[pre + ".attn1.to_out.0"], o_hi, o_lo, h)
+                n_hi, n_lo = layernorm(blk.norm2, h)
+                q, _, _ = self._conv(pool, w[pre + ".attn2.to_q"], a_hi=n_hi, a_lo=n_lo, shape=(B, H, W))
+                ekv = w[pre + ".attn2.to_kv"]
+                if ctx is None:
+                    kv, _, _ = self._conv(pool, ekv, a_hi=n_hi, a_lo=n_lo, shape=(B, H, W))
+                else:
+                    kv, _, _ = self._conv(pool, ekv, a_f32=ctx, shape=tuple(ctx.shape[:3]))
+                pool.put(n_hi, n_lo)
+                o_hi, o_lo = pool.get(tok, bf), pool.get(tok, bf)
+                self._attention_padded(pool, heads, d, (q, kv), 1, True, out_hi=o_hi, out_lo=o_lo)
+                pool.put(q, kv)
+                h = project_out(w[pre + ".attn2.to_out.0"], o_hi, o_lo, h)
                 h = feed_forward(pre, blk, h)
                 continue
             _, q_hi, q_lo = self._conv(pool, w[pre + ".attn1.qkv"], a_hi=n_hi, a_lo=n_lo, shape=(B, H, W), out_split=True,

@@ -717,34 +717,68 @@ def _qkv_heads(t, heads, order):
     return v[:, :, 0], v[:, :, 1], v[:, :, 2]
 
 
+def _pad_heads(be, t, heads, scales, order, planes=False):
+    """fp32 [..., G*dp] copy of an fp32 NHWC tensor t [..., G*d] on the padded-head route (prep(heads=...): each
+    head's columns zero-filled from d to dp = d rounded up to 8, tensor i of len(scales) scaled by scales[i]), and with
+    planes also its split planes; returns (fp32, hi, lo)."""
+    d = t.shape[-1] // (len(scales) * heads)
+    shape = t.shape[:-1] + (len(scales) * heads * cabi.pad_heads_width(d),)
+    f = torch.empty(shape, dtype=torch.float32, device=t.device)
+    hi = lo = None
+    if planes:
+        hi, lo = torch.empty(shape, dtype=torch.bfloat16, device=t.device), torch.empty(shape, dtype=torch.bfloat16, device=t.device)
+    be.prep(t, None, raw_f32=f, raw_hi=hi, raw_lo=lo, heads=(heads, scales, order))
+    return f, hi, lo
+
+
+def _unpad_heads(be, t, heads, scales, order, d):
+    """fp32 [..., G*d] of a padded [..., G*dp] tensor (prep(heads=...)), tensor i scaled by scales[i]."""
+    out = torch.empty(t.shape[:-1] + (len(scales) * heads * d,), dtype=torch.float32, device=t.device)
+    be.prep(t, None, raw_f32=out, heads=(heads, scales, order))
+    return out
+
+
 class AttentionCoreFn(torch.autograd.Function):
     """softmax((q s)(k s)^T) v per head (QKVAttentionLegacy / QKVAttention, openaimodel.py:350-413) on a
     [B,3C,H,W] qkv tensor -> [B,C,H,W].  Forward: the sampling path's attention kernels (wgmma for
     head_dim 64 and 128, the fp32-qkv mma.sync kernel for the other multiples of 8 up to the backend's
-    attn_max_head_dim, 256 on CudaBackend); backward:
-    bbdm_attention_bwd (flash-style recompute, exact fp32) -- the T x T matrix is never stored, which also replaces
-    the reference's checkpoint() around the block (openaimodel.py:318)."""
+    attn_max_head_dim, 256 on CudaBackend; a width d that is not a multiple of 8 runs at d rounded up to 8 with the
+    heads repacked, _pad_heads); backward: bbdm_attention_bwd (flash-style recompute, exact fp32) -- the T x T matrix
+    is never stored, which also replaces the reference's checkpoint() around the block (openaimodel.py:318)."""
 
     @staticmethod
     def forward(ctx, qkv, heads, order):
         be = backend()
         B, C3, H, W = qkv.shape
         Cc, T = C3 // 3, H * W
+        d = Cc // heads
         dev = qkv.device
         qn = _nhwc(qkv.detach()).contiguous()
-        if cabi.attn_gemm_route(be, Cc // heads):
+        ctx.heads, ctx.order = heads, order
+        ctx.pad = cabi.attn_pad_route(be, d)
+        if cabi.attn_gemm_route(be, d):
             out = _gemm_heads(be, *_qkv_heads(qn, heads, order), (H, W)).view(B, T, Cc)
-        elif Cc // heads in cabi.ATTN_TC_HEAD_DIMS:
-            out = torch.empty((B, T, Cc), dtype=torch.float32, device=dev)
-            q_hi = torch.empty((B, H, W, C3), dtype=torch.bfloat16, device=dev)
-            q_lo = torch.empty_like(q_hi)
-            be.prep(qn, None, raw_hi=q_hi, raw_lo=q_lo)
+            ctx.save_for_backward(qn, out)
+            return out.view(B, H, W, Cc).permute(0, 3, 1, 2)
+        q_hi = q_lo = None
+        dk = cabi.pad_heads_width(d) if ctx.pad else d           # the head width the kernels run
+        if ctx.pad:
+            # q and k scaled by (dp/d)^(1/4): the kernels' dp^-1/4 pre-scaling then gives the reference's d^-1/2
+            c = cabi.pad_heads_scale(d)
+            qn, q_hi, q_lo = _pad_heads(be, qn, heads, (c, c, 1.0), order, planes=dk in cabi.ATTN_TC_HEAD_DIMS)
+            C3 = qn.shape[-1]
+        out = torch.empty((B, T, C3 // 3), dtype=torch.float32, device=dev)
+        if dk in cabi.ATTN_TC_HEAD_DIMS:
+            if q_hi is None:
+                q_hi = torch.empty((B, H, W, C3), dtype=torch.bfloat16, device=dev)
+                q_lo = torch.empty_like(q_hi)
+                be.prep(qn, None, raw_hi=q_hi, raw_lo=q_lo)
             be.attention_tc(q_hi.view(B, T, C3), q_lo.view(B, T, C3), heads, order, out, None, None)
         else:
-            out = torch.empty((B, T, Cc), dtype=torch.float32, device=dev)
             be.attention(qn.view(B, T, C3), heads, order, out, None, None)
         ctx.save_for_backward(qn, out)
-        ctx.heads, ctx.order = heads, order
+        if ctx.pad:
+            out = _unpad_heads(be, out, heads, (1.0,), 0, d)
         return out.view(B, H, W, Cc).permute(0, 3, 1, 2)
 
     @staticmethod
@@ -755,15 +789,22 @@ class AttentionCoreFn(torch.autograd.Function):
         T = H * W
         dev = dout.device
         don = _nhwc(dout).contiguous()
-        dqkv = torch.empty_like(qn)
         if cabi.attn_gemm_route(be, C3 // 3 // ctx.heads):
+            dqkv = torch.empty_like(qn)
             _gemm_heads(be, *_qkv_heads(qn, ctx.heads, ctx.order), (H, W), dout=don.view(B, T, ctx.heads, -1),
                         grads=_qkv_heads(dqkv, ctx.heads, ctx.order))
             return dqkv.permute(0, 3, 1, 2), None, None
+        if ctx.pad:       # qn and out are the padded forward's; dout comes compact
+            don = _pad_heads(be, don, ctx.heads, (1.0,), 0)[0]
+        dqkv = torch.empty_like(qn)
         lse = torch.empty((B * ctx.heads * T,), dtype=torch.float32, device=dev)
         delta = torch.empty_like(lse)
         be.attention_bwd(qn.view(B, T, C3), out, don.view(B, T, C3 // 3), ctx.heads, ctx.order,
                          dqkv.view(B, T, C3), lse, delta)
+        if ctx.pad:       # d(c q) / dq = c: dq = c dq', dk = c dk', dv unchanged
+            d = dout.shape[1] // ctx.heads
+            c = cabi.pad_heads_scale(d)
+            dqkv = _unpad_heads(be, dqkv, ctx.heads, (c, c, 1.0), ctx.order, d)
         return dqkv.permute(0, 3, 1, 2), None, None
 
 
@@ -772,7 +813,8 @@ def attention_core(qkv4: torch.Tensor, heads: int, new_order: bool, enabled: boo
     B, C3, H, W = qkv4.shape
     hd = C3 // 3 // heads
     if not (enabled and _on_device(qkv4) and qkv4.dtype == torch.float32
-            and (cabi.attn_head_dims(backend())[0](hd) or (cabi.attn_gemm_route(backend(), hd) and W >= 4))
+            and (cabi.attn_head_dims(backend())[0](hd) or cabi.attn_pad_route(backend(), hd)
+                 or (cabi.attn_gemm_route(backend(), hd) and W >= 4))
             and (C3 // 3) % 4 == 0 and B * heads <= 65535):
         return None
     return AttentionCoreFn.apply(qkv4, heads, 1 if new_order else 0)
@@ -858,7 +900,8 @@ class CrossAttentionCoreFn(torch.autograd.Function):
     """softmax(q k^T D^-1/2) v per head (CrossAttention, attention.py:166-192) for queries q [B, C, H, W] and keys|values
     kv [B, 2C, Hc, Wc] (k = channels [0, C), v = [C, 2C)) -> [B, C, H, W].  Forward: bbdm_attention_cross; backward:
     bbdm_attention_cross_bwd (flash-style recompute, exact fp32): no Tq x Tkv tensor is stored, which also replaces
-    the reference's checkpoint() around the transformer block."""
+    the reference's checkpoint() around the transformer block.  A head width d that is not a multiple of 8 runs at d
+    rounded up to 8 with the heads repacked (_pad_heads)."""
 
     @staticmethod
     def forward(ctx, q, kv, heads):
@@ -873,18 +916,28 @@ class CrossAttentionCoreFn(torch.autograd.Function):
             out = _gemm_heads(be, qn.view(B, Tq, heads, -1), kv5[:, :, 0], kv5[:, :, 1], (H, W)).view(B, Tq, Cc)
             ctx.save_for_backward(qn, kvn, out)
             return out.view(B, H, W, Cc).permute(0, 3, 1, 2)
-        planes = []
-        for t in (qn, kvn):
-            hi = torch.empty(t.shape, dtype=torch.bfloat16, device=dev)
-            lo = torch.empty_like(hi)
-            be.prep(t, None, raw_hi=hi, raw_lo=lo)
-            planes += [hi, lo]
-        q_hi, q_lo, kv_hi, kv_lo = planes
-        out = torch.empty((B, Tq, Cc), dtype=torch.float32, device=dev)
-        be.attention_cross(q_hi.view(B, Tq, Cc), q_lo.view(B, Tq, Cc), kv_hi.view(B, Tkv, 2 * Cc),
-                           kv_lo.view(B, Tkv, 2 * Cc), heads, out_f32=out)
+        d = Cc // heads
+        ctx.pad = cabi.attn_pad_route(be, d)
+        if ctx.pad:
+            # heads at d rounded up to 8, q and k scaled by (dp/d)^(1/4): the kernel's dp^-1/2 becomes d^-1/2
+            c = cabi.pad_heads_scale(d)
+            qn, q_hi, q_lo = _pad_heads(be, qn, heads, (c,), 1, planes=True)
+            kvn, kv_hi, kv_lo = _pad_heads(be, kvn, heads, (c, 1.0), 1, planes=True)
+        else:
+            planes = []
+            for t in (qn, kvn):
+                hi = torch.empty(t.shape, dtype=torch.bfloat16, device=dev)
+                lo = torch.empty_like(hi)
+                be.prep(t, None, raw_hi=hi, raw_lo=lo)
+                planes += [hi, lo]
+            q_hi, q_lo, kv_hi, kv_lo = planes
+        Ck = qn.shape[-1]
+        out = torch.empty((B, Tq, Ck), dtype=torch.float32, device=dev)
+        be.attention_cross(q_hi.view(B, Tq, Ck), q_lo.view(B, Tq, Ck), kv_hi.view(B, Tkv, 2 * Ck),
+                           kv_lo.view(B, Tkv, 2 * Ck), heads, out_f32=out)
         ctx.save_for_backward(qn, kvn, out)
-        ctx.heads = heads
+        if ctx.pad:
+            out = _unpad_heads(be, out, heads, (1.0,), 0, d)
         return out.view(B, H, W, Cc).permute(0, 3, 1, 2)
 
     @staticmethod
@@ -902,10 +955,17 @@ class CrossAttentionCoreFn(torch.autograd.Function):
                         dout=don.view(B, Tq, ctx.heads, -1), grads=(dq.view(B, Tq, ctx.heads, -1), dkv5[:, :, 0],
                                                                     dkv5[:, :, 1]))
             return dq.permute(0, 3, 1, 2), dkv.permute(0, 3, 1, 2), None
+        if ctx.pad:       # qn, kvn and out are the padded forward's; dout comes compact
+            don = _pad_heads(be, don, ctx.heads, (1.0,), 0)[0]
         lse = torch.empty((B * ctx.heads * Tq,), dtype=torch.float32, device=dev)
         delta = torch.empty_like(lse)
         be.attention_cross_bwd(qn.view(B, Tq, Cc), kvn.view(B, Tkv, 2 * Cc), out, don.view(B, Tq, Cc), ctx.heads,
                                dq.view(B, Tq, Cc), dkv.view(B, Tkv, 2 * Cc), lse, delta)
+        if ctx.pad:       # dq = c dq', dk = c dk', dv unchanged
+            d = dout.shape[1] // ctx.heads
+            c = cabi.pad_heads_scale(d)
+            dq = _unpad_heads(be, dq, ctx.heads, (c,), 0, d)
+            dkv = _unpad_heads(be, dkv, ctx.heads, (c, 1.0), 1, d)
         return dq.permute(0, 3, 1, 2), dkv.permute(0, 3, 1, 2), None
 
 

@@ -141,12 +141,14 @@ class SpatialTransformer(nn.Module):
     def _native_ok(self, x, context):
         """Shapes the training Functions' kernels take: tensor-core GEMM channel counts (proj_in's, in_channels ->
         inner, at the backend's channel multiple) and token grid, GroupNorm over 32 groups, LayerNorm width, attention
-        head size (or a backend with the GEMM route for heads wider than its attention kernels take), a few-channel
-        fp32 context; no active dropout."""
+        head size (or a backend with the padded-head route for widths that are not a multiple of 8, or the GEMM route
+        for heads wider than its attention kernels take), a few-channel fp32 context; no active dropout."""
         inner = self.n_heads * self.d_head
+        be = train.backend()
         ok = (train.native_ok(self.proj_in, x) and self.in_channels % 32 == 0 and self.in_channels <= 4096
-              and inner <= cabi.LN_MAX_C and (cabi.attn_head_dims(train.backend())[0](self.d_head)
-                                              or cabi.attn_gemm_route(train.backend(), self.d_head))
+              and inner <= cabi.LN_MAX_C and (cabi.attn_head_dims(be)[0](self.d_head)
+                                              or cabi.attn_pad_route(be, self.d_head)
+                                              or cabi.attn_gemm_route(be, self.d_head))
               and x.shape[0] * self.n_heads <= 65535
               and not (self.training and any(m.p > 0 for m in self.modules() if isinstance(m, nn.Dropout))))
         if context is not None:

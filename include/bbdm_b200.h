@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define BBDM_ABI_VERSION 10
+#define BBDM_ABI_VERSION 11
 
 enum {
   BBDM_OK = 0,
@@ -545,6 +545,21 @@ int bbdm_attention_tc(const void* qkv_hi, const void* qkv_lo, int B, int T, int 
  * deterministic. */
 int bbdm_attention_bwd(const float* qkv, const float* out, const float* dout, int B, int T, int C, int heads,
                        int order, float* dqkv, float* lse, float* delta, void* stream);
+
+/* Repack of attention heads whose width d is not a multiple of 8, so that the kernels above run them at
+ * dp = d rounded up to 8.  A row holds G = tensors * heads groups of d columns (one head's q, k or v): order 0 puts
+ * the tensors of a head together (the legacy qkv layout), order 1 all heads of one tensor together (q, k|v, dout).
+ * Every value of a group is multiplied by its tensor's scale (scale0..2; the caller folds (dp/d)^(1/4) into q and k,
+ * so the kernels' dp^-1/2 softmax scale becomes d^-1/2), with one fp32 rounding.
+ *   pad:   src [rows, G*d] fp32 -> [rows, G*dp], zeros in columns d..dp-1 of every group; out_f32 16-byte aligned,
+ *          the planes 8-byte aligned.
+ *   unpad: src [rows, G*dp] fp32 -> [rows, G*d].
+ * out: fp32 and/or split-bf16 planes (hi = bf16(x), lo = bf16(x - hi), as bbdm_prep_operand splits).  tensors 1..3.
+ * No host synchronisation or allocation (capturable). */
+int bbdm_attention_pad_heads(const float* src, int64_t rows, int heads, int tensors, int d, int order, float scale0,
+                             float scale1, float scale2, float* out_f32, void* out_hi, void* out_lo, void* stream);
+int bbdm_attention_unpad_heads(const float* src, int64_t rows, int heads, int tensors, int d, int order, float scale0,
+                               float scale1, float scale2, float* out_f32, void* out_hi, void* out_lo, void* stream);
 
 /* ---- VQGAN ends of the latent models ---------------------------------------
  * Row softmax of a [rows, cols] fp32 score matrix, p = softmax(scale * s), written as split-bf16 planes
